@@ -181,7 +181,9 @@ CG_API int cg_merkle_root(const uint8_t *bytes, const uint64_t *offsets, uint64_
 CG_API int cg_merkle_root_fixed(const uint8_t *bytes, uint64_t leaf_len, uint64_t n, uint8_t out_root[32]);
 /* device-resident: fixed-size leaves in HBM -> roots of consecutive 2^block_log2-leaf blocks
  * (d_out_roots[ceil(n / 2^block_log2)][32], device memory).  Shards call this, all-gather the
- * block roots (the one collective on this path) and finish with cg_merkle_fold. */
+ * block roots (the one collective on this path) and finish with cg_merkle_fold.
+ * block_log2 must be at most 40 (as for cg_merkle_root_sharded_device): larger values return
+ * CG_ERR_INVALID_ARG before any buffer is touched. */
 CG_API int cg_merkle_block_roots_device(const void *d_bytes, uint64_t leaf_len, uint64_t n, uint32_t block_log2,
                                         void *d_out_roots, void *stream);
 /* fold m 32-byte subtree roots (host memory) into one root with the same level-wise rule */

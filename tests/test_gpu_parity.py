@@ -72,12 +72,18 @@ def test_reference_vectors_through_the_kernels(N, oracle):
         rs.close()
 
 
-@pytest.mark.parametrize("n_rules,stride", [(17, 0), (17, 2), (64, 0), (120, 2), (500, 0), (500, 2), (2000, 0), (5000, 0)])
+@pytest.mark.parametrize("n_rules,stride", [(17, 0), (17, 2), (64, 0), (120, 2), (120, 4), (500, 0), (500, 2), (2000, 0), (5000, 0)])
 def test_policy_scan_equals_oracle(N, oracle, n_rules, stride):
-    """stride 0 = the compiler's choice (17 built-ins: 4; larger sets: 2; 2000 / 5000 rules: level-1b tables in HBM)"""
+    """stride 0 = the compiler's choice (17 built-ins: 4; larger sets: 2; 2000 / 5000 rules: level-1b tables in HBM);
+    stride 4 forced on a synthetic set turns the factors no gram covers at four alignments into trigger bytes or
+    always-candidate rules (spans checked too)"""
     rl = W.make_rules(n_rules)
     rules = W.rules_as_tuples(rl)
     rs = N.Ruleset(rules, options=stride, strict=True)
+    info = rs.info()
+    assert stride == 0 or info.stride == stride
+    if stride == 4:
+        assert info.n_triggers + info.n_always_candidate >= 1
     n = 6000 if n_rules <= 2000 else 2500
     data_t, off_t, inj = W.make_messages(n, 256, rl, p_hit=0.05, seed=4242 + n_rules)
     data = data_t.numpy()
@@ -87,6 +93,9 @@ def test_policy_scan_equals_oracle(N, oracle, n_rules, stride):
     assert [(int(h["msg"]), int(h["rule"])) for h in hits] == ehits
     assert np.array_equal(words, ewords)
     assert len(ehits) >= len(inj)          # every injected token is a true hit
+    if stride == 4:
+        got = [(int(s["msg"]), int(s["rule"]), int(s["start16"]), int(s["end16"])) for s in rs.find_matches_batch(data, off)]
+        assert got == oracle_spans(oracle, rules, data, off)
     rs.close()
 
 

@@ -961,6 +961,8 @@ int cg_merkle_root_fixed(const uint8_t* bytes, uint64_t leaf_len, uint64_t n, ui
 int cg_merkle_block_roots_device(const void* d_bytes, uint64_t leaf_len, uint64_t n, uint32_t block_log2, void* d_out_roots, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  // (beyond 2^40 leaves per block the block count below would need a shift of 64 or more: undefined, and it sizes the copy)
+  if (block_log2 > 40) return fail(CG_ERR_INVALID_ARG, "block_log2 must be at most 40");
   if (!n) return CG_OK;
   if (!d_bytes || !d_out_roots) return fail(CG_ERR_INVALID_ARG, "null argument");
   int rc;
