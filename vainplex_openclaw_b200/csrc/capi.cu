@@ -34,7 +34,6 @@ struct Ctx {
   uint32_t prof_pieces = 0;
   bool profiling = false;
   cg_stats stats{};
-  uint64_t launches = 0;
   // grow-only staging in HBM
   uint8_t* d_bytes = nullptr; size_t cap_bytes = 0; uint8_t* d_bytes_raw = nullptr;   // d_bytes = d_bytes_raw + 256: readable in front (sha_words)
   uint32_t* d_off32 = nullptr; size_t cap_off32 = 0;
@@ -55,6 +54,7 @@ int cuda_fail(cudaError_t e, const char* what) {
   return CG_ERR_CUDA;
 }
 #define CU(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) return cuda_fail(_e, #x); } while (0)
+void count_launches(int k) { G.stats.kernel_launches += k; }
 
 template <typename T>
 int grow(T** p, size_t* cap, size_t need_elems) {
@@ -95,18 +95,19 @@ struct cg_ruleset {
   // that batch marked incomplete by finalize_kernel) is seen by the next call / by cg_scan_join and the scratch grows
   static constexpr int kMirror = 16;
   uint32_t* h_counters = nullptr; cudaEvent_t e_cnt[kMirror] = {}; bool cnt_pending[kMirror] = {};
-  uint32_t grow_l1 = 0, grow_slot = 0, grow_ev = 0;     // capacities learnt from overflows
+  uint32_t grow_l1 = 0, grow_slot = 0, grow_ev = 0, grow_span = 0;     // capacities learnt from overflows
   uint32_t sticky_flags = 0;      // error flags of batches since the last cg_scan_join
   // verify_small_kernel's grid (CTAs per SM): one while the island matcher decides (nearly) everything, four once a step has
   // sent more than 2048 pairs to the VM (non-ASCII traffic); back to one below 256.  Part of the cached graphs' keys.
   int verify_ctas = 1;
   void size_verify_grid() { const uint32_t ev = last_counters[1]; if (ev > 2048u) verify_ctas = 4; else if (ev < 256u) verify_ctas = 1; }
   uint32_t last_counters[kCounterWords] = {};
-  // the device-resident step replayed as one CUDA graph (keyed on its arguments and scratch capacities)
-  struct CachedGraph { int kernels = 0; cudaGraphExec_t exec = nullptr; const void* bytes = nullptr; const void* off = nullptr; void* words = nullptr; uint32_t n = 0; uint64_t caps[4] = {0, 0, 0, 0}; uint64_t used = 0; };
+  uint64_t scratch_gen = 0;       // advanced by every change to what a captured step holds (scratch buffers, DevRuleset)
+  // the device-resident step replayed as one CUDA graph (keyed on its arguments, the scratch generation and the verify grid)
+  struct CachedGraph { int kernels = 0; cudaGraphExec_t exec = nullptr; const void* bytes = nullptr; const void* off = nullptr; void* words = nullptr; uint32_t n = 0; uint64_t gen = 0; int ctas = 0; uint64_t used = 0; };
   // cg_scan_one: pinned staging + one device block ([offsets][message bytes] in, [word][counters][hit row] out) and the
   // step as a graph over those fixed addresses (the message length is data, so one graph serves every message)
-  struct OnePath { cudaGraphExec_t exec = nullptr; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint64_t caps[4] = {0, 0, 0, 0}; int kernels = 0; } one;
+  struct OnePath { cudaGraphExec_t exec = nullptr; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint64_t gen = 0; int ctas = 0; int kernels = 0; } one;
   CachedGraph graphs[2];          // two entries: callers that alternate between two input/output buffer sets replay, never re-capture
   uint64_t graph_clock = 0;
   ~cg_ruleset() {
@@ -137,6 +138,7 @@ int upload(cg_ruleset* rs, const std::vector<T>& v, const T** out, size_t pad_el
 }
 
 int ensure_work(cg_ruleset* rs, ScanWork& w, uint32_t n_msgs, uint32_t l1_cap, uint32_t slot_cap, uint32_t event_cap, uint32_t span_cap) {
+  rs->scratch_gen++;                                        // (prepare_step calls this only when some buffer must grow)
   if (!w.counters) { CU(cudaMalloc((void**)&w.counters, kCounterWords * sizeof(uint32_t))); CU(cudaMalloc((void**)&w.persist, 16)); CU(cudaMemset(w.persist, 0, 16)); CU(cudaDeviceSynchronize()); }
   if (n_msgs > w.msg_cap) { cudaFree(w.slot_of_msg); w.slot_of_msg = nullptr; w.msg_cap = 0; CU(cudaMalloc((void**)&w.slot_of_msg, (size_t)n_msgs * 4)); w.msg_cap = n_msgs; }
   if (l1_cap > w.l1_cap) {
@@ -186,18 +188,31 @@ int run_scan_device(cg_ruleset* rs, const uint8_t* d_bytes, const uint32_t* d_of
   if (G.profiling) cudaEventRecord(G.pev[3], st);
   k += launch_finalize(rs->dev, w, d_words, n, G.sm_count, st);
   if (G.profiling) cudaEventRecord(G.pev[4], st);
-  G.launches += k; G.stats.kernel_launches += k;
+  count_launches(k);
   CU(cudaGetLastError());
   return CG_OK;
 }
 
 void prepare_kernels() { static bool done = false; if (!done) { prepare_scan_kernels(); done = true; } }
 
-// capacities a batch of n messages starts with (confirmed occurrences are rare: about one per hundred messages on chat text)
-void default_caps(const cg_ruleset* rs, uint32_t n, uint32_t* l1, uint32_t* slot, uint32_t* ev) {
+// capacities a batch of n messages starts with (confirmed occurrences are rare: about one per hundred messages on chat text;
+// a step without spans writes none)
+void default_caps(const cg_ruleset* rs, uint32_t n, bool spans, uint32_t* l1, uint32_t* slot, uint32_t* ev, uint32_t* span) {
   *l1 = std::max(std::max<uint32_t>(std::max<uint32_t>(2 * n, 1u << 16), rs->work.l1_cap), rs->grow_l1);
   *slot = std::max(std::max<uint32_t>(std::max<uint32_t>(n / 4, 4096), rs->work.slot_cap), rs->grow_slot);
   *ev = std::max(std::max<uint32_t>(std::max<uint32_t>(n, 4096), rs->work.event_cap), rs->grow_ev);
+  *span = spans ? std::max(std::max<uint32_t>(std::max<uint32_t>(n, 4096), rs->work.span_cap), rs->grow_span) : 1;
+}
+// the verify grid and the scratch of a step over n messages; growing waits for st (nothing may still use a replaced buffer)
+int prepare_step(cg_ruleset* rs, uint32_t n, bool spans, cudaStream_t st) {
+  rs->size_verify_grid();
+  const ScanWork& w = rs->work;
+  uint32_t l1, slot, ev, span;
+  default_caps(rs, n, spans, &l1, &slot, &ev, &span);
+  n = std::max<uint32_t>(n, 1);
+  if (n <= w.msg_cap && l1 <= w.l1_cap && slot <= w.slot_cap && ev <= w.event_cap && span <= w.span_cap) return CG_OK;
+  CU(cudaStreamSynchronize(st));
+  return ensure_work(rs, rs->work, n, l1, slot, ev, span);
 }
 // fq is cut into four equal pieces at most: the fullest piece decides
 static uint32_t queue_need(const uint32_t* hc) { uint32_t m = 0; for (int i = 24; i < 28; i++) m = std::max(m, hc[i]); return m > 0xffffffffu / scan_pieces() ? 0xffffffffu : scan_pieces() * m; }
@@ -207,6 +222,39 @@ void learn_caps(cg_ruleset* rs, const uint32_t* hc) {
   if (flags & ERR_L1_OVERFLOW) { const uint32_t need = std::max(hc[4], queue_need(hc)); rs->grow_l1 = std::max<uint32_t>(rs->grow_l1, std::max<uint32_t>(2 * need, need + 65536)); }
   if (flags & ERR_SLOT_OVERFLOW) rs->grow_slot = std::max<uint32_t>(rs->grow_slot, std::max<uint32_t>(2 * hc[0], hc[0] + 4096));
   if (flags & ERR_EVENT_OVERFLOW) rs->grow_ev = std::max<uint32_t>(rs->grow_ev, std::max<uint32_t>(2 * hc[1], hc[1] + 4096));
+  if (flags & ERR_SPAN_OVERFLOW) rs->grow_span = std::max<uint32_t>(rs->grow_span, std::max<uint32_t>(2 * hc[2], hc[2] + 4096));
+}
+const char* const kVmOverflow = "matcher thread list / stack overflow on device";
+// a finished step's counter block -> CG_OK, CG_ERR_TOO_LARGE, or 1 = a queue overflowed (the capacities the step needs
+// have been learnt)
+int absorb_counters(cg_ruleset* rs, const uint32_t* hc) {
+  memcpy(rs->last_counters, hc, sizeof rs->last_counters);
+  if (hc[3] & (ERR_VM_STACK | ERR_VM_LIST)) return fail(CG_ERR_TOO_LARGE, kVmOverflow);
+  if (hc[3]) learn_caps(rs, hc);
+  return hc[3] ? 1 : CG_OK;
+}
+// the kernels enqueue() puts on st, captured as one graph; they are counted each time the graph is launched, not here
+template <typename Enqueue>
+int capture(cudaStream_t st, Enqueue&& enqueue, cudaGraphExec_t* exec, int* kernels) {
+  cudaGraph_t g = nullptr;
+  const uint64_t before = G.stats.kernel_launches;
+  CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  const int rc = enqueue();
+  cudaError_t e = cudaStreamEndCapture(st, &g);
+  *kernels = (int)(G.stats.kernel_launches - before); G.stats.kernel_launches = before;
+  if (rc != CG_OK || e != cudaSuccess) { if (g) cudaGraphDestroy(g); cudaGetLastError(); return rc != CG_OK ? rc : cuda_fail(e, "cudaStreamEndCapture"); }
+  e = cudaGraphInstantiate(exec, g, 0);
+  cudaGraphDestroy(g);
+  if (e != cudaSuccess) { *exec = nullptr; return cuda_fail(e, "cudaGraphInstantiate"); }
+  return CG_OK;
+}
+// the rules of one hit row (rw words), lowest first: put(i, rule) for the i-th rule of the output while i < cap; returns nh
+// plus the number of rules in the row
+template <typename Put>
+uint32_t append_hit_row(const uint32_t* row, uint32_t rw, uint32_t nh, uint32_t cap, Put&& put) {
+  for (uint32_t k = 0; k < rw; k++)
+    for (uint32_t v = row[k]; v; v &= v - 1, nh++) if (nh < cap) put(nh, k * 32 + (uint32_t)__builtin_ctz(v));
+  return nh;
 }
 
 struct HostScan {
@@ -224,7 +272,6 @@ int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uin
   if (!rs || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
   int rc;
   if (n && (rc = check_offsets(offsets, n))) return rc;
-  rs->size_verify_grid();
   const size_t first = n ? offsets[0] : 0, total = n ? offsets[n] : 0;
   if ((rc = grow_bytes(total + 64))) return rc;
   if ((rc = grow(&G.d_off32, &G.cap_off32, (size_t)n + 1))) return rc;
@@ -235,30 +282,32 @@ int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uin
     CU(cudaMemsetAsync(G.d_bytes + total, 0, 64, st));
     CU(cudaMemcpyAsync(G.d_off32, offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
   }
-  uint32_t l1_cap, slot_cap, event_cap, span_cap = spans ? std::max<uint32_t>(std::max<uint32_t>(n, 4096), rs->work.span_cap) : 1;
-  default_caps(rs, n, &l1_cap, &slot_cap, &event_cap);
   hs->counters.assign(kCounterWords, 0);
   for (int attempt = 0; attempt < 10; attempt++) {
-    if ((rc = ensure_work(rs, rs->work, std::max<uint32_t>(n, 1), l1_cap, slot_cap, event_cap, span_cap))) return rc;
+    if ((rc = prepare_step(rs, n, spans, st))) return rc;
     CU(cudaEventRecord(G.ev0, st));
     if (n) { if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32, n, G.d_words, spans, st))) return rc; }
     else CU(cudaMemsetAsync(rs->work.counters, 0, kCounterWords * sizeof(uint32_t), st));
     CU(cudaEventRecord(G.ev1, st));
     CU(cudaMemcpyAsync(hs->counters.data(), rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    memcpy(rs->last_counters, hs->counters.data(), sizeof rs->last_counters);
     float ms = 0; cudaEventElapsedTime(&ms, G.ev0, G.ev1); G.stats.last_scan_ms = ms;
-    uint32_t flags = hs->counters[3];
-    if (flags & (ERR_VM_STACK | ERR_VM_LIST)) return fail(CG_ERR_TOO_LARGE, "matcher thread list / stack overflow on device");
-    if (flags & ERR_L1_OVERFLOW) { l1_cap = std::max<uint32_t>(l1_cap * 2, std::max(hs->counters[4], queue_need(hs->counters.data())) + 1024); continue; }
-    if (flags & ERR_SLOT_OVERFLOW) { slot_cap = std::max<uint32_t>(slot_cap * 4, hs->counters[0] + 1024); continue; }
-    if (flags & ERR_EVENT_OVERFLOW) { event_cap = std::max<uint32_t>(event_cap * 4, hs->counters[1] + 1024); continue; }
-    if (flags & ERR_SPAN_OVERFLOW) { span_cap = std::max<uint32_t>(span_cap * 4, hs->counters[2] + 1024); continue; }
+    if ((rc = absorb_counters(rs, hs->counters.data())) == 1) continue;
+    if (rc) return rc;
     G.stats.messages_scanned += n; G.stats.bytes_scanned += total - first;
     G.stats.candidate_events += hs->counters[1]; G.stats.verified_pairs += hs->counters[1];
     return CG_OK;
   }
   return fail(CG_ERR_CAPACITY, "candidate queues kept overflowing");
+}
+
+int ensure_copy_streams() {
+  if (G.s_h2d) return CG_OK;
+  const int C = Ctx::kChunks;
+  CU(cudaStreamCreateWithFlags(&G.s_h2d, cudaStreamNonBlocking)); CU(cudaStreamCreateWithFlags(&G.s_d2h, cudaStreamNonBlocking));
+  for (int c = 0; c < C; c++) { CU(cudaEventCreateWithFlags(&G.e_h2d[c], cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&G.e_done[c], cudaEventDisableTiming)); }
+  CU(cudaMallocHost((void**)&G.h_chunk_counters, (size_t)C * kCounterWords * 4));
+  return CG_OK;
 }
 
 // Words-only scan of a large host batch in kChunks pieces: the H2D copy of piece c+1 and the D2H copy of piece c-1 run
@@ -268,22 +317,15 @@ int scan_host_chunked(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offs
   const int C = Ctx::kChunks;
   int rc;
   if ((rc = check_offsets(offsets, n))) return rc;
-  rs->size_verify_grid();
   const size_t total = offsets[n];
   if ((rc = grow_bytes(total + 64))) return rc;
   if ((rc = grow(&G.d_off32, &G.cap_off32, (size_t)n + 1))) return rc;
   if ((rc = grow(&G.d_words, &G.cap_words, (size_t)n + 1))) return rc;
-  if (!G.s_h2d) {
-    CU(cudaStreamCreateWithFlags(&G.s_h2d, cudaStreamNonBlocking)); CU(cudaStreamCreateWithFlags(&G.s_d2h, cudaStreamNonBlocking));
-    for (int c = 0; c < C; c++) { CU(cudaEventCreateWithFlags(&G.e_h2d[c], cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&G.e_done[c], cudaEventDisableTiming)); }
-    CU(cudaMallocHost((void**)&G.h_chunk_counters, (size_t)C * kCounterWords * 4));
-  }
+  if ((rc = ensure_copy_streams())) return rc;
   cudaStream_t st = G.stream;
   const uint32_t per = (n + C - 1) / C;
-  uint32_t l1_cap, slot_cap, event_cap;
-  default_caps(rs, per, &l1_cap, &slot_cap, &event_cap);
-  CU(cudaStreamSynchronize(st));
-  if ((rc = ensure_work(rs, rs->work, std::max<uint32_t>(per, 1), l1_cap, slot_cap, event_cap, 1))) return rc;
+  CU(cudaStreamSynchronize(st));                            // (whatever still read the staging buffers is done: s_h2d does not wait for st)
+  if ((rc = prepare_step(rs, per, false, st))) return rc;
   CU(cudaMemcpyAsync(G.d_off32, offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, G.s_h2d));
   CU(cudaMemsetAsync(G.d_bytes + total, 0, 64, G.s_h2d));
   CU(cudaEventRecord(G.ev0, st));
@@ -308,15 +350,16 @@ int scan_host_chunked(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offs
   CU(cudaStreamSynchronize(st)); CU(cudaStreamSynchronize(G.s_d2h)); CU(cudaStreamSynchronize(G.s_h2d));
   float ms = 0; cudaEventElapsedTime(&ms, G.ev0, G.ev1); G.stats.last_scan_ms = ms;
   bool overflow = false;
+  uint64_t events = 0;
   for (int c = 0; c < used; c++) {
-    const uint32_t* hc = G.h_chunk_counters + (size_t)c * kCounterWords; const uint32_t flags = hc[3];
-    if (flags & (ERR_VM_STACK | ERR_VM_LIST)) return fail(CG_ERR_TOO_LARGE, "matcher thread list / stack overflow on device");
-    if (flags) { learn_caps(rs, hc); overflow = true; }
-    G.stats.candidate_events += hc[1]; G.stats.verified_pairs += hc[1];
+    const uint32_t* hc = G.h_chunk_counters + (size_t)c * kCounterWords;
+    if ((rc = absorb_counters(rs, hc)) < 0) return rc;
+    overflow |= rc == 1;
+    events += hc[1];
   }
-  if (used) memcpy(rs->last_counters, G.h_chunk_counters + (size_t)(used - 1) * kCounterWords, sizeof rs->last_counters);
   if (overflow) return 1;
   G.stats.messages_scanned += n; G.stats.bytes_scanned += total - offsets[0];
+  G.stats.candidate_events += events; G.stats.verified_pairs += events;
   return CG_OK;
 }
 
@@ -328,8 +371,8 @@ void poll_mirrors(cg_ruleset* rs, bool wait) {
     else if (cudaEventQuery(rs->e_cnt[i]) != cudaSuccess) { cudaGetLastError(); continue; }
     rs->cnt_pending[i] = false;
     const uint32_t* hc = rs->h_counters + (size_t)i * kCounterWords;
-    memcpy(rs->last_counters, hc, sizeof rs->last_counters);
-    if (hc[3]) { rs->sticky_flags |= hc[3]; learn_caps(rs, hc); }
+    rs->sticky_flags |= hc[3];
+    absorb_counters(rs, hc);                                // (cg_scan_join reports the flags)
   }
 }
 
@@ -414,7 +457,7 @@ int cg_scan_work_counters(const cg_ruleset* rs, uint32_t out16[16]) {
 }
 
 int cg_get_stats(cg_stats* out) { if (!out) return fail(CG_ERR_INVALID_ARG, "null"); *out = G.stats; return CG_OK; }
-uint64_t cg_launch_count(void) { return G.launches; }
+uint64_t cg_launch_count(void) { return G.stats.kernel_launches; }
 
 int cg_rule_check(const char* source, uint32_t source_len, uint32_t flags, char* err, uint32_t err_len) {
   CompiledRule r = compile_rule(source ? source : "", source_len, flags);
@@ -559,10 +602,7 @@ int cg_scan_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets,
     for (uint32_t oi = 0; oi < n_slots; oi++) {
       uint32_t s = order[oi];
       if (hs.slot_msg[s] == 0xffffffffu) continue;
-      for (uint32_t k = 0; k < rw; k++) {
-        uint32_t v = hs.hit[(size_t)s * rw + k];
-        while (v) { uint32_t b = __builtin_ctz(v); v &= v - 1; if (out_hits && nh < hits_cap) { out_hits[nh].msg = hs.slot_msg[s]; out_hits[nh].rule = k * 32 + b; } nh++; }
-      }
+      nh = append_hit_row(&hs.hit[(size_t)s * rw], rw, nh, out_hits ? hits_cap : 0, [&](uint32_t i, uint32_t r) { out_hits[i].msg = hs.slot_msg[s]; out_hits[i].rule = r; });
     }
   }
   if (out_nhits) *out_nhits = nh;
@@ -581,31 +621,17 @@ int scan_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* 
   cudaStream_t st = G.stream;
   int rc;
   if (!o.h_pin) { CU(cudaMallocHost((void**)&o.h_pin, kOneIn + kOneOut)); memset(o.h_pin, 0, kOneIn + kOneOut); CU(cudaMalloc((void**)&o.d_buf, kOneIn + kOneOut)); CU(cudaMemset(o.d_buf, 0, kOneIn + kOneOut)); }
-  ScanWork& w = rs->work;
-  uint32_t l1, slot, ev; default_caps(rs, 1, &l1, &slot, &ev);
-  if (!w.counters || !w.msg_cap || l1 > w.l1_cap || slot > w.slot_cap || ev > w.event_cap || !w.spans) {
-    CU(cudaStreamSynchronize(st));
-    for (auto& g : rs->graphs) if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
-    if ((rc = ensure_work(rs, w, 1, l1, slot, ev, 1))) return rc;
-  }
-  rs->size_verify_grid();
-  const uint64_t caps[4] = {w.l1_cap, w.slot_cap, w.event_cap | ((uint64_t)rs->verify_ctas << 40), w.msg_cap};
+  if ((rc = prepare_step(rs, 1, false, st))) return rc;
   const uint8_t* d_bytes = o.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(o.d_buf);
   uint32_t* d_out = reinterpret_cast<uint32_t*>(o.d_buf + kOneIn); uint64_t* d_word = reinterpret_cast<uint64_t*>(o.d_buf + kOneIn + kOneOut - 8);   // (the word lands behind the hit row, then is packed to the front)
-  if (!o.exec || memcmp(caps, o.caps, sizeof caps)) {
+  if (!o.exec || o.gen != rs->scratch_gen || o.ctas != rs->verify_ctas) {
     if (o.exec) { cudaGraphExecDestroy(o.exec); o.exec = nullptr; }
-    cudaGraph_t g = nullptr;
-    const uint64_t before = G.launches;
-    CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    rc = run_scan_device(rs, d_bytes, d_off, 1, d_word, false, st);
-    if (rc == CG_OK) { const int k = launch_pack_one(rs->dev, w, d_word, d_out, kOneRw - 2, st); G.launches += k; }
-    cudaError_t e = cudaStreamEndCapture(st, &g);
-    o.kernels = (int)(G.launches - before); G.stats.kernel_launches -= o.kernels - 1; G.launches = before;
-    if (rc != CG_OK || e != cudaSuccess) { if (g) cudaGraphDestroy(g); cudaGetLastError(); return rc != CG_OK ? rc : cuda_fail(e, "cudaStreamEndCapture"); }
-    e = cudaGraphInstantiate(&o.exec, g, 0);
-    cudaGraphDestroy(g);
-    if (e != cudaSuccess) { o.exec = nullptr; return cuda_fail(e, "cudaGraphInstantiate"); }
-    memcpy(o.caps, caps, sizeof caps);
+    if ((rc = capture(st, [&] {
+          const int r = run_scan_device(rs, d_bytes, d_off, 1, d_word, false, st);
+          if (r == CG_OK) count_launches(launch_pack_one(rs->dev, rs->work, d_word, d_out, kOneRw - 2, st));
+          return r;
+        }, &o.exec, &o.kernels))) return rc;
+    o.gen = rs->scratch_gen; o.ctas = rs->verify_ctas;
   }
   uint32_t* hoff = reinterpret_cast<uint32_t*>(o.h_pin); hoff[0] = 256; hoff[1] = 256 + len;
   if (len) memcpy(o.h_pin + 256, bytes, len);
@@ -614,16 +640,13 @@ int scan_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* 
   CU(cudaGraphLaunch(o.exec, st));
   CU(cudaMemcpyAsync(o.h_pin + kOneIn, d_out, (2 + kCounterWords + rs->dev.rw) * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  G.launches += o.kernels; G.stats.kernel_launches += o.kernels;
+  count_launches(o.kernels);
   const uint32_t* ho = reinterpret_cast<const uint32_t*>(o.h_pin + kOneIn);
   const uint32_t* hc = ho + 2;
-  memcpy(rs->last_counters, hc, sizeof rs->last_counters);
-  if (hc[3] & (ERR_VM_STACK | ERR_VM_LIST)) return fail(CG_ERR_TOO_LARGE, "matcher thread list / stack overflow on device");
-  if (hc[3]) { learn_caps(rs, hc); return 1; }                    // a queue overflowed: the general path retries with larger scratch
+  if ((rc = absorb_counters(rs, hc))) return rc;                 // 1: a queue overflowed, the general path retries with larger scratch
   G.stats.messages_scanned += 1; G.stats.bytes_scanned += len; G.stats.candidate_events += hc[1]; G.stats.verified_pairs += hc[1];
   if (out_word) *out_word = (uint64_t)ho[0] | ((uint64_t)ho[1] << 32);
-  uint32_t nh = 0;
-  for (uint32_t k = 0; k < rs->dev.rw; k++) { uint32_t v = ho[2 + kCounterWords + k]; while (v) { const uint32_t b = (uint32_t)__builtin_ctz(v); v &= v - 1; if (out_rules && nh < rules_cap) out_rules[nh] = k * 32 + b; nh++; } }
+  const uint32_t nh = append_hit_row(ho + 2 + kCounterWords, rs->dev.rw, 0, out_rules ? rules_cap : 0, [&](uint32_t i, uint32_t r) { out_rules[i] = r; });
   if (out_nrules) *out_nrules = nh;
   G.stats.hits += nh;
   if (out_rules && nh > rules_cap) return fail(CG_ERR_CAPACITY, "out_rules too small");
@@ -705,7 +728,7 @@ int cg_ruleset_set_policy(cg_ruleset* rs, const uint32_t* rule_policy, const uin
   int rc;
   if ((rc = upload(rs, pol, &rs->dev.rule_policy))) return rc;
   if ((rc = upload(rs, act, &rs->dev.rule_action))) return rc;
-  for (auto& g : rs->graphs) if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }      // DevRuleset is captured by value
+  rs->scratch_gen++;                                        // DevRuleset is captured by value
   return CG_OK;
 }
 
@@ -722,7 +745,7 @@ int cg_policy_verdict_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t
   cudaStream_t st = G.stream;
   CU(cudaMemsetAsync(d_verdicts, 0, (size_t)n * 4, st));
   int k = launch_verdicts(rs->dev, rs->work, d_verdicts, G.sm_count, st);
-  G.launches += k; G.stats.kernel_launches += k;
+  count_launches(k);
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(out_verdicts, d_verdicts, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
@@ -773,7 +796,7 @@ int cg_redact_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offset
   }
   int kl = launch_redact_digests(G.d_bytes, d_start, d_len, ns, d_dig, st);
   kl += launch_redact_splice(G.d_bytes, G.d_off32, d_out_off, d_span_begin, d_start, d_len, d_cat, d_dig, d_out, n, G.sm_count, st);
-  G.launches += kl; G.stats.kernel_launches += kl; G.stats.sha256_items += ns;
+  count_launches(kl); G.stats.sha256_items += ns;
   CU(cudaGetLastError());
   if (pos) CU(cudaMemcpyAsync(out_bytes, d_out, (size_t)pos, cudaMemcpyDeviceToHost, st));
   if (ns && out_digests32) CU(cudaMemcpyAsync(out_digests32, d_dig, (size_t)ns * 32, cudaMemcpyDeviceToHost, st));
@@ -789,7 +812,6 @@ int cg_scan_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offs
   cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
   if (!n) return CG_OK;
   static const bool use_graph = !(getenv("CG_NO_GRAPH") && atoi(getenv("CG_NO_GRAPH")));
-  ScanWork& w = rs->work;
   int rc;
   if (!rs->h_counters) {
     CU(cudaMallocHost((void**)&rs->h_counters, (size_t)cg_ruleset::kMirror * kCounterWords * 4));
@@ -797,49 +819,30 @@ int cg_scan_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offs
   }
   // did an earlier batch overflow a queue?  (its result words say "incomplete"; grow the scratch before this one runs)
   poll_mirrors(rs, false);
-  uint32_t want_l1, want_slot, want_ev;
-  default_caps(rs, n, &want_l1, &want_slot, &want_ev);
-  if (n > w.msg_cap || want_l1 > w.l1_cap || want_slot > w.slot_cap || want_ev > w.event_cap || !w.counters || !w.spans) {
-    // (re)allocation: nothing may still be using the old buffers
-    CU(cudaStreamSynchronize(st));
-    for (auto& g : rs->graphs) if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
-    if ((rc = ensure_work(rs, w, std::max<uint32_t>(n, 1), want_l1, want_slot, want_ev, 1))) return rc;
-  }
-  rs->size_verify_grid();
+  if ((rc = prepare_step(rs, n, false, st))) return rc;
+  const auto enqueue = [&] { return run_scan_device(rs, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, n, (uint64_t*)d_out_words, false, st); };
   if (!use_graph || G.profiling) {
-    rc = run_scan_device(rs, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, n, (uint64_t*)d_out_words, false, st);
+    rc = enqueue();
   } else {
-    // memsets + scan + resolve + verify + finalize captured once per (arguments, capacities), then replayed:
-    // one launch per step instead of six, so the host never becomes the bottleneck
-    const uint64_t caps[4] = {w.l1_cap, w.slot_cap, w.event_cap | ((uint64_t)rs->verify_ctas << 40), w.msg_cap};
+    // memsets + scan + resolve + verify + finalize captured once per (arguments, scratch generation, verify grid), then
+    // replayed: one launch per step instead of six, so the host never becomes the bottleneck
     cg_ruleset::CachedGraph* hit = nullptr;
-    for (auto& g : rs->graphs) if (g.exec && g.bytes == d_bytes && g.off == d_offsets && g.words == d_out_words && g.n == n && !memcmp(caps, g.caps, sizeof caps)) hit = &g;
+    for (auto& g : rs->graphs) if (g.exec && g.bytes == d_bytes && g.off == d_offsets && g.words == d_out_words && g.n == n && g.gen == rs->scratch_gen && g.ctas == rs->verify_ctas) hit = &g;
     if (!hit) {
       hit = rs->graphs[0].used <= rs->graphs[1].used ? &rs->graphs[0] : &rs->graphs[1];       // least recently used entry
       if (hit->exec) { cudaGraphExecDestroy(hit->exec); hit->exec = nullptr; }
-      cudaGraph_t g = nullptr;
-      const uint64_t launches_before = G.launches;
-      CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      rc = run_scan_device(rs, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, n, (uint64_t*)d_out_words, false, st);
-      cudaError_t e = cudaStreamEndCapture(st, &g);
-      hit->kernels = (int)(G.launches - launches_before);
-      G.stats.kernel_launches -= G.launches - launches_before; G.launches = launches_before;      // counted per replay below
-      if (rc != CG_OK || e != cudaSuccess) { if (g) cudaGraphDestroy(g); cudaGetLastError(); return rc != CG_OK ? rc : cuda_fail(e, "cudaStreamEndCapture"); }
-      e = cudaGraphInstantiate(&hit->exec, g, 0);
-      cudaGraphDestroy(g);
-      if (e != cudaSuccess) { hit->exec = nullptr; return cuda_fail(e, "cudaGraphInstantiate"); }
-      hit->bytes = d_bytes; hit->off = d_offsets; hit->words = d_out_words; hit->n = n; memcpy(hit->caps, caps, sizeof caps);
+      if ((rc = capture(st, enqueue, &hit->exec, &hit->kernels))) return rc;
+      hit->bytes = d_bytes; hit->off = d_offsets; hit->words = d_out_words; hit->n = n; hit->gen = rs->scratch_gen; hit->ctas = rs->verify_ctas;
     }
     hit->used = ++rs->graph_clock;
     CU(cudaGraphLaunch(hit->exec, st));
-    const int kk = hit->kernels;                 // kernels inside the graph (counted while it was captured)
-    G.launches += kk; G.stats.kernel_launches += kk;
+    count_launches(hit->kernels);
   }
   if (rc == CG_OK) {
     G.stats.messages_scanned += n;
     const int slot = (int)(rs->seq % cg_ruleset::kMirror);
     if (rs->cnt_pending[slot]) { cudaEventSynchronize(rs->e_cnt[slot]); poll_mirrors(rs, false); }
-    CU(cudaMemcpyAsync(rs->h_counters + (size_t)slot * kCounterWords, w.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(rs->h_counters + (size_t)slot * kCounterWords, rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(rs->e_cnt[slot], st));
     rs->cnt_pending[slot] = true; rs->seq++;
   }
@@ -853,7 +856,7 @@ int cg_scan_join(cg_ruleset* rs, void* stream) {
   CU(cudaStreamSynchronize(stream ? (cudaStream_t)stream : G.stream));
   poll_mirrors(rs, true);
   const uint32_t flags = rs->sticky_flags; rs->sticky_flags = 0;
-  if (flags & (ERR_VM_STACK | ERR_VM_LIST)) return fail(CG_ERR_TOO_LARGE, "matcher thread list / stack overflow on device (result words of that batch are all ones)");
+  if (flags & (ERR_VM_STACK | ERR_VM_LIST)) return fail(CG_ERR_TOO_LARGE, std::string(kVmOverflow) + " (result words of that batch are all ones)");
   if (flags) return fail(CG_ERR_CAPACITY, "a candidate queue overflowed: the result words of that batch are all ones; the scratch has been grown, scan the batch again");
   return CG_OK;
 }
@@ -873,7 +876,7 @@ int cg_sha256_batch(const uint8_t* bytes, const uint64_t* offsets, uint32_t n, u
   if (total) CU(cudaMemcpyAsync(G.d_bytes, bytes, total, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(G.d_off64, offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
   int k = launch_sha256_batch(G.d_bytes, G.d_off64, n, (uint8_t*)G.d_dig[0], st);
-  G.launches += k; G.stats.kernel_launches += k; G.stats.sha256_items += n;
+  count_launches(k); G.stats.sha256_items += n;
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(out, G.d_dig[0], (size_t)n * 32, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
@@ -889,7 +892,7 @@ int fold_levels(uint64_t n, uint64_t stop_at, int cur, cudaStream_t st, uint32_t
     uint32_t step = 1;
     if (n <= (1u << 15)) { step = 5; while (step > 1 && (lv + step > max_levels || ((n + (1ull << step) - 1) >> step) < stop_at)) step--; }
     int k = step > 1 ? launch_merkle_reduce(G.d_dig[cur], n, step, G.d_dig[cur ^ 1], st) : launch_merkle_level(G.d_dig[cur], n, G.d_dig[cur ^ 1], st);
-    G.launches += k; G.stats.kernel_launches += k;
+    count_launches(k);
     n = (n + (1ull << step) - 1) >> step; cur ^= 1; lv += step;
   }
   return cur;
@@ -902,7 +905,7 @@ int empty_root(uint8_t out[32]) {
   if ((rc = grow_bytes(64))) return rc;
   CU(cudaMemsetAsync(G.d_off64, 0, 16, G.stream));
   int k = launch_sha256_batch(G.d_bytes, G.d_off64, 1, (uint8_t*)G.d_dig[0], G.stream);
-  G.launches += k; G.stats.kernel_launches += k;
+  count_launches(k);
   CU(cudaMemcpyAsync(out, G.d_dig[0], 32, cudaMemcpyDeviceToHost, G.stream));
   CU(cudaStreamSynchronize(G.stream));
   return CG_OK;
@@ -925,7 +928,7 @@ int cg_merkle_root(const uint8_t* bytes, const uint64_t* offsets, uint64_t n, ui
   CU(cudaMemcpyAsync(G.d_off64, offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
   CU(cudaEventRecord(G.ev0, st));
   int k = launch_merkle_leaves_var(G.d_bytes, G.d_off64, n, G.d_dig[0], st);
-  G.launches += k; G.stats.kernel_launches += k; G.stats.merkle_leaves += n;
+  count_launches(k); G.stats.merkle_leaves += n;
   int cur = fold_levels(n, 1, 0, st);
   CU(cudaEventRecord(G.ev1, st));
   CU(cudaGetLastError());
@@ -948,7 +951,7 @@ int cg_merkle_root_fixed(const uint8_t* bytes, uint64_t leaf_len, uint64_t n, ui
   if (total) CU(cudaMemcpyAsync(G.d_bytes, bytes, total, cudaMemcpyHostToDevice, st));
   CU(cudaEventRecord(G.ev0, st));
   int k = launch_merkle_leaves_fixed(G.d_bytes, leaf_len, n, G.d_dig[0], st);
-  G.launches += k; G.stats.kernel_launches += k; G.stats.merkle_leaves += n;
+  count_launches(k); G.stats.merkle_leaves += n;
   int cur = fold_levels(n, 1, 0, st);
   CU(cudaEventRecord(G.ev1, st));
   CU(cudaGetLastError());
@@ -970,7 +973,7 @@ int cg_merkle_block_roots_device(const void* d_bytes, uint64_t leaf_len, uint64_
   if ((rc = grow(&G.d_dig[1], &G.cap_dig[1], (size_t)(n + 1) / 2 * 8 + 8))) return rc;
   cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
   int k = launch_merkle_leaves_fixed((const uint8_t*)d_bytes, leaf_len, n, G.d_dig[0], st);
-  G.launches += k; G.stats.kernel_launches += k; G.stats.merkle_leaves += n;
+  count_launches(k); G.stats.merkle_leaves += n;
   int cur = fold_levels(n, 1, 0, st, block_log2);
   uint64_t nblocks = (n + ((1ull << block_log2) - 1)) >> block_log2;
   CU(cudaMemcpyAsync(d_out_roots, G.d_dig[cur], nblocks * 32, cudaMemcpyDeviceToDevice, st));
@@ -1002,7 +1005,7 @@ int log_range_root(cg_merkle_log* L, const uint32_t* d_in, uint64_t cnt, uint32_
     uint32_t step = 1;
     if (m <= (1u << 15)) { step = 5; while (step > 1 && (m >> (step - 1)) == 0) step--; while (step > 1 && ((m + (1ull << (step - 1)) - 1) >> (step - 1)) == 1) step--; }
     int k = step > 1 ? launch_merkle_reduce(src, m, step, dst, st) : launch_merkle_level(src, m, dst, st);
-    G.launches += k; G.stats.kernel_launches += k;
+    count_launches(k);
     m = (m + (1ull << step) - 1) >> step; src = dst; dst = dst == L->d_a ? L->d_b : L->d_a;
   }
   CU(cudaMemcpyAsync(d_out, src, 32, cudaMemcpyDeviceToDevice, st));
@@ -1022,7 +1025,7 @@ int log_root_device(cg_merkle_log* L, cudaStream_t st) {
     CU(cudaMemcpyAsync(L->d_tmp + 8 * nl, L->d_slots + 8 * h, 32, cudaMemcpyDeviceToDevice, st)); nl++;
   }
   int k = launch_merkle_chain(L->d_tmp, nl, L->d_slots + 8 * lowest, L->d_tmp + 8 * 65, st);
-  G.launches += k; G.stats.kernel_launches += k;
+  count_launches(k);
   return CG_OK;
 }
 }  // namespace
@@ -1094,21 +1097,13 @@ int log_absorb(cg_merkle_log* L, const uint32_t* d_dig, uint64_t m, cudaStream_t
     int h = 0; while ((1ull << h) < s) h++;
     uint32_t nl = 0; int top = h;                           // slots h, h+1, ... that are occupied merge into the new subtree
     while ((pos >> top) & 1ull) { CU(cudaMemcpyAsync(L->d_tmp + 8 * nl, L->d_slots + 8 * top, 32, cudaMemcpyDeviceToDevice, st)); nl++; top++; }
-    if (nl) { k = launch_merkle_chain(L->d_tmp, nl, acc, L->d_slots + 8 * top, st); G.launches += k; G.stats.kernel_launches += k; }
+    if (nl) { k = launch_merkle_chain(L->d_tmp, nl, acc, L->d_slots + 8 * top, st); count_launches(k); }
     else CU(cudaMemcpyAsync(L->d_slots + 8 * top, acc, 32, cudaMemcpyDeviceToDevice, st));
     pos += s; rem -= s;
   }
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(st));
   L->n += m;
-  return CG_OK;
-}
-int ensure_copy_streams() {
-  if (G.s_h2d) return CG_OK;
-  const int C = Ctx::kChunks;
-  CU(cudaStreamCreateWithFlags(&G.s_h2d, cudaStreamNonBlocking)); CU(cudaStreamCreateWithFlags(&G.s_d2h, cudaStreamNonBlocking));
-  for (int c = 0; c < C; c++) { CU(cudaEventCreateWithFlags(&G.e_h2d[c], cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&G.e_done[c], cudaEventDisableTiming)); }
-  CU(cudaMallocHost((void**)&G.h_chunk_counters, (size_t)C * kCounterWords * 4));
   return CG_OK;
 }
 }  // namespace
@@ -1152,7 +1147,7 @@ int cg_merkle_log_append(cg_merkle_log* L, const uint8_t* bytes, const uint64_t*
     CU(cudaEventRecord(G.e_h2d[c], G.s_h2d));
     CU(cudaStreamWaitEvent(st, G.e_h2d[c], 0));
     int k = launch_merkle_leaves_var(G.d_bytes, G.d_off64 + m0, m1 - m0, d_dig + (size_t)m0 * 8, st);
-    G.launches += k; G.stats.kernel_launches += k;
+    count_launches(k);
   }
   G.stats.merkle_leaves += m;
   return log_absorb(L, d_dig, m, st);
@@ -1184,7 +1179,7 @@ int cg_merkle_log_append_jsonl(cg_merkle_log* L, const uint8_t* bytes, uint64_t 
   uint32_t* d_dig;
   if ((rc = log_digest_room(L, n_lines, st, &d_dig))) return rc;
   k += launch_merkle_leaves_var(G.d_bytes, G.d_off64, n_lines, d_dig, st, /*trim_newline=*/true);
-  G.launches += k; G.stats.kernel_launches += k; G.stats.merkle_leaves += n_lines;
+  count_launches(k); G.stats.merkle_leaves += n_lines;
   if (out_lines) *out_lines = n_lines;
   return log_absorb(L, d_dig, n_lines, st);
 }
@@ -1274,7 +1269,7 @@ int cg_merkle_verify_consistency(uint64_t first_size, uint64_t second_size, cons
   CU(cudaMemcpyAsync(d_r2, root_second, 32, cudaMemcpyHostToDevice, st));
   if (path_len) CU(cudaMemcpyAsync(d_path, path32, (size_t)path_len * 32, cudaMemcpyHostToDevice, st));
   int k = launch_merkle_consistency(first_size, second_size, d_r1, d_r2, d_path, path_len, d_ok, st);
-  G.launches += k; G.stats.kernel_launches += k;
+  count_launches(k);
   uint32_t ok = 0;
   CU(cudaMemcpyAsync(&ok, d_ok, 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
@@ -1300,7 +1295,7 @@ int cg_merkle_verify_proof(const uint8_t* leaf_bytes, uint64_t leaf_len, uint64_
   CU(cudaMemcpyAsync(d_root, root, 32, cudaMemcpyHostToDevice, st));
   if (path_len) CU(cudaMemcpyAsync(d_path, path32, (size_t)path_len * 32, cudaMemcpyHostToDevice, st));
   k += launch_merkle_verify(d_leaf, index, tree_size, d_path, path_len, d_root, d_ok, st);
-  G.launches += k; G.stats.kernel_launches += k;
+  count_launches(k);
   uint32_t ok = 0;
   CU(cudaMemcpyAsync(&ok, d_ok, 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
