@@ -54,7 +54,20 @@ int cuda_fail(cudaError_t e, const char* what) {
   return CG_ERR_CUDA;
 }
 #define CU(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) return cuda_fail(_e, #x); } while (0)
+int require_ready() { return G.ready ? CG_OK : fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)"); }
 void count_launches(int k) { G.stats.kernel_launches += k; }
+
+// NCCL, bound at run time (nccl_load), and the communicator of cg_comm_init
+struct NcclApi {
+  void* h = nullptr; void* comm = nullptr; int rank = 0, world = 1;
+  int (*GetUniqueId)(void*) = nullptr;
+  int (*CommInitRank)(void**, int, cg_nccl_id, int) = nullptr;
+  int (*AllGather)(const void*, void*, size_t, int, void*, cudaStream_t) = nullptr;
+  int (*CommDestroy)(void*) = nullptr;
+  const char* (*GetErrorString)(int) = nullptr;
+  uint32_t* d_roots = nullptr; size_t cap_roots = 0;     // cg_merkle_root_sharded_device: every rank's block roots (grow-only)
+} g_nccl;
+void free_shard_roots() { if (g_nccl.d_roots) cudaFree(g_nccl.d_roots); g_nccl.d_roots = nullptr; g_nccl.cap_roots = 0; }
 
 template <typename T>
 int grow(T** p, size_t* cap, size_t need_elems) {
@@ -268,7 +281,7 @@ int check_offsets(const uint32_t* offsets, uint32_t n) {
 
 // full host-buffer scan with capacity retry; leaves words in G.d_words
 int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, bool spans, HostScan* hs) {
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!rs || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
   int rc;
   if (n && (rc = check_offsets(offsets, n))) return rc;
@@ -417,6 +430,7 @@ void cg_shutdown(void) {
   if (G.h_chunk_counters) cudaFreeHost(G.h_chunk_counters);
   if (G.s_h2d) { cudaStreamDestroy(G.s_h2d); cudaStreamDestroy(G.s_d2h); for (int c = 0; c < Ctx::kChunks; c++) { cudaEventDestroy(G.e_h2d[c]); cudaEventDestroy(G.e_done[c]); } }
   cudaFree(G.d_bytes_raw); cudaFree(G.d_off32); cudaFree(G.d_off64); cudaFree(G.d_words); cudaFree(G.d_dig[0]); cudaFree(G.d_dig[1]);
+  free_shard_roots();
   cudaEventDestroy(G.ev0); cudaEventDestroy(G.ev1); for (int i = 0; i < 5; i++) cudaEventDestroy(G.pev[i]); for (int i = 0; i < 8; i++) cudaEventDestroy(G.pev_scan[i]); cudaStreamDestroy(G.stream);
   G = Ctx();
 }
@@ -470,7 +484,7 @@ int cg_rule_check(const char* source, uint32_t source_len, uint32_t flags, char*
 int cg_ruleset_create(const cg_rule* rules, uint32_t n_rules, uint32_t options, cg_ruleset** out, int32_t* status_per_rule) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!out || (n_rules && !rules)) return fail(CG_ERR_INVALID_ARG, "null argument");
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   std::unique_ptr<cg_ruleset> rs(new cg_ruleset());
   std::vector<RuleSrc> src(n_rules);
   rs->category.resize(n_rules);
@@ -716,7 +730,7 @@ int cg_find_matches_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* 
 
 int cg_ruleset_set_policy(cg_ruleset* rs, const uint32_t* rule_policy, const uint8_t* rule_action, uint32_t n_rules) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!rs || !rule_policy || !rule_action || n_rules != rs->dev.n_rules) return fail(CG_ERR_INVALID_ARG, "one (policy, action) pair per rule of the set");
   std::vector<uint32_t> pol(rule_policy, rule_policy + n_rules), act(n_rules);
   for (uint32_t i = 0; i < n_rules; i++) {
@@ -806,7 +820,7 @@ int cg_redact_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offset
 
 int cg_scan_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_words, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!rs || !d_bytes || !d_offsets || !d_out_words) return fail(CG_ERR_INVALID_ARG, "null argument");
   if ((uintptr_t)d_bytes & 15u) return fail(CG_ERR_INVALID_ARG, "d_bytes must be 16-byte aligned");
   cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
@@ -851,7 +865,7 @@ int cg_scan_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offs
 
 int cg_scan_join(cg_ruleset* rs, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!rs) return fail(CG_ERR_INVALID_ARG, "null argument");
   CU(cudaStreamSynchronize(stream ? (cudaStream_t)stream : G.stream));
   poll_mirrors(rs, true);
@@ -865,7 +879,7 @@ int cg_scan_join(cg_ruleset* rs, void* stream) {
 
 int cg_sha256_batch(const uint8_t* bytes, const uint64_t* offsets, uint32_t n, uint8_t* out) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!n) return CG_OK;
   if (!offsets || !out) return fail(CG_ERR_INVALID_ARG, "null argument");
   size_t total = offsets[n]; int rc;
@@ -884,19 +898,6 @@ int cg_sha256_batch(const uint8_t* bytes, const uint64_t* offsets, uint32_t n, u
 }
 
 namespace {
-// fold the n digests in G.d_dig[cur] down to `target` nodes (level by level); returns buffer index
-int fold_levels(uint64_t n, uint64_t stop_at, int cur, cudaStream_t st, uint32_t max_levels = 64) {
-  uint32_t lv = 0;
-  while (n > stop_at && lv < max_levels) {
-    // large levels: one kernel per level, every lane busy; from 2^15 nodes down: up to five levels per kernel inside warps
-    uint32_t step = 1;
-    if (n <= (1u << 15)) { step = 5; while (step > 1 && (lv + step > max_levels || ((n + (1ull << step) - 1) >> step) < stop_at)) step--; }
-    int k = step > 1 ? launch_merkle_reduce(G.d_dig[cur], n, step, G.d_dig[cur ^ 1], st) : launch_merkle_level(G.d_dig[cur], n, G.d_dig[cur ^ 1], st);
-    count_launches(k);
-    n = (n + (1ull << step) - 1) >> step; cur ^= 1; lv += step;
-  }
-  return cur;
-}
 int empty_root(uint8_t out[32]) {
   // SHA-256("") -- computed by the same kernel, not on the CPU
   int rc;
@@ -910,74 +911,106 @@ int empty_root(uint8_t out[32]) {
   CU(cudaStreamSynchronize(G.stream));
   return CG_OK;
 }
+
+// One-shot trees: size_dig(n) makes room for n staged nodes in G.d_dig[0]; fold_dig folds n nodes at d_nodes (read in place,
+// may be G.d_dig[0]) by at most max_levels levels, ping-ponging between G.d_dig[1] and G.d_dig[0]; *out = the folded nodes
+int size_dig(uint64_t n) {
+  int rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)n * 8);
+  return rc ? rc : grow(&G.d_dig[1], &G.cap_dig[1], (size_t)(n + 1) / 2 * 8 + 8);
+}
+int fold_dig(const uint32_t* d_nodes, uint64_t n, uint32_t max_levels, cudaStream_t st, const uint32_t** out) {
+  count_launches(launch_merkle_fold(d_nodes, n, max_levels, G.d_dig[1], G.d_dig[0], st, out));
+  CU(cudaGetLastError());
+  return CG_OK;
+}
+
+// root of n leaves in G.d_bytes (ragged at d_off, else leaf_len bytes each) -> host; leaves and fold time last_merkle_ms
+int staged_root(uint64_t n, const uint64_t* d_off, uint64_t leaf_len, uint8_t out_root[32]) {
+  cudaStream_t st = G.stream; const uint32_t* d_root; int rc;
+  if ((rc = size_dig(n))) return rc;
+  CU(cudaEventRecord(G.ev0, st));
+  count_launches(d_off ? launch_merkle_leaves_var(G.d_bytes, d_off, n, G.d_dig[0], st) : launch_merkle_leaves_fixed(G.d_bytes, leaf_len, n, G.d_dig[0], st));
+  G.stats.merkle_leaves += n;
+  if ((rc = fold_dig(G.d_dig[0], n, 64, st, &d_root))) return rc;
+  CU(cudaEventRecord(G.ev1, st));
+  CU(cudaMemcpyAsync(out_root, d_root, 32, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  float ms = 0; cudaEventElapsedTime(&ms, G.ev0, G.ev1); G.stats.last_merkle_ms = ms;
+  return CG_OK;
+}
+
+// roots of the aligned 2^block_log2-leaf blocks of n fixed-size leaves in device memory -> d_roots (32 bytes per block)
+int block_roots(const void* d_bytes, uint64_t leaf_len, uint64_t n, uint32_t block_log2, void* d_roots, cudaStream_t st) {
+  const uint32_t* d_res; int rc;
+  if ((rc = size_dig(n))) return rc;
+  count_launches(launch_merkle_leaves_fixed((const uint8_t*)d_bytes, leaf_len, n, G.d_dig[0], st)); G.stats.merkle_leaves += n;
+  if ((rc = fold_dig(G.d_dig[0], n, block_log2, st, &d_res))) return rc;
+  CU(cudaMemcpyAsync(d_roots, d_res, ((n + (1ull << block_log2) - 1) >> block_log2) * 32, cudaMemcpyDeviceToDevice, st));
+  return CG_OK;
+}
 }  // namespace
 
 int cg_merkle_root(const uint8_t* bytes, const uint64_t* offsets, uint64_t n, uint8_t out_root[32]) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!out_root) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (n == 0) return empty_root(out_root);
   if (!offsets) return fail(CG_ERR_INVALID_ARG, "null argument");
   size_t total = offsets[n]; int rc;
   if ((rc = grow_bytes(total + 64))) return rc;
   if ((rc = grow(&G.d_off64, &G.cap_off64, (size_t)n + 1))) return rc;
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)n * 8))) return rc;
-  if ((rc = grow(&G.d_dig[1], &G.cap_dig[1], (size_t)(n + 1) / 2 * 8 + 8))) return rc;
-  cudaStream_t st = G.stream;
-  if (total) CU(cudaMemcpyAsync(G.d_bytes, bytes, total, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(G.d_off64, offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
-  CU(cudaEventRecord(G.ev0, st));
-  int k = launch_merkle_leaves_var(G.d_bytes, G.d_off64, n, G.d_dig[0], st);
-  count_launches(k); G.stats.merkle_leaves += n;
-  int cur = fold_levels(n, 1, 0, st);
-  CU(cudaEventRecord(G.ev1, st));
-  CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out_root, G.d_dig[cur], 32, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  float ms = 0; cudaEventElapsedTime(&ms, G.ev0, G.ev1); G.stats.last_merkle_ms = ms;
-  return CG_OK;
+  if (total) CU(cudaMemcpyAsync(G.d_bytes, bytes, total, cudaMemcpyHostToDevice, G.stream));
+  CU(cudaMemcpyAsync(G.d_off64, offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, G.stream));
+  return staged_root(n, G.d_off64, 0, out_root);
 }
 
 int cg_merkle_root_fixed(const uint8_t* bytes, uint64_t leaf_len, uint64_t n, uint8_t out_root[32]) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!out_root) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (n == 0) return empty_root(out_root);
   size_t total = (size_t)leaf_len * n; int rc;
   if ((rc = grow_bytes(total + 64))) return rc;
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)n * 8))) return rc;
-  if ((rc = grow(&G.d_dig[1], &G.cap_dig[1], (size_t)(n + 1) / 2 * 8 + 8))) return rc;
-  cudaStream_t st = G.stream;
-  if (total) CU(cudaMemcpyAsync(G.d_bytes, bytes, total, cudaMemcpyHostToDevice, st));
-  CU(cudaEventRecord(G.ev0, st));
-  int k = launch_merkle_leaves_fixed(G.d_bytes, leaf_len, n, G.d_dig[0], st);
-  count_launches(k); G.stats.merkle_leaves += n;
-  int cur = fold_levels(n, 1, 0, st);
-  CU(cudaEventRecord(G.ev1, st));
-  CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out_root, G.d_dig[cur], 32, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  float ms = 0; cudaEventElapsedTime(&ms, G.ev0, G.ev1); G.stats.last_merkle_ms = ms;
-  return CG_OK;
+  if (total) CU(cudaMemcpyAsync(G.d_bytes, bytes, total, cudaMemcpyHostToDevice, G.stream));
+  return staged_root(n, nullptr, leaf_len, out_root);
 }
 
 int cg_merkle_block_roots_device(const void* d_bytes, uint64_t leaf_len, uint64_t n, uint32_t block_log2, void* d_out_roots, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
-  // (beyond 2^40 leaves per block the block count below would need a shift of 64 or more: undefined, and it sizes the copy)
+  if (int rc = require_ready()) return rc;
+  // (beyond 2^40 leaves per block the block count would need a shift of 64 or more: undefined, and it sizes the copy)
   if (block_log2 > 40) return fail(CG_ERR_INVALID_ARG, "block_log2 must be at most 40");
   if (!n) return CG_OK;
   if (!d_bytes || !d_out_roots) return fail(CG_ERR_INVALID_ARG, "null argument");
-  int rc;
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)n * 8))) return rc;
-  if ((rc = grow(&G.d_dig[1], &G.cap_dig[1], (size_t)(n + 1) / 2 * 8 + 8))) return rc;
-  cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
-  int k = launch_merkle_leaves_fixed((const uint8_t*)d_bytes, leaf_len, n, G.d_dig[0], st);
-  count_launches(k); G.stats.merkle_leaves += n;
-  int cur = fold_levels(n, 1, 0, st, block_log2);
-  uint64_t nblocks = (n + ((1ull << block_log2) - 1)) >> block_log2;
-  CU(cudaMemcpyAsync(d_out_roots, G.d_dig[cur], nblocks * 32, cudaMemcpyDeviceToDevice, st));
-  CU(cudaGetLastError());
+  return block_roots(d_bytes, leaf_len, n, block_log2, d_out_roots, stream ? (cudaStream_t)stream : G.stream);
+}
+
+int cg_merkle_fold(const uint8_t* nodes32, uint64_t m, uint8_t out_root[32]) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  if (!out_root) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (m == 0) return empty_root(out_root);
+  if (!nodes32) return fail(CG_ERR_INVALID_ARG, "null argument");
+  cudaStream_t st = G.stream; const uint32_t* d_root; int rc;
+  if ((rc = size_dig(m))) return rc;
+  CU(cudaMemcpyAsync(G.d_dig[0], nodes32, m * 32, cudaMemcpyHostToDevice, st));
+  if ((rc = fold_dig(G.d_dig[0], m, 64, st, &d_root))) return rc;
+  CU(cudaMemcpyAsync(out_root, d_root, 32, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return CG_OK;
+}
+
+int cg_merkle_fold_device(const void* d_nodes32, uint64_t m, void* d_out_root32, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  if (!m || !d_nodes32 || !d_out_root32) return fail(CG_ERR_INVALID_ARG, "null or empty input");
+  cudaStream_t st = stream ? (cudaStream_t)stream : G.stream; const uint32_t* d_root; int rc;
+  if ((rc = size_dig(m))) return rc;
+  // the fold reads the nodes in place, unless they are off the 16-byte alignment of the kernels' loads: then from a copy
+  const uint32_t* d_nodes = (const uint32_t*)d_nodes32;
+  if ((uintptr_t)d_nodes32 & 15) { CU(cudaMemcpyAsync(G.d_dig[0], d_nodes32, m * 32, cudaMemcpyDeviceToDevice, st)); d_nodes = G.d_dig[0]; }
+  if ((rc = fold_dig(d_nodes, m, 64, st, &d_root))) return rc;
+  CU(cudaMemcpyAsync(d_out_root32, d_root, 32, cudaMemcpyDeviceToDevice, st));
   return CG_OK;
 }
 
@@ -1000,19 +1033,13 @@ int log_range_root(cg_merkle_log* L, const uint32_t* d_in, uint64_t cnt, uint32_
   if (cnt == 1) { CU(cudaMemcpyAsync(d_out, d_in, 32, cudaMemcpyDeviceToDevice, st)); return CG_OK; }
   if ((rc = grow(&L->d_a, &L->cap_a, (size_t)(cnt + 1) / 2 * 8 + 8))) return rc;
   if ((rc = grow(&L->d_b, &L->cap_b, (size_t)(cnt + 3) / 4 * 8 + 8))) return rc;
-  const uint32_t* src = d_in; uint32_t* dst = L->d_a; uint64_t m = cnt;
-  while (m > 1) {
-    uint32_t step = 1;
-    if (m <= (1u << 15)) { step = 5; while (step > 1 && (m >> (step - 1)) == 0) step--; while (step > 1 && ((m + (1ull << (step - 1)) - 1) >> (step - 1)) == 1) step--; }
-    int k = step > 1 ? launch_merkle_reduce(src, m, step, dst, st) : launch_merkle_level(src, m, dst, st);
-    count_launches(k);
-    m = (m + (1ull << step) - 1) >> step; src = dst; dst = dst == L->d_a ? L->d_b : L->d_a;
-  }
-  CU(cudaMemcpyAsync(d_out, src, 32, cudaMemcpyDeviceToDevice, st));
+  const uint32_t* d_root;
+  count_launches(launch_merkle_fold(d_in, cnt, 64, L->d_a, L->d_b, st, &d_root));
+  CU(cudaMemcpyAsync(d_out, d_root, 32, cudaMemcpyDeviceToDevice, st));
   return CG_OK;
 }
 int log_check(cg_merkle_log* L) {
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!L) return fail(CG_ERR_INVALID_ARG, "null argument");
   return CG_OK;
 }
@@ -1032,7 +1059,7 @@ int log_root_device(cg_merkle_log* L, cudaStream_t st) {
 
 int cg_merkle_log_create(cg_merkle_log** out, int keep_leaf_digests) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!out) return fail(CG_ERR_INVALID_ARG, "null argument");
   std::unique_ptr<cg_merkle_log> L(new cg_merkle_log());
   L->keep = keep_leaf_digests != 0;
@@ -1260,7 +1287,7 @@ int cg_merkle_log_consistency(cg_merkle_log* L, uint64_t first_size, uint8_t* ou
 int cg_merkle_verify_consistency(uint64_t first_size, uint64_t second_size, const uint8_t root_first[32], const uint8_t root_second[32],
                                  const uint8_t* path32, uint32_t path_len, int* out_ok) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!out_ok || !root_first || !root_second || (path_len && !path32) || path_len > 64) return fail(CG_ERR_INVALID_ARG, "bad argument");
   int rc; cudaStream_t st = G.stream;
   if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)(path_len + 4) * 8))) return rc;
@@ -1281,7 +1308,7 @@ int cg_merkle_verify_consistency(uint64_t first_size, uint64_t second_size, cons
 int cg_merkle_verify_proof(const uint8_t* leaf_bytes, uint64_t leaf_len, uint64_t index, uint64_t tree_size, const uint8_t* path32, uint32_t path_len,
                            const uint8_t root[32], int* out_ok) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!out_ok || !root || (leaf_len && !leaf_bytes) || (path_len && !path32) || path_len > 64) return fail(CG_ERR_INVALID_ARG, "bad argument");
   int rc; cudaStream_t st = G.stream;
   if ((rc = grow_bytes((size_t)leaf_len + 64))) return rc;
@@ -1304,21 +1331,6 @@ int cg_merkle_verify_proof(const uint8_t* leaf_bytes, uint64_t leaf_len, uint64_
   return CG_OK;
 }
 
-int cg_merkle_fold_device(const void* d_nodes32, uint64_t m, void* d_out_root32, void* stream) {
-  std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
-  if (!m || !d_nodes32 || !d_out_root32) return fail(CG_ERR_INVALID_ARG, "null or empty input");
-  int rc;
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)m * 8))) return rc;
-  if ((rc = grow(&G.d_dig[1], &G.cap_dig[1], (size_t)(m + 1) / 2 * 8 + 8))) return rc;
-  cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
-  CU(cudaMemcpyAsync(G.d_dig[0], d_nodes32, m * 32, cudaMemcpyDeviceToDevice, st));
-  int cur = fold_levels(m, 1, 0, st);
-  CU(cudaMemcpyAsync(d_out_root32, G.d_dig[cur], 32, cudaMemcpyDeviceToDevice, st));
-  CU(cudaGetLastError());
-  return CG_OK;
-}
-
 // ---------------------------------------------------------------------------------- multi-GPU: one process per GPU
 // The scan shards by message with no exchange at all (cg_shard_range is the split rule).  The Merkle tree has ONE exchange:
 // every rank's roots of aligned 2^k-leaf blocks are all-gathered and every rank folds the same list.  NCCL is bound at run
@@ -1334,14 +1346,6 @@ void cg_shard_range(uint64_t n, int rank, int world, uint64_t align, uint64_t* l
 }
 
 namespace {
-struct NcclApi {
-  void* h = nullptr; void* comm = nullptr; int rank = 0, world = 1;
-  int (*GetUniqueId)(void*) = nullptr;
-  int (*CommInitRank)(void**, int, cg_nccl_id, int) = nullptr;
-  int (*AllGather)(const void*, void*, size_t, int, void*, cudaStream_t) = nullptr;
-  int (*CommDestroy)(void*) = nullptr;
-  const char* (*GetErrorString)(int) = nullptr;
-} g_nccl;
 int nccl_load() {
   if (g_nccl.h) return CG_OK;
   void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
@@ -1368,7 +1372,7 @@ int cg_comm_unique_id(cg_nccl_id* out) {
 }
 int cg_comm_init(int rank, int world, const cg_nccl_id* id) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
+  if (int rc = require_ready()) return rc;
   if (!id || world < 1 || rank < 0 || rank >= world) return fail(CG_ERR_INVALID_ARG, "bad rank / world / id");
   int rc = nccl_load(); if (rc) return rc;
   if (g_nccl.comm) { g_nccl.CommDestroy(g_nccl.comm); g_nccl.comm = nullptr; }
@@ -1379,59 +1383,45 @@ int cg_comm_init(int rank, int world, const cg_nccl_id* id) {
 void cg_comm_destroy(void) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (g_nccl.comm && g_nccl.CommDestroy) { if (G.ready) cudaStreamSynchronize(G.stream); g_nccl.CommDestroy(g_nccl.comm); }
+  free_shard_roots();
   g_nccl.comm = nullptr; g_nccl.world = 1; g_nccl.rank = 0;
 }
 
 /* Root of the tree over the leaves of ALL ranks (rank r holds leaves [lo_r, hi_r) of cg_shard_range(n_total, r, world, 2^block_log2),
- * device-resident): block roots here, one all-gather of (count, roots) per rank, the same fold on every rank. */
+ * device-resident): block roots here, one all-gather of (count, roots) per rank, the same fold on every rank.  The all-gather runs
+ * outside the library lock (its first call may wait for the peers to connect) on the communicator's root buffer. */
 int cg_merkle_root_sharded_device(const void* d_bytes, uint64_t leaf_len, uint64_t n_local, uint64_t n_total, uint32_t block_log2, uint8_t out_root[32], void* stream) {
+  std::unique_lock<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
   if (!out_root || block_log2 > 40) return fail(CG_ERR_INVALID_ARG, "bad argument");
-  int rank, world; void* comm;
-  { std::lock_guard<std::mutex> lk(g_mu); rank = g_nccl.rank; world = g_nccl.world; comm = g_nccl.comm; }
+  const int rank = g_nccl.rank, world = g_nccl.world; void* const comm = g_nccl.comm;
   if (world > 1 && !comm) return fail(CG_ERR_NOT_INITIALIZED, "cg_comm_init has not been called");
   uint64_t lo, hi; cg_shard_range(n_total, rank, world, 1ull << block_log2, &lo, &hi);
   if (hi - lo != n_local) return fail(CG_ERR_INVALID_ARG, "n_local is not this rank's share of n_total (cg_shard_range with align = 2^block_log2)");
+  if (n_local && !d_bytes) return fail(CG_ERR_INVALID_ARG, "null argument");
   cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
   // every rank contributes max_blocks slots (its own roots first); the counts follow from the split rule, no second exchange
-  uint64_t max_blocks = 0; std::vector<uint64_t> nblk((size_t)world);
-  for (int r = 0; r < world; r++) { uint64_t a, b; cg_shard_range(n_total, r, world, 1ull << block_log2, &a, &b); nblk[(size_t)r] = (b - a + (1ull << block_log2) - 1) >> block_log2; max_blocks = std::max(max_blocks, nblk[(size_t)r]); }
-  if (max_blocks == 0) return cg_merkle_fold(nullptr, 0, out_root);
-  uint8_t *d_mine = nullptr, *d_all = nullptr, *d_real = nullptr, *d_root = nullptr;
-  CU(cudaMalloc((void**)&d_mine, max_blocks * 32)); CU(cudaMalloc((void**)&d_all, (size_t)world * max_blocks * 32)); CU(cudaMalloc((void**)&d_real, (size_t)world * max_blocks * 32 + 32)); CU(cudaMalloc((void**)&d_root, 32));
-  int rc = CG_OK;
-  CU(cudaMemsetAsync(d_mine, 0, max_blocks * 32, st));
-  if (n_local) rc = cg_merkle_block_roots_device(d_bytes, leaf_len, n_local, block_log2, d_mine, st);
-  if (rc == CG_OK) {
-    if (world > 1) { int r = g_nccl.AllGather(d_mine, d_all, max_blocks * 32, /*ncclChar*/ 0, comm, st); if (r) rc = nccl_fail(r, "ncclAllGather"); }
-    else CU(cudaMemcpyAsync(d_all, d_mine, max_blocks * 32, cudaMemcpyDeviceToDevice, st));
+  uint64_t max_blocks = 0, total_blocks = 0; std::vector<uint64_t> nblk((size_t)world);
+  for (int r = 0; r < world; r++) { uint64_t a, b; cg_shard_range(n_total, r, world, 1ull << block_log2, &a, &b); nblk[(size_t)r] = (b - a + (1ull << block_log2) - 1) >> block_log2; max_blocks = std::max(max_blocks, nblk[(size_t)r]); total_blocks += nblk[(size_t)r]; }
+  if (max_blocks == 0) return empty_root(out_root);
+  int rc;
+  if ((rc = grow(&g_nccl.d_roots, &g_nccl.cap_roots, (size_t)world * max_blocks * 8))) return rc;
+  uint32_t* const all = g_nccl.d_roots; uint32_t* const mine = all + (size_t)rank * max_blocks * 8;   // (an in-place all-gather)
+  CU(cudaMemsetAsync(mine, 0, max_blocks * 32, st));
+  if (n_local && (rc = block_roots(d_bytes, leaf_len, n_local, block_log2, mine, st))) return rc;
+  if (world > 1) {
+    lk.unlock(); const int r = g_nccl.AllGather(mine, all, max_blocks * 32, /*ncclChar*/ 0, comm, st); lk.lock();
+    if (r) return nccl_fail(r, "ncclAllGather");
+    // (a cg_shutdown, cg_comm_destroy or other sharded call during the gather is misuse, but must not make the fold read freed memory)
+    if (!G.ready || g_nccl.d_roots != all) return fail(CG_ERR_NOT_INITIALIZED, "the library or the communicator's buffer changed during the all-gather");
   }
-  uint64_t total_blocks = 0;
-  if (rc == CG_OK) {
-    for (int r = 0; r < world; r++) { if (nblk[(size_t)r]) CU(cudaMemcpyAsync(d_real + total_blocks * 32, d_all + (size_t)r * max_blocks * 32, nblk[(size_t)r] * 32, cudaMemcpyDeviceToDevice, st)); total_blocks += nblk[(size_t)r]; }
-    rc = cg_merkle_fold_device(d_real, total_blocks, d_root, st);
-  }
-  if (rc == CG_OK) { CU(cudaMemcpyAsync(out_root, d_root, 32, cudaMemcpyDeviceToHost, st)); CU(cudaStreamSynchronize(st)); }
-  cudaFree(d_mine); cudaFree(d_all); cudaFree(d_real); cudaFree(d_root);
-  return rc;
-}
-
-int cg_merkle_fold(const uint8_t* nodes32, uint64_t m, uint8_t out_root[32]) {
-  {
-    std::lock_guard<std::mutex> lk(g_mu);
-    if (!G.ready) return fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)");
-    if (!out_root) return fail(CG_ERR_INVALID_ARG, "null argument");
-    if (m == 0) return empty_root(out_root);
-    if (!nodes32) return fail(CG_ERR_INVALID_ARG, "null argument");
-    int rc;
-    if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)m * 8))) return rc;
-    if ((rc = grow(&G.d_dig[1], &G.cap_dig[1], (size_t)(m + 1) / 2 * 8 + 8))) return rc;
-    cudaStream_t st = G.stream;
-    CU(cudaMemcpyAsync(G.d_dig[0], nodes32, m * 32, cudaMemcpyHostToDevice, st));
-    int cur = fold_levels(m, 1, 0, st);
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(out_root, G.d_dig[cur], 32, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-  }
+  const uint32_t* d_root;                                   // the fold's input: the gathered roots without the empty slots
+  if ((rc = size_dig(total_blocks))) return rc;
+  uint32_t* d = G.d_dig[0];
+  for (int r = 0; r < world; r++) if (nblk[(size_t)r]) { CU(cudaMemcpyAsync(d, all + (size_t)r * max_blocks * 8, nblk[(size_t)r] * 32, cudaMemcpyDeviceToDevice, st)); d += nblk[(size_t)r] * 8; }
+  if ((rc = fold_dig(G.d_dig[0], total_blocks, 64, st, &d_root))) return rc;
+  CU(cudaMemcpyAsync(out_root, d_root, 32, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   return CG_OK;
 }
 

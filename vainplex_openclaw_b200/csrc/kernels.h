@@ -125,9 +125,9 @@ int launch_merkle_leaves_var(const uint8_t* d_bytes, const uint64_t* d_off, uint
 int launch_newline_split(const uint8_t* d_bytes, uint64_t len, uint32_t* d_piece_counts, uint64_t* d_total_lines, cudaStream_t stream);
 int launch_newline_starts(const uint8_t* d_bytes, uint64_t len, const uint32_t* d_piece_rank, uint64_t* d_starts, uint64_t n_lines, cudaStream_t stream);
 int launch_merkle_consistency(uint64_t first, uint64_t second, const uint32_t* d_first32, const uint32_t* d_second32, const uint32_t* d_path, uint32_t path_len, uint32_t* d_ok, cudaStream_t stream);
-// one tree level: out[i] = node(in[2i], in[2i+1]) ; an unpaired last node is copied
-int launch_merkle_level(const uint32_t* d_in, uint64_t n_in, uint32_t* d_out, cudaStream_t stream);
-// reduce `levels` (1..5) tree levels inside one kernel: every aligned group of 2^levels nodes -> its root (warp shuffles)
-int launch_merkle_reduce(const uint32_t* d_in, uint64_t n_in, uint32_t levels, uint32_t* d_out, cudaStream_t stream);
+// fold the n nodes at d_in (16-byte aligned) level by level until one is left or max_levels levels are done; the first level
+// writes d_a, later ones d_b, d_a, ...; only the first reads d_in (d_b may be d_in).  *d_result = the folded nodes.
+int launch_merkle_fold(const uint32_t* d_in, uint64_t n, uint32_t max_levels, uint32_t* d_a, uint32_t* d_b, cudaStream_t stream,
+                       const uint32_t** d_result);
 
 }  // namespace cg

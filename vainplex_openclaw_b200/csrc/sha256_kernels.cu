@@ -505,17 +505,33 @@ int launch_merkle_leaves_var(const uint8_t* d_bytes, const uint64_t* d_off, uint
   merkle_leaves_var_kernel<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(d_bytes, d_off, n, d_out, trim_newline ? 1 : 0);
   return 1;
 }
-int launch_merkle_level(const uint32_t* d_in, uint64_t n_in, uint32_t* d_out, cudaStream_t stream) {
+static int launch_merkle_level(const uint32_t* d_in, uint64_t n_in, uint32_t* d_out, cudaStream_t stream) {
   uint64_t n_out = (n_in + 1) / 2;
   if (!n_out) return 0;
   merkle_level_kernel<<<(unsigned)((n_out + 127) / 128), 128, 0, stream>>>(d_in, n_in, d_out);
   return 1;
 }
-int launch_merkle_reduce(const uint32_t* d_in, uint64_t n_in, uint32_t levels, uint32_t* d_out, cudaStream_t stream) {
+static int launch_merkle_reduce(const uint32_t* d_in, uint64_t n_in, uint32_t levels, uint32_t* d_out, cudaStream_t stream) {
   if (!n_in || levels == 0 || levels > 5) return 0;
   const uint64_t n_groups = (n_in + (1ull << levels) - 1) >> levels, warps = (n_groups + (32u >> levels) - 1) / (32u >> levels);
   merkle_reduce_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, stream>>>(d_in, n_in, levels, d_out);
   return 1;
+}
+// Above 2^15 nodes a level is one launch of merkle_level_kernel (every lane busy); from 2^15 nodes down merkle_reduce_kernel
+// folds min(5, levels left under max_levels, ceil(log2 n)) levels per launch, where a launch costs more than idle lanes do.
+int launch_merkle_fold(const uint32_t* d_in, uint64_t n, uint32_t max_levels, uint32_t* d_a, uint32_t* d_b, cudaStream_t stream,
+                       const uint32_t** d_result) {
+  int k = 0;
+  const uint32_t* src = d_in; uint32_t* dst = d_a;
+  for (uint32_t lv = 0; n > 1 && lv < max_levels;) {
+    uint32_t step = 1;
+    if (n <= (1u << 15)) { step = std::min(5u, max_levels - lv); while (step > 1 && (1ull << (step - 1)) >= n) step--; }
+    k += step > 1 ? launch_merkle_reduce(src, n, step, dst, stream) : launch_merkle_level(src, n, dst, stream);
+    n = (n + (1ull << step) - 1) >> step; lv += step;
+    src = dst; dst = dst == d_a ? d_b : d_a;
+  }
+  *d_result = src;
+  return k;
 }
 
 }  // namespace cg
