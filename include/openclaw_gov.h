@@ -165,8 +165,25 @@ CG_API int cg_redact_batch(cg_ruleset *rs, const uint8_t *bytes, const uint32_t 
  * CG_ERR_CAPACITY once: scan that batch again.  (cg_scan_batch, the host-buffer call, retries by itself.) */
 CG_API int cg_scan_batch_device(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, uint32_t n,
                                 void *d_out_words, void *stream);
-/* Waits for `stream` and returns the status of every device-path batch issued since the previous join: CG_OK,
- * CG_ERR_CAPACITY (see above) or CG_ERR_TOO_LARGE (the VM ran out of thread-list space; words all ones as well). */
+/* findMatches + resolveOverlaps for a batch in HBM.  Same input rules as cg_scan_batch_device (d_bytes 16-byte aligned,
+ * readable 16 bytes past offsets[n]).  d_out_spans: cg_span[spans_cap] (may be NULL when spans_cap is 0); d_out_nspans: one
+ * uint32 = resolved spans of the batch.  Asynchronous and in order on `stream` like cg_scan_batch_device; its status comes
+ * from cg_scan_join: CG_ERR_CAPACITY when the batch has more than spans_cap spans (the first spans_cap are written), or when
+ * an internal queue overflowed (then *d_out_nspans = 0xffffffff, nothing is written, the scratch grows: issue it again). */
+CG_API int cg_find_matches_batch_device(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, uint32_t n,
+                                        void *d_out_spans, uint32_t spans_cap, void *d_out_nspans, void *stream);
+/* RedactionEngine.scanString for a batch in HBM (cg_redact_batch's packing and placeholder).  d_out_bytes: out_cap bytes;
+ * d_out_offsets: uint32[n+1]; d_out_spans: cg_span[spans_cap]; d_out_digests32: 32 bytes per span, 16-byte aligned;
+ * d_out_sizes: uint64[2] = {output bytes needed, resolved spans}, 8-byte aligned.  Sizes and offsets are always written;
+ * spans, digests and output bytes only while they fit (no byte past out_cap or spans_cap is ever written).  cg_scan_join
+ * reports CG_ERR_CAPACITY when they did not (issue again with the sizes), CG_ERR_TOO_LARGE for 4 GiB of output or more, and
+ * CG_ERR_CAPACITY once after an internal queue overflow (both sizes = ~0, nothing else written; issue the batch again). */
+CG_API int cg_redact_batch_device(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, uint32_t n,
+                                  void *d_out_bytes, uint64_t out_cap, void *d_out_offsets,
+                                  void *d_out_spans, uint32_t spans_cap, void *d_out_digests32, void *d_out_sizes, void *stream);
+/* Waits for `stream` and returns the status of every device-path batch (scan, find-matches, redact) issued since the
+ * previous join: CG_OK, CG_ERR_CAPACITY (see above) or CG_ERR_TOO_LARGE (the VM ran out of thread-list space; words all
+ * ones as well; or a redacted batch of 4 GiB or more). */
 CG_API int cg_scan_join(cg_ruleset *rs, void *stream);
 
 /* ---- SHA-256.  Replaces createHash("sha256").update(s).digest() at src/util.ts:77-79,

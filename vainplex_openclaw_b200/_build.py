@@ -7,7 +7,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libopenclaw_gov.so")
-SOURCES = ["capi.cu", "scan_kernels.cu", "sha256_kernels.cu", "rulec.cpp", "ruleset_image.cpp"]
+SOURCES = ["capi.cu", "scan_kernels.cu", "span_resolve.cu", "sha256_kernels.cu", "rulec.cpp", "ruleset_image.cpp"]
 HEADERS = ["kernels.h", "rulec.h", "pike_vm.h", "gram_filter.h", "ruleset_image.h", os.path.join("..", "..", "include", "openclaw_gov.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared"]

@@ -54,7 +54,7 @@ EXPORTS = ["cg_init", "cg_shutdown", "cg_last_error", "cg_version", "cg_device_c
            "cg_merkle_log_append_jsonl", "cg_merkle_log_consistency", "cg_merkle_verify_consistency", "cg_merkle_log_reserve",
            "cg_shard_range", "cg_comm_unique_id", "cg_comm_init", "cg_comm_destroy", "cg_merkle_root_sharded_device",
            "cg_ruleset_create", "cg_ruleset_destroy", "cg_ruleset_get_info", "cg_rule_check", "cg_scan_batch",
-           "cg_scan_one", "cg_find_matches_batch", "cg_scan_batch_device", "cg_sha256_batch", "cg_merkle_root",
+           "cg_scan_one", "cg_find_matches_batch", "cg_scan_batch_device", "cg_find_matches_batch_device", "cg_redact_batch_device", "cg_sha256_batch", "cg_merkle_root",
            "cg_merkle_root_fixed", "cg_merkle_block_roots_device", "cg_merkle_fold", "cg_merkle_fold_device"]
 
 _lib = None
@@ -117,6 +117,8 @@ def load():
     L.cg_scan_one.argtypes = [vp, vp, u32, C.POINTER(u64), vp, u32, C.POINTER(u32)]; L.cg_scan_one.restype = i32
     L.cg_find_matches_batch.argtypes = [vp, vp, vp, u32, vp, u32, C.POINTER(u32)]; L.cg_find_matches_batch.restype = i32
     L.cg_scan_batch_device.argtypes = [vp, vp, vp, u32, vp, vp]; L.cg_scan_batch_device.restype = i32
+    L.cg_find_matches_batch_device.argtypes = [vp, vp, vp, u32, vp, u32, vp, vp]; L.cg_find_matches_batch_device.restype = i32
+    L.cg_redact_batch_device.argtypes = [vp, vp, vp, u32, vp, u64, vp, vp, u32, vp, vp, vp]; L.cg_redact_batch_device.restype = i32
     L.cg_sha256_batch.argtypes = [vp, vp, u32, vp]; L.cg_sha256_batch.restype = i32
     L.cg_merkle_root.argtypes = [vp, vp, u64, vp]; L.cg_merkle_root.restype = i32
     L.cg_merkle_root_fixed.argtypes = [vp, u64, u64, vp]; L.cg_merkle_root_fixed.restype = i32
@@ -282,6 +284,19 @@ class Ruleset:
 
     def scan_batch_device(self, d_bytes: int, d_off: int, n: int, d_words: int, stream: int = 0):
         check(load().cg_scan_batch_device(self.handle, d_bytes, d_off, n, d_words, stream))
+
+    def find_matches_batch_device(self, d_bytes: int, d_off: int, n: int, d_spans: int, spans_cap: int, d_nspans: int, stream: int = 0):
+        """cg_find_matches_batch_device on raw device pointers (asynchronous; status from scan_join): resolved spans
+        (SPAN_DTYPE, at most spans_cap) into d_spans, their number (uint32) into d_nspans."""
+        check(load().cg_find_matches_batch_device(self.handle, d_bytes, d_off, n, d_spans or None, spans_cap, d_nspans, stream))
+
+    def redact_batch_device(self, d_bytes: int, d_off: int, n: int, d_out: int, out_cap: int, d_out_off: int, d_spans: int,
+                            spans_cap: int, d_digests: int, d_sizes: int, stream: int = 0):
+        """cg_redact_batch_device on raw device pointers (asynchronous; status from scan_join): redacted bytes into d_out,
+        offsets (uint32[n+1]) into d_out_off, spans and their SHA-256 (32 bytes each) into d_spans / d_digests, and
+        uint64[2] = (bytes needed, resolved spans) into d_sizes."""
+        check(load().cg_redact_batch_device(self.handle, d_bytes, d_off, n, d_out or None, out_cap, d_out_off, d_spans or None,
+                                            spans_cap, d_digests or None, d_sizes, stream))
 
 
 def sha256_batch(data: np.ndarray, off64: np.ndarray) -> np.ndarray:

@@ -43,7 +43,8 @@ struct Ctx {
   // chunked host-buffer scans: H2D of chunk c+1 and D2H of chunk c-1 overlap the kernels of chunk c
   static constexpr int kChunks = 8;
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr; cudaEvent_t e_h2d[kChunks] = {}, e_done[kChunks] = {}; uint32_t* h_chunk_counters = nullptr;
-  // cg_redact_batch / cg_policy_verdict_batch staging (grow-only)
+  // cg_find_matches_batch / cg_redact_batch / cg_policy_verdict_batch staging (grow-only)
+  cg_span* d_spans = nullptr; size_t cap_spans = 0;
   uint8_t* d_redact_out = nullptr; size_t cap_redact_out = 0; uint32_t* d_redact_meta = nullptr; size_t cap_redact_meta = 0;
   uint32_t* d_verdicts = nullptr; size_t cap_verdicts = 0;
 } G;
@@ -110,6 +111,7 @@ struct cg_ruleset {
   uint32_t* h_counters = nullptr; cudaEvent_t e_cnt[kMirror] = {}; bool cnt_pending[kMirror] = {};
   uint32_t grow_l1 = 0, grow_slot = 0, grow_ev = 0, grow_span = 0;     // capacities learnt from overflows
   uint32_t sticky_flags = 0;      // error flags of batches since the last cg_scan_join
+  uint32_t sticky_status = 0;     // 1 << span resolution status (kResolve*) of batches since the last cg_scan_join
   // verify_small_kernel's grid (CTAs per SM): one while the island matcher decides (nearly) everything, four once a step has
   // sent more than 2048 pairs to the VM (non-ASCII traffic); back to one below 256.  Part of the cached graphs' keys.
   int verify_ctas = 1;
@@ -133,6 +135,8 @@ struct cg_ruleset {
     for (void* p : allocs) cudaFree(p);
     cudaFree(work.heavy_idx); cudaFree(work.l1_pos); cudaFree(work.l1_fac); cudaFree(work.fq); cudaFree(work.slot_of_msg);
     cudaFree(work.counters); cudaFree(work.persist); cudaFree(work.slot_msg); cudaFree(work.cand); cudaFree(work.hit); cudaFree(work.events); cudaFree(work.event_pos); cudaFree(work.event_pre); cudaFree(work.spans);
+    cudaFree(work.words); cudaFree(work.seg_cnt); cudaFree(work.seg_begin); cudaFree(work.kept_cnt); cudaFree(work.kept_begin); cudaFree(work.out_len); cudaFree(work.out_off);
+    cudaFree(work.sorted); cudaFree(work.sort_tmp); cudaFree(work.sp_start); cudaFree(work.sp_len); cudaFree(work.sp_cat); cudaFree(work.scan_part);
   }
 };
 
@@ -150,7 +154,8 @@ int upload(cg_ruleset* rs, const std::vector<T>& v, const T** out, size_t pad_el
   return CG_OK;
 }
 
-int ensure_work(cg_ruleset* rs, ScanWork& w, uint32_t n_msgs, uint32_t l1_cap, uint32_t slot_cap, uint32_t event_cap, uint32_t span_cap) {
+// (res_msgs: messages the span resolver must have room for; 0 for a step without spans)
+int ensure_work(cg_ruleset* rs, ScanWork& w, uint32_t n_msgs, uint32_t l1_cap, uint32_t slot_cap, uint32_t event_cap, uint32_t span_cap, uint32_t res_msgs) {
   rs->scratch_gen++;                                        // (prepare_step calls this only when some buffer must grow)
   if (!w.counters) { CU(cudaMalloc((void**)&w.counters, kCounterWords * sizeof(uint32_t))); CU(cudaMalloc((void**)&w.persist, 16)); CU(cudaMemset(w.persist, 0, 16)); CU(cudaDeviceSynchronize()); }
   if (n_msgs > w.msg_cap) { cudaFree(w.slot_of_msg); w.slot_of_msg = nullptr; w.msg_cap = 0; CU(cudaMalloc((void**)&w.slot_of_msg, (size_t)n_msgs * 4)); w.msg_cap = n_msgs; }
@@ -170,7 +175,23 @@ int ensure_work(cg_ruleset* rs, ScanWork& w, uint32_t n_msgs, uint32_t l1_cap, u
     w.slot_cap = slot_cap;
   }
   if (event_cap > w.event_cap) { cudaFree(w.events); cudaFree(w.event_pos); cudaFree(w.event_pre); cudaFree(w.heavy_idx); w.events = nullptr; w.event_pos = w.event_pre = w.heavy_idx = nullptr; w.event_cap = 0; CU(cudaMalloc((void**)&w.events, (size_t)event_cap * sizeof(uint2))); CU(cudaMalloc((void**)&w.heavy_idx, (size_t)event_cap * 4)); CU(cudaMalloc((void**)&w.event_pos, (size_t)event_cap * 4)); CU(cudaMalloc((void**)&w.event_pre, (size_t)event_cap * 4)); w.event_cap = event_cap; }
-  if (span_cap > w.span_cap) { cudaFree(w.spans); w.spans = nullptr; w.span_cap = 0; CU(cudaMalloc((void**)&w.spans, (size_t)span_cap * 24)); w.span_cap = span_cap; }
+  if (span_cap > w.span_cap) {
+    cudaFree(w.spans); cudaFree(w.sorted); cudaFree(w.sort_tmp); cudaFree(w.sp_start); cudaFree(w.sp_len); cudaFree(w.sp_cat);
+    w.spans = w.sp_start = w.sp_len = w.sp_cat = nullptr; w.sorted = w.sort_tmp = nullptr; w.span_cap = 0;
+    CU(cudaMalloc((void**)&w.spans, (size_t)span_cap * 24));
+    CU(cudaMalloc((void**)&w.sorted, (size_t)span_cap * 16)); CU(cudaMalloc((void**)&w.sort_tmp, (size_t)span_cap * 16));
+    CU(cudaMalloc((void**)&w.sp_start, (size_t)span_cap * 4)); CU(cudaMalloc((void**)&w.sp_len, (size_t)span_cap * 4)); CU(cudaMalloc((void**)&w.sp_cat, (size_t)span_cap * 4));
+    w.span_cap = span_cap;
+  }
+  if (res_msgs > w.res_cap || (res_msgs && !w.scan_part)) {
+    cudaFree(w.words); cudaFree(w.seg_cnt); cudaFree(w.seg_begin); cudaFree(w.kept_cnt); cudaFree(w.kept_begin); cudaFree(w.out_len); cudaFree(w.out_off);
+    w.words = w.out_len = w.out_off = nullptr; w.seg_cnt = w.seg_begin = w.kept_cnt = w.kept_begin = nullptr; w.res_cap = 0;
+    const size_t m = (size_t)res_msgs + 1;
+    CU(cudaMalloc((void**)&w.words, m * 8)); CU(cudaMalloc((void**)&w.out_len, m * 8)); CU(cudaMalloc((void**)&w.out_off, m * 8));
+    CU(cudaMalloc((void**)&w.seg_cnt, m * 4)); CU(cudaMalloc((void**)&w.seg_begin, m * 4)); CU(cudaMalloc((void**)&w.kept_cnt, m * 4)); CU(cudaMalloc((void**)&w.kept_begin, m * 4));
+    if (!w.scan_part) CU(cudaMalloc((void**)&w.scan_part, (size_t)kScanPartials * 8));
+    w.res_cap = res_msgs;
+  }
   return CG_OK;
 }
 
@@ -223,9 +244,10 @@ int prepare_step(cg_ruleset* rs, uint32_t n, bool spans, cudaStream_t st) {
   uint32_t l1, slot, ev, span;
   default_caps(rs, n, spans, &l1, &slot, &ev, &span);
   n = std::max<uint32_t>(n, 1);
-  if (n <= w.msg_cap && l1 <= w.l1_cap && slot <= w.slot_cap && ev <= w.event_cap && span <= w.span_cap) return CG_OK;
+  const uint32_t res = spans ? n : 0;
+  if (n <= w.msg_cap && l1 <= w.l1_cap && slot <= w.slot_cap && ev <= w.event_cap && span <= w.span_cap && res <= w.res_cap) return CG_OK;
   CU(cudaStreamSynchronize(st));
-  return ensure_work(rs, rs->work, n, l1, slot, ev, span);
+  return ensure_work(rs, rs->work, n, l1, slot, ev, span, res);
 }
 // fq is cut into four equal pieces at most: the fullest piece decides
 static uint32_t queue_need(const uint32_t* hc) { uint32_t m = 0; for (int i = 24; i < 28; i++) m = std::max(m, hc[i]); return m > 0xffffffffu / scan_pieces() ? 0xffffffffu : scan_pieces() * m; }
@@ -279,7 +301,7 @@ int check_offsets(const uint32_t* offsets, uint32_t n) {
   return CG_OK;
 }
 
-// full host-buffer scan with capacity retry; leaves words in G.d_words
+// full host-buffer scan with capacity retry; leaves words in G.d_words (a span-mode step: in the rule set's scratch)
 int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, bool spans, HostScan* hs) {
   if (int rc = require_ready()) return rc;
   if (!rs || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
@@ -299,7 +321,7 @@ int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uin
   for (int attempt = 0; attempt < 10; attempt++) {
     if ((rc = prepare_step(rs, n, spans, st))) return rc;
     CU(cudaEventRecord(G.ev0, st));
-    if (n) { if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32, n, G.d_words, spans, st))) return rc; }
+    if (n) { if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32, n, spans ? rs->work.words : G.d_words, spans, st))) return rc; }
     else CU(cudaMemsetAsync(rs->work.counters, 0, kCounterWords * sizeof(uint32_t), st));
     CU(cudaEventRecord(G.ev1, st));
     CU(cudaMemcpyAsync(hs->counters.data(), rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
@@ -385,8 +407,27 @@ void poll_mirrors(cg_ruleset* rs, bool wait) {
     rs->cnt_pending[i] = false;
     const uint32_t* hc = rs->h_counters + (size_t)i * kCounterWords;
     rs->sticky_flags |= hc[3];
+    if (!hc[3]) rs->sticky_status |= hc[16] ? 1u << hc[16] : 0u;
+    G.stats.spans += hc[20]; G.stats.sha256_items += hc[21];     // (zero for words-only steps)
     absorb_counters(rs, hc);                                // (cg_scan_join reports the flags)
   }
+}
+
+// device path: the pinned counter mirror ring (allocated by the first device-path call)
+int ensure_mirrors(cg_ruleset* rs) {
+  if (rs->h_counters) return CG_OK;
+  CU(cudaMallocHost((void**)&rs->h_counters, (size_t)cg_ruleset::kMirror * kCounterWords * 4));
+  for (auto& e : rs->e_cnt) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  return CG_OK;
+}
+// device path: copy the counter block of the batch just enqueued on st into the next mirror slot
+int mirror_counters(cg_ruleset* rs, cudaStream_t st) {
+  const int slot = (int)(rs->seq % cg_ruleset::kMirror);
+  if (rs->cnt_pending[slot]) { cudaEventSynchronize(rs->e_cnt[slot]); poll_mirrors(rs, false); }
+  CU(cudaMemcpyAsync(rs->h_counters + (size_t)slot * kCounterWords, rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaEventRecord(rs->e_cnt[slot], st));
+  rs->cnt_pending[slot] = true; rs->seq++;
+  return CG_OK;
 }
 
 }  // namespace
@@ -426,7 +467,7 @@ void cg_shutdown(void) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!G.ready) return;
   cudaDeviceSynchronize();
-  cudaFree(G.d_redact_out); cudaFree(G.d_redact_meta); cudaFree(G.d_verdicts);
+  cudaFree(G.d_spans); cudaFree(G.d_redact_out); cudaFree(G.d_redact_meta); cudaFree(G.d_verdicts);
   if (G.h_chunk_counters) cudaFreeHost(G.h_chunk_counters);
   if (G.s_h2d) { cudaStreamDestroy(G.s_h2d); cudaStreamDestroy(G.s_d2h); for (int c = 0; c < Ctx::kChunks; c++) { cudaEventDestroy(G.e_h2d[c]); cudaEventDestroy(G.e_done[c]); } }
   cudaFree(G.d_bytes_raw); cudaFree(G.d_off32); cudaFree(G.d_off64); cudaFree(G.d_words); cudaFree(G.d_dig[0]); cudaFree(G.d_dig[1]);
@@ -558,6 +599,15 @@ int cg_ruleset_create(const cg_rule* rules, uint32_t n_rules, uint32_t options, 
   { const uint64_t* fs = nullptr; if ((rc = upload(rs.get(), H.factor_skip, &fs, 8))) return rc; d.factor_skip = getenv("CG_NO_SKIP") ? nullptr : reinterpret_cast<const unsigned long long*>(fs); }
   if (getenv("CG_NO_BITPROG")) d.bit_words = nullptr;
   d.rule_policy = nullptr; d.rule_action = nullptr;
+  {
+    // the span resolver's tie-break: rank of every rule in (category, rule) order
+    std::vector<uint32_t> order(n_rules), rank(n_rules);
+    for (uint32_t i = 0; i < n_rules; i++) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return rs->category[a] < rs->category[b]; });
+    for (uint32_t i = 0; i < n_rules; i++) rank[order[i]] = i;
+    if ((rc = upload(rs.get(), rs->category, &rs->work.rule_category))) return rc;
+    if ((rc = upload(rs.get(), rank, &rs->work.rule_rank))) return rc;
+  }
   d.n_rules = n_rules; d.rw = (n_rules + 31) / 32; if (d.rw == 0) d.rw = 1;
   d.max_prog_len = 0; for (uint32_t i = 0; i < n_rules; i++) d.max_prog_len = std::max(d.max_prog_len, prog_off[i + 1] - prog_off[i]);
   prepare_kernels();
@@ -681,48 +731,42 @@ int cg_scan_one(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* ou
 }
 
 namespace {
-// findMatches + resolveOverlaps for a batch: resolved spans sorted by (msg, start).  Leaves the input in G.d_bytes / G.d_off32.
-int find_matches_resolved(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, std::vector<cg_span>* out) {
+// findMatches + resolveOverlaps for a host batch: scan_host (with its retries), then the span resolver on the library stream.
+// Resolved spans land in G.d_spans; redacting, G.d_redact_meta holds [sizes, 4 words][out offsets, n + 1][digests, 16-byte
+// aligned, room for every raw span] and *out_offsets the output offsets.  *ns = resolved spans, *need = redacted bytes.
+// Leaves the input in G.d_bytes / G.d_off32.
+int resolve_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, bool redact, uint32_t* out_offsets,
+                 uint32_t* ns, uint64_t* need, uint32_t** d_digests) {
   HostScan hs;
   int rc = scan_host(rs, bytes, offsets, n, true, &hs);
   if (rc) return rc;
-  uint32_t ns = hs.counters[2];
-  std::vector<cg_span> raw(ns);
-  if (ns) { CU(cudaMemcpyAsync(raw.data(), rs->work.spans, (size_t)ns * 24, cudaMemcpyDeviceToHost, G.stream)); CU(cudaStreamSynchronize(G.stream)); }
-  // collection order of findMatches (registry.ts:216-236): category order, storage order, position
-  const std::vector<uint32_t>& cat = rs->category;
-  std::sort(raw.begin(), raw.end(), [&](const cg_span& a, const cg_span& b) {
-    if (a.msg != b.msg) return a.msg < b.msg;
-    if (cat[a.rule] != cat[b.rule]) return cat[a.rule] < cat[b.rule];
-    if (a.rule != b.rule) return a.rule < b.rule;
-    return a.start16 < b.start16;
-  });
-  // resolveOverlaps (registry.ts:288-316): stable sort by start asc, length desc, category order; greedy keep
-  out->clear();
-  for (size_t i = 0; i < raw.size();) {
-    size_t j = i; while (j < raw.size() && raw[j].msg == raw[i].msg) j++;
-    std::stable_sort(raw.begin() + i, raw.begin() + j, [&](const cg_span& a, const cg_span& b) {
-      if (a.start16 != b.start16) return a.start16 < b.start16;
-      uint32_t la = a.end16 - a.start16, lb = b.end16 - b.start16;
-      if (la != lb) return la > lb;
-      return cat[a.rule] < cat[b.rule];
-    });
-    int64_t last_end = -1;
-    for (size_t k = i; k < j; k++) if ((int64_t)raw[k].start16 >= last_end) { out->push_back(raw[k]); last_end = raw[k].end16; }
-    i = j;
-  }
-  G.stats.spans += out->size();
+  const ScanWork& w = rs->work;
+  cudaStream_t st = G.stream;
+  const size_t dig_at = ((size_t)n + 1 + 4 + 3) & ~(size_t)3;
+  if ((rc = grow(&G.d_spans, &G.cap_spans, (size_t)w.span_cap))) return rc;
+  if ((rc = grow(&G.d_redact_meta, &G.cap_redact_meta, dig_at + (redact ? (size_t)w.span_cap * 8 : 0)))) return rc;
+  uint32_t* d_sizes = G.d_redact_meta; uint32_t* d_out_off = G.d_redact_meta + 4;
+  *d_digests = G.d_redact_meta + dig_at;
+  const SpanOutputs o{reinterpret_cast<uint32_t*>(G.d_spans), w.span_cap, d_out_off, ~0ull, d_sizes, redact};
+  count_launches(launch_span_resolve(w, G.d_off32, n, o, G.sm_count, st));
+  CU(cudaGetLastError());
+  uint64_t sizes[2] = {0, 0};
+  CU(cudaMemcpyAsync(sizes, d_sizes, redact ? 16 : 4, cudaMemcpyDeviceToHost, st));
+  if (redact) CU(cudaMemcpyAsync(out_offsets, d_out_off, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  *ns = redact ? (uint32_t)sizes[1] : (uint32_t)sizes[0]; *need = redact ? sizes[0] : 0;
+  G.stats.spans += *ns;
   return CG_OK;
 }
 }  // namespace
 
 int cg_find_matches_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans) {
   std::lock_guard<std::mutex> lk(g_mu);
-  std::vector<cg_span> res;
-  int rc = find_matches_resolved(rs, bytes, offsets, n, &res);
+  uint32_t outn = 0; uint64_t need = 0; uint32_t* d_dig = nullptr;
+  int rc = resolve_host(rs, bytes, offsets, n, false, nullptr, &outn, &need, &d_dig);
   if (rc) return rc;
-  const uint32_t outn = (uint32_t)res.size();
-  if (out_spans) memcpy(out_spans, res.data(), (size_t)std::min(outn, spans_cap) * sizeof(cg_span));
+  const uint32_t k = std::min(outn, spans_cap);
+  if (out_spans && k) { CU(cudaMemcpyAsync(out_spans, G.d_spans, (size_t)k * sizeof(cg_span), cudaMemcpyDeviceToHost, G.stream)); CU(cudaStreamSynchronize(G.stream)); }
   if (out_nspans) *out_nspans = outn;
   if (out_spans && outn > spans_cap) return fail(CG_ERR_CAPACITY, "out_spans too small");
   return CG_OK;
@@ -770,49 +814,24 @@ int cg_redact_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offset
                     uint64_t* out_need, uint32_t* out_offsets, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans, uint8_t* out_digests32) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!out_offsets || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
-  std::vector<cg_span> res;
-  int rc = find_matches_resolved(rs, bytes, offsets, n, &res);            // input bytes / offsets stay in G.d_bytes / G.d_off32
+  uint32_t ns = 0; uint64_t pos = 0; uint32_t* d_dig = nullptr;
+  int rc = resolve_host(rs, bytes, offsets, n, true, out_offsets, &ns, &pos, &d_dig);     // input bytes / offsets stay in G.d_bytes / G.d_off32
   if (rc) return rc;
-  const uint32_t ns = (uint32_t)res.size();
-  static const uint32_t kCatLen[4] = {10, 9, 3, 6};                         // credential, financial, pii, custom
-  // host: output offsets and the per-message span index (O(n + spans)); device: digests and the splice itself
-  std::vector<uint32_t> span_begin((size_t)n + 1), span_start(ns), span_len(ns), span_cat(ns);
-  uint64_t pos = 0; uint32_t k = 0;
-  for (uint32_t m = 0; m < n; m++) {
-    span_begin[m] = k; out_offsets[m] = (uint32_t)pos;
-    uint64_t len = offsets[m + 1] - offsets[m];
-    for (; k < ns && res[k].msg == m; k++) {
-      span_start[k] = offsets[m] + res[k].start_byte; span_len[k] = res[k].end_byte - res[k].start_byte; span_cat[k] = rs->category[res[k].rule] & 3u;
-      len = len - span_len[k] + 20u + kCatLen[span_cat[k]];
-    }
-    pos += len;
-  }
-  span_begin[n] = k; out_offsets[n] = (uint32_t)pos;
   if (out_need) *out_need = pos;
   if (out_nspans) *out_nspans = ns;
   if (pos >> 32) return fail(CG_ERR_TOO_LARGE, "redacted batch exceeds 4 GiB");
   if ((out_spans && ns > spans_cap) || pos > out_cap || !out_bytes) return fail(CG_ERR_CAPACITY, "output buffer too small (see *out_need / *out_nspans)");
-  if (out_spans) memcpy(out_spans, res.data(), (size_t)ns * sizeof(cg_span));
   cudaStream_t st = G.stream;
   if ((rc = grow(&G.d_redact_out, &G.cap_redact_out, (size_t)pos + 64))) return rc;
   uint8_t* d_out = G.d_redact_out;
-  const size_t meta_words = 2 * ((size_t)n + 1) + 3 * (size_t)ns + 8 * (size_t)ns + 16;
-  if ((rc = grow(&G.d_redact_meta, &G.cap_redact_meta, meta_words))) return rc;
-  uint32_t* d_meta = G.d_redact_meta;
-  uint32_t* d_out_off = d_meta; uint32_t* d_span_begin = d_out_off + n + 1; uint32_t* d_start = d_span_begin + n + 1;
-  uint32_t* d_len = d_start + ns; uint32_t* d_cat = d_len + ns; uint32_t* d_dig = d_cat + ns; d_dig += (8 - ((d_dig - d_meta) & 7)) & 7;   // 32-byte aligned digests
-  CU(cudaMemcpyAsync(d_out_off, out_offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d_span_begin, span_begin.data(), ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
-  if (ns) {
-    CU(cudaMemcpyAsync(d_start, span_start.data(), (size_t)ns * 4, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d_len, span_len.data(), (size_t)ns * 4, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d_cat, span_cat.data(), (size_t)ns * 4, cudaMemcpyHostToDevice, st));
-  }
-  int kl = launch_redact_digests(G.d_bytes, d_start, d_len, ns, d_dig, st);
-  kl += launch_redact_splice(G.d_bytes, G.d_off32, d_out_off, d_span_begin, d_start, d_len, d_cat, d_dig, d_out, n, G.sm_count, st);
+  // device: digests and the splice itself, over the resolver's per-span arrays; it set their counts (counters[21], [22])
+  const ScanWork& w = rs->work;
+  int kl = launch_redact_digests(G.d_bytes, w.sp_start, w.sp_len, w.counters + 21, d_dig, G.sm_count, st);
+  kl += launch_redact_splice(G.d_bytes, G.d_off32, G.d_redact_meta + 4, w.kept_begin, w.sp_start, w.sp_len, w.sp_cat, d_dig, d_out, w.counters + 22, n, G.sm_count, st);
   count_launches(kl); G.stats.sha256_items += ns;
   CU(cudaGetLastError());
   if (pos) CU(cudaMemcpyAsync(out_bytes, d_out, (size_t)pos, cudaMemcpyDeviceToHost, st));
+  if (ns && out_spans) CU(cudaMemcpyAsync(out_spans, G.d_spans, (size_t)ns * sizeof(cg_span), cudaMemcpyDeviceToHost, st));
   if (ns && out_digests32) CU(cudaMemcpyAsync(out_digests32, d_dig, (size_t)ns * 32, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
@@ -827,10 +846,7 @@ int cg_scan_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offs
   if (!n) return CG_OK;
   static const bool use_graph = !(getenv("CG_NO_GRAPH") && atoi(getenv("CG_NO_GRAPH")));
   int rc;
-  if (!rs->h_counters) {
-    CU(cudaMallocHost((void**)&rs->h_counters, (size_t)cg_ruleset::kMirror * kCounterWords * 4));
-    for (auto& e : rs->e_cnt) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  }
+  if ((rc = ensure_mirrors(rs))) return rc;
   // did an earlier batch overflow a queue?  (its result words say "incomplete"; grow the scratch before this one runs)
   poll_mirrors(rs, false);
   if ((rc = prepare_step(rs, n, false, st))) return rc;
@@ -854,11 +870,7 @@ int cg_scan_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offs
   }
   if (rc == CG_OK) {
     G.stats.messages_scanned += n;
-    const int slot = (int)(rs->seq % cg_ruleset::kMirror);
-    if (rs->cnt_pending[slot]) { cudaEventSynchronize(rs->e_cnt[slot]); poll_mirrors(rs, false); }
-    CU(cudaMemcpyAsync(rs->h_counters + (size_t)slot * kCounterWords, rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(rs->e_cnt[slot], st));
-    rs->cnt_pending[slot] = true; rs->seq++;
+    rc = mirror_counters(rs, st);
   }
   return rc;
 }
@@ -869,10 +881,63 @@ int cg_scan_join(cg_ruleset* rs, void* stream) {
   if (!rs) return fail(CG_ERR_INVALID_ARG, "null argument");
   CU(cudaStreamSynchronize(stream ? (cudaStream_t)stream : G.stream));
   poll_mirrors(rs, true);
-  const uint32_t flags = rs->sticky_flags; rs->sticky_flags = 0;
+  const uint32_t flags = rs->sticky_flags, status = rs->sticky_status; rs->sticky_flags = rs->sticky_status = 0;
   if (flags & (ERR_VM_STACK | ERR_VM_LIST)) return fail(CG_ERR_TOO_LARGE, std::string(kVmOverflow) + " (result words of that batch are all ones)");
-  if (flags) return fail(CG_ERR_CAPACITY, "a candidate queue overflowed: the result words of that batch are all ones; the scratch has been grown, scan the batch again");
+  if (status & (1u << kResolveTooLarge)) return fail(CG_ERR_TOO_LARGE, "redacted batch exceeds 4 GiB");
+  if (flags) return fail(CG_ERR_CAPACITY, "a candidate queue overflowed: the result words (or sizes) of that batch are all ones; the scratch has been grown, scan the batch again");
+  if (status & (1u << kResolveCapacity)) return fail(CG_ERR_CAPACITY, "output buffer too small: the sizes a batch needs are in its d_out_sizes / d_out_nspans");
   return CG_OK;
+}
+
+namespace {
+// findMatches (+ redaction) of a batch in HBM, enqueued on st: the span-mode step, the resolver, digests and splice (redact),
+// then the counter block into the mirror ring.  Never waits for the device except when the scratch must grow.
+int spans_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, const SpanOutputs& o, void* d_out_bytes,
+                 void* d_digests, void* stream) {
+  if (!rs || !d_bytes || !d_offsets || !o.sizes) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if ((uintptr_t)d_bytes & 15u) return fail(CG_ERR_INVALID_ARG, "d_bytes must be 16-byte aligned");
+  cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
+  const uint8_t* bytes = (const uint8_t*)d_bytes; const uint32_t* off = (const uint32_t*)d_offsets;
+  int rc;
+  if ((rc = ensure_mirrors(rs))) return rc;
+  poll_mirrors(rs, false);                                  // (an earlier batch overflowed?  grow before this one runs)
+  if ((rc = prepare_step(rs, n, true, st))) return rc;
+  const ScanWork& w = rs->work;
+  if (n) { if ((rc = run_scan_device(rs, bytes, off, n, w.words, true, st))) return rc; }
+  else CU(cudaMemsetAsync(w.counters, 0, kCounterWords * sizeof(uint32_t), st));
+  int k = launch_span_resolve(w, off, n, o, G.sm_count, st);
+  if (o.redact) {
+    k += launch_redact_digests(bytes, w.sp_start, w.sp_len, w.counters + 21, (uint32_t*)d_digests, G.sm_count, st);
+    k += launch_redact_splice(bytes, off, o.out_offsets, w.kept_begin, w.sp_start, w.sp_len, w.sp_cat, (const uint32_t*)d_digests,
+                              (uint8_t*)d_out_bytes, w.counters + 22, n, G.sm_count, st);
+  }
+  count_launches(k);
+  CU(cudaGetLastError());
+  G.stats.messages_scanned += n;
+  return mirror_counters(rs, st);
+}
+}  // namespace
+
+int cg_find_matches_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_spans, uint32_t spans_cap,
+                                 void* d_out_nspans, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  if (spans_cap && !d_out_spans) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (((uintptr_t)d_offsets | (uintptr_t)d_out_spans | (uintptr_t)d_out_nspans) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets, d_out_spans and d_out_nspans must be 4-byte aligned");
+  const SpanOutputs o{(uint32_t*)d_out_spans, d_out_spans ? spans_cap : 0u, nullptr, 0, d_out_nspans, false};
+  return spans_device(rs, d_bytes, d_offsets, n, o, nullptr, nullptr, stream);
+}
+
+int cg_redact_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_bytes, uint64_t out_cap,
+                           void* d_out_offsets, void* d_out_spans, uint32_t spans_cap, void* d_out_digests32, void* d_out_sizes, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  if (!d_out_offsets || (out_cap && !d_out_bytes) || (spans_cap && (!d_out_spans || !d_out_digests32))) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (((uintptr_t)d_offsets | (uintptr_t)d_out_offsets | (uintptr_t)d_out_spans) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets, d_out_offsets and d_out_spans must be 4-byte aligned");
+  if ((uintptr_t)d_out_sizes & 7u) return fail(CG_ERR_INVALID_ARG, "d_out_sizes must be 8-byte aligned");
+  if ((uintptr_t)d_out_digests32 & 15u) return fail(CG_ERR_INVALID_ARG, "d_out_digests32 must be 16-byte aligned");
+  const SpanOutputs o{(uint32_t*)d_out_spans, spans_cap, (uint32_t*)d_out_offsets, d_out_bytes ? out_cap : 0ull, d_out_sizes, true};
+  return spans_device(rs, d_bytes, d_offsets, n, o, d_out_bytes, d_out_digests32, stream);
 }
 
 // ---------------------------------------------------------------------------------- SHA / Merkle

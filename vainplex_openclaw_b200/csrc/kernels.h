@@ -59,6 +59,7 @@ struct ScanWork {
   uint32_t* counters;            // 32 words: [0]=n_slots [1]=n_events [2]=n_spans [3]=error flags [4]=n_l1 (confirmed factor occurrences) [5]=verify cursor
                                  //           [6]=flagged grams (level 1a) [7..15]=debug [17]=n_heavy [18]=verify cursor (light events) [19]=grams past the recheck map
                                  //           [24..27]=flag words queued, [28..31]=(gram, entry) pairs compared, per piece of the batch
+                                 //           span resolution: [16]=status (kResolve*) [20]=resolved spans [21]=digests to compute [22]=messages to splice
   uint32_t* l1_pos;              // [l1_cap] factor occurrences scan_kernel confirms itself (head check, trigger bytes): buffer offset of the
   uint32_t* l1_fac;              //          factor's first byte, factor id
   uint2* fq;                     // [l1_cap] scan_kernel's flag words: x = the lane's chunk number after the round, y = 4 tiles x 8 (4) probe bits
@@ -74,10 +75,31 @@ struct ScanWork {
   uint32_t* spans;               // [span_cap * 6] msg, rule, start_byte, end_byte, start16, end16
   uint32_t l1_cap, msg_cap, slot_cap, event_cap, span_cap;
   uint32_t q_cap, q_slot;        // this launch's piece of fq (a step scans the batch in up to 4 pieces: q_slot 0..3) and its counter [24 + q_slot]
+  // span resolution (span-mode steps only): [res_cap + 1] per message, [span_cap] per raw span
+  uint64_t* words;               // [res_cap] result words of span-mode steps
+  uint32_t* seg_cnt;             // raw spans per message (counted down again by the scatter)
+  uint32_t* seg_begin;           // exclusive scan of seg_cnt: the message's segment of `sorted`
+  uint32_t* kept_cnt;            // spans resolveOverlaps keeps per message
+  uint32_t* kept_begin;          // exclusive scan of kept_cnt: the message's first resolved span
+  uint64_t* out_len;             // redacted bytes per message
+  uint64_t* out_off;             // exclusive scan of out_len
+  uint4* sorted;                 // [span_cap] (start16, ~length16, rule rank, raw span index) in message order; kept keys first
+  uint4* sort_tmp;               // [span_cap] merge passes of long segments
+  uint32_t* sp_start;            // [span_cap] per resolved span: buffer offset of its first byte, byte length, category
+  uint32_t* sp_len;              //            (redact_splice_kernel's input)
+  uint32_t* sp_cat;
+  uint64_t* scan_part;           // [kScanPartials] partial sums of the exclusive scans
+  uint32_t res_cap;
+  // per rule its category (CG_CAT_*) and its rank in (category, rule) order, uploaded with the rule set.  (Kept here, not in
+  // DevRuleset: every scan kernel takes DevRuleset by value, and a larger one changes their code.)
+  const uint32_t* rule_category; const uint32_t* rule_rank;
 };
 
 enum : uint32_t { ERR_EVENT_OVERFLOW = 1, ERR_SPAN_OVERFLOW = 2, ERR_VM_STACK = 4, ERR_VM_LIST = 8, ERR_SLOT_OVERFLOW = 16, ERR_L1_OVERFLOW = 32 };
+// span resolution status (counters[16]); kept out of the error flags, which mean "a queue overflowed"
+enum : uint32_t { kResolveOk = 0, kResolveCapacity = 1, kResolveTooLarge = 2 };
 constexpr uint32_t kCounterWords = 32;
+constexpr uint32_t kScanPartials = 1024;         // blocks an exclusive scan uses at most
 constexpr uint32_t kConfirmTableBudget = 176u * 1024u;     // shared memory confirm_kernel may spend on its tables (beside 32 KB of rings)
 constexpr uint64_t kWordIncomplete = ~0ull;      // result word of every message of a batch whose queues overflowed / whose VM failed
 
@@ -106,16 +128,37 @@ int launch_pack_one(const DevRuleset& rs, const ScanWork& w, const uint64_t* d_w
 // raises the dynamic shared-memory limits of every kernel once (not legal inside stream capture)
 void prepare_scan_kernels();
 
+// exclusive prefix sums: out[i] = in[0] + ... + in[i - 1] for i < count (count >= 1; d_part: kScanPartials elements)
+int launch_exclusive_scan(const uint32_t* d_in, uint32_t* d_out, uint32_t count, uint64_t* d_part, int sm_count, cudaStream_t stream);
+int launch_exclusive_scan(const uint64_t* d_in, uint64_t* d_out, uint32_t count, uint64_t* d_part, int sm_count, cudaStream_t stream);
+// where resolved spans go (device pointers).  spans: 6 words per span, the first spans_cap written; redact: out_offsets[n+1],
+// and sizes = u64[2] {output bytes needed, resolved spans}, else sizes = u32[1] resolved spans; sizes are ~0 when the step
+// is incomplete (a queue overflowed or the VM failed).  The status goes to counters[16]: kResolveTooLarge (redact, 4 GiB or
+// more), kResolveCapacity (more spans than spans_cap, or more bytes than out_cap).
+struct SpanOutputs {
+  uint32_t* spans; uint32_t spans_cap;
+  uint32_t* out_offsets; uint64_t out_cap;
+  void* sizes;
+  bool redact;
+};
+// resolveOverlaps of a span-mode step over n messages (d_off as scanned): a fixed number of kernels for given n and mode,
+// whatever the span count.  Redact also leaves the splice's input in w.sp_* / w.kept_begin and sets counters[21] / [22] to the
+// spans to digest / messages to splice (0 unless every output fits).
+int launch_span_resolve(const ScanWork& w, const uint32_t* d_off, uint32_t n, const SpanOutputs& o, int sm_count, cudaStream_t stream);
+
 // SHA-256 / Merkle
 int launch_sha256_batch(const uint8_t* d_bytes, const uint64_t* d_off, uint32_t n, uint8_t* d_out, cudaStream_t stream);
 // Merkle log: acc = node(left[k], acc) chains; audit-path verification
 int launch_merkle_chain(const uint32_t* d_left, uint32_t n_left, const uint32_t* d_acc_in, uint32_t* d_acc_out, cudaStream_t stream);
 int launch_merkle_verify(const uint32_t* d_leaf32, uint64_t index, uint64_t size, const uint32_t* d_path, uint32_t path_len, const uint32_t* d_root32, uint32_t* d_ok, cudaStream_t stream);
-// redacted output: SHA-256 of every span, then copy + placeholder splice (one warp per message)
-int launch_redact_digests(const uint8_t* d_bytes, const uint32_t* d_start, const uint32_t* d_len, uint32_t ns, uint32_t* d_out, cudaStream_t stream);
+// redacted output: SHA-256 of every span, then copy + placeholder splice (one warp per message).  Both read their item
+// count from device memory (*d_ns spans, *d_n <= n_max messages), so that the resolver decides on the device whether they run.
+// d_out digests: 16-byte aligned.
+int launch_redact_digests(const uint8_t* d_bytes, const uint32_t* d_start, const uint32_t* d_len, const uint32_t* d_ns, uint32_t* d_out,
+                          int sm_count, cudaStream_t stream);
 int launch_redact_splice(const uint8_t* d_bytes, const uint32_t* d_off, const uint32_t* d_out_off, const uint32_t* d_span_begin,
                          const uint32_t* d_span_start, const uint32_t* d_span_len, const uint32_t* d_span_cat, const uint32_t* d_digests,
-                         uint8_t* d_out, uint32_t n, int sm_count, cudaStream_t stream);
+                         uint8_t* d_out, const uint32_t* d_n, uint32_t n_max, int sm_count, cudaStream_t stream);
 // leaf digests of fixed-size leaves: out[i] = SHA-256(0x00 || leaf_i)
 int launch_merkle_leaves_fixed(const uint8_t* d_bytes, uint64_t leaf_len, uint64_t n, uint32_t* d_out, cudaStream_t stream);
 // ragged leaves, word-granular: d_bytes must be one of the library's own buffers (readable 4 bytes before the first leaf and

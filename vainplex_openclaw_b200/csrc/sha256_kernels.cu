@@ -411,14 +411,15 @@ int launch_merkle_verify(const uint32_t* d_leaf32, uint64_t index, uint64_t size
 // redacted-output assembly (RedactionEngine.applyReplacements, engine.ts:165-181, with the vault's placeholder
 // "[REDACTED:<category>:<first 8 hex digits of SHA-256(match)>]", vault.ts:33-35,75-104)
 // ------------------------------------------------------------------------------------------
-// SHA-256 of every matched text: span i = bytes[start[i], start[i] + len[i])
+// SHA-256 of every matched text: span i = bytes[start[i], start[i] + len[i]) for i < *ns (the count is the resolver's)
 __global__ void __launch_bounds__(128) redact_digest_kernel(const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ start,
-                                                             const uint32_t* __restrict__ len, uint32_t ns, uint32_t* __restrict__ out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= ns) return;
-  uint32_t h[8];
-  sha_bytes(-1, bytes + start[i], len[i], h);
-  store_digest(out + (size_t)i * 8, h);
+                                                             const uint32_t* __restrict__ len, const uint32_t* __restrict__ ns, uint32_t* __restrict__ out) {
+  const uint32_t cnt = *ns;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += gridDim.x * blockDim.x) {
+    uint32_t h[8];
+    sha_bytes(-1, bytes + start[i], len[i], h);
+    store_digest(out + (size_t)i * 8, h);
+  }
 }
 
 __constant__ char kCatName[4][12] = {"credential", "financial", "pii", "custom"};       // CATEGORY_ORDER, registry.ts:17-22
@@ -430,8 +431,8 @@ __global__ void __launch_bounds__(256) redact_splice_kernel(const uint8_t* __res
                                                              const uint32_t* __restrict__ out_off, const uint32_t* __restrict__ span_begin,
                                                              const uint32_t* __restrict__ span_start, const uint32_t* __restrict__ span_len,
                                                              const uint32_t* __restrict__ span_cat, const uint32_t* __restrict__ digests,
-                                                             uint8_t* __restrict__ out, uint32_t n) {
-  const uint32_t lane = threadIdx.x & 31u, wpb = blockDim.x >> 5;
+                                                             uint8_t* __restrict__ out, const uint32_t* __restrict__ n_msgs) {
+  const uint32_t lane = threadIdx.x & 31u, wpb = blockDim.x >> 5, n = *n_msgs;
   for (uint32_t msg = blockIdx.x * wpb + (threadIdx.x >> 5); msg < n; msg += gridDim.x * wpb) {
     const uint32_t b = off[msg], e = off[msg + 1];
     uint32_t src = b, dst = out_off[msg];
@@ -462,17 +463,17 @@ __global__ void __launch_bounds__(256) redact_splice_kernel(const uint8_t* __res
   }
 }
 
-int launch_redact_digests(const uint8_t* d_bytes, const uint32_t* d_start, const uint32_t* d_len, uint32_t ns, uint32_t* d_out, cudaStream_t stream) {
-  if (!ns) return 0;
-  redact_digest_kernel<<<(ns + 127) / 128, 128, 0, stream>>>(d_bytes, d_start, d_len, ns, d_out);
+int launch_redact_digests(const uint8_t* d_bytes, const uint32_t* d_start, const uint32_t* d_len, const uint32_t* d_ns, uint32_t* d_out,
+                          int sm_count, cudaStream_t stream) {
+  redact_digest_kernel<<<sm_count * 8, 128, 0, stream>>>(d_bytes, d_start, d_len, d_ns, d_out);
   return 1;
 }
 int launch_redact_splice(const uint8_t* d_bytes, const uint32_t* d_off, const uint32_t* d_out_off, const uint32_t* d_span_begin,
                          const uint32_t* d_span_start, const uint32_t* d_span_len, const uint32_t* d_span_cat, const uint32_t* d_digests,
-                         uint8_t* d_out, uint32_t n, int sm_count, cudaStream_t stream) {
-  if (!n) return 0;
-  const uint32_t grid = std::min<uint32_t>((n + 7) / 8, (uint32_t)sm_count * 8u);
-  redact_splice_kernel<<<grid, 256, 0, stream>>>(d_bytes, d_off, d_out_off, d_span_begin, d_span_start, d_span_len, d_span_cat, d_digests, d_out, n);
+                         uint8_t* d_out, const uint32_t* d_n, uint32_t n_max, int sm_count, cudaStream_t stream) {
+  if (!n_max) return 0;
+  const uint32_t grid = std::min<uint32_t>((n_max + 7) / 8, (uint32_t)sm_count * 8u);
+  redact_splice_kernel<<<grid, 256, 0, stream>>>(d_bytes, d_off, d_out_off, d_span_begin, d_span_start, d_span_len, d_span_cat, d_digests, d_out, d_n);
   return 1;
 }
 
