@@ -133,6 +133,13 @@ CG_API int cg_scan_one(cg_ruleset *rs, const uint8_t *bytes, uint32_t len, uint6
  * by (msg, start); `rule` is the index passed to cg_ruleset_create. */
 CG_API int cg_find_matches_batch(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, uint32_t n,
                                  cg_span *out_spans, uint32_t spans_cap, uint32_t *out_nspans);
+/* findMatches + resolveOverlaps for one message, blocking (the synchronous hooks' path, src/redaction/hooks.ts:158-206,
+ * 405-456).  Spans, *out_nspans, return code and statistics equal cg_find_matches_batch with n = 1 (span.msg = 0): on
+ * CG_ERR_CAPACITY the first spans_cap spans are written.  A message of at most 16 KB costs one H2D copy, one CUDA graph,
+ * one D2H copy and one synchronise (DESIGN.md section 4.5); longer ones, and the rare result too long for the staging
+ * block, take the batch call's path. */
+CG_API int cg_find_matches_one(cg_ruleset *rs, const uint8_t *bytes, uint32_t len,
+                               cg_span *out_spans, uint32_t spans_cap, uint32_t *out_nspans);
 
 /* ---- verdicts instead of hit bits (SURVEY.md section 8 f3): aggregateMatches / matchPolicy of src/policy-evaluator.ts:44-146
  * for rule sets whose rules are the messageContains patterns of a policy list.  rule_policy[i] = index of rule i's policy
@@ -154,6 +161,11 @@ CG_API int cg_policy_verdict_batch(cg_ruleset *rs, const uint8_t *bytes, const u
 CG_API int cg_redact_batch(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, uint32_t n,
                            uint8_t *out_bytes, uint64_t out_cap, uint64_t *out_need, uint32_t *out_offsets,
                            cg_span *out_spans, uint32_t spans_cap, uint32_t *out_nspans, uint8_t *out_digests32);
+/* RedactionEngine.scanString for one message, blocking: bytes, spans and digests equal cg_redact_batch with n = 1
+ * (*out_need = redacted length; CG_ERR_CAPACITY with the sizes set and nothing else written when a capacity is short).
+ * Same single-message path as cg_find_matches_one. */
+CG_API int cg_redact_one(cg_ruleset *rs, const uint8_t *bytes, uint32_t len, uint8_t *out_bytes, uint64_t out_cap,
+                         uint64_t *out_need, cg_span *out_spans, uint32_t spans_cap, uint32_t *out_nspans, uint8_t *out_digests32);
 
 /* ---- device-resident variant (inputs/outputs already in HBM; used by bench.py `value` and by callers that pipeline
  * their own copies).  Pointers are CUDA device pointers; `stream` is a cudaStream_t (NULL = the library's own stream);

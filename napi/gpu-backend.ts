@@ -3,7 +3,7 @@
  * (packages/openclaw-governance/src/gpu-backend.ts).  It keeps the plugin's classes and call sites and swaps the two hot
  * loops and the hash for calls into the N-API addon built from napi/openclaw_gov_napi.c:
  *
- *   PatternRegistry.findMatches   src/redaction/registry.ts:212-242,288-316   -> findMatchesBatch (spans already resolved)
+ *   PatternRegistry.findMatches   src/redaction/registry.ts:212-242,288-316   -> findMatchesOne / findMatchesBatch (spans already resolved)
  *   matchesAny                    src/conditions/context.ts:9-25              -> scanBatch over every pattern of the policy set
  *   ResponseGate mustMatch / mustNotMatch  src/response-gate.ts:104-149       -> scanBatch
  *   tool param `matches`          src/conditions/tool.ts:36-45                -> scanBatch
@@ -27,6 +27,8 @@ type Addon = {
   scanOne(handle: unknown, bytes: Uint8Array): { word: bigint; rules: Uint32Array };
   findMatchesBatch(handle: unknown, bytes: Uint8Array, offsets: Uint32Array): Uint32Array;
   redactBatch(handle: unknown, bytes: Uint8Array, offsets: Uint32Array): { bytes: Uint8Array; offsets: Uint32Array; spans: Uint32Array; digests: Uint8Array };
+  findMatchesOne(handle: unknown, bytes: Uint8Array): Uint32Array;
+  redactOne(handle: unknown, bytes: Uint8Array): { bytes: Uint8Array; spans: Uint32Array; digests: Uint8Array };
   setPolicy(handle: unknown, rulePolicy: Uint32Array, ruleAction: Uint8Array): void;
   verdictBatch(handle: unknown, bytes: Uint8Array, offsets: Uint32Array): Uint32Array;
   sha256Batch(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array;
@@ -88,8 +90,15 @@ export class GpuPatternRegistry {
     return out;
   }
 
-  findMatches(text: string) {
-    return this.findMatchesBatch([text])[0];
+  /** findMatches for one string (the synchronous hooks' path): one blocking call, one device round trip. */
+  findMatches(text: string): ReturnType<GpuPatternRegistry["findMatchesBatch"]>[number] {
+    const spans = addon.findMatchesOne(this.handle, enc.encode(text));   // msg (= 0), rule, startByte, endByte, start16, end16
+    const out: ReturnType<GpuPatternRegistry["findMatchesBatch"]>[number] = [];
+    for (let k = 0; k < spans.length; k += 6) {
+      const [, rule, , , s16, e16] = spans.subarray(k, k + 6);
+      out.push({ pattern: this.patterns[rule], match: text.slice(s16, e16), index: s16, length: e16 - s16 });
+    }
+    return out;
   }
 }
 

@@ -19,6 +19,8 @@
  *   scanOne(handle, bytes: Uint8Array): {word: bigint, rules: Uint32Array}
  *   findMatchesBatch(handle, bytes, offsets): Uint32Array  // 6 words per span: msg, rule, startByte, endByte, start16, end16
  *   redactBatch(handle, bytes, offsets): {bytes, offsets, spans, digests}  // scanString for a batch, spliced on the device
+ *   findMatchesOne(handle, bytes: Uint8Array): Uint32Array  // one message, blocking: findMatchesBatch's spans for a batch of one
+ *   redactOne(handle, bytes: Uint8Array): {bytes, spans, digests}  // one message, blocking: scanString spliced on the device
  *   setPolicy(handle, rulePolicy: Uint32Array, ruleAction: Uint8Array): void ; verdictBatch(handle, bytes, offsets): Uint32Array
  *   sha256Batch(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array  // 32 bytes per item
  *   merkleRoot(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array   // 32 bytes
@@ -375,12 +377,61 @@ static napi_value js_redact_batch(napi_env env, napi_callback_info info) {
   return res;
 }
 
+/* ---- one message, blocking: the synchronous hooks' findMatches / scanString (cg_find_matches_one / cg_redact_one) */
+static uint8_t one_empty[1];                          /* the message of an empty Uint8Array */
+static napi_value js_find_matches_one(napi_env env, napi_callback_info info) {
+  ARGS(env, info, 2)
+  cg_ruleset *rs; uint8_t *bytes; size_t nb;
+  NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
+  if (!get_ta(env, argv[1], &bytes, &nb, napi_uint8_array) || nb > UINT32_MAX) { napi_throw_type_error(env, NULL, "findMatchesOne(handle, Uint8Array)"); return NULL; }
+  if (!nb) bytes = one_empty;                       /* an empty typed array may report NULL: the C ABI rejects a NULL message */
+  uint32_t ns = 0, cap = 64; cg_span *tmp = (cg_span *)malloc(sizeof(cg_span) * cap);
+  int rc = tmp ? cg_find_matches_one(rs, bytes, (uint32_t)nb, tmp, cap, &ns) : CG_ERR_NOMEM;
+  if (rc == CG_ERR_CAPACITY) { cap = ns; cg_span *t2 = (cg_span *)realloc(tmp, sizeof(cg_span) * cap); if (t2) { tmp = t2; rc = cg_find_matches_one(rs, bytes, (uint32_t)nb, tmp, cap, &ns); } }
+  if (rc != CG_OK) { free(tmp); napi_throw_error(env, NULL, rc == CG_ERR_NOMEM ? "out of host memory" : cg_last_error()); return NULL; }
+  napi_value ab, arr; void *data;
+  if (napi_create_arraybuffer(env, (size_t)ns * sizeof(cg_span), &data, &ab) != napi_ok) { free(tmp); napi_throw_error(env, NULL, "N-API call failed"); return NULL; }
+  memcpy(data, tmp, (size_t)ns * sizeof(cg_span)); free(tmp);
+  NAPI_CALL(env, napi_create_typedarray(env, napi_uint32_array, (size_t)ns * 6, ab, 0, &arr));
+  return arr;
+}
+
+static napi_value js_redact_one(napi_env env, napi_callback_info info) {
+  ARGS(env, info, 2)
+  cg_ruleset *rs; uint8_t *bytes; size_t nb;
+  NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
+  if (!get_ta(env, argv[1], &bytes, &nb, napi_uint8_array) || nb > UINT32_MAX) { napi_throw_type_error(env, NULL, "redactOne(handle, Uint8Array)"); return NULL; }
+  if (!nb) bytes = one_empty;
+  uint32_t ns = 0, cap_spans = 64; uint64_t need = 0, cap_bytes = (uint64_t)nb + 1024;
+  uint8_t *out = NULL, *dig = NULL; cg_span *spans = NULL; int rc = CG_ERR_NOMEM;
+  for (;;) {
+    uint8_t *o2 = (uint8_t *)realloc(out, cap_bytes); cg_span *s2 = (cg_span *)realloc(spans, sizeof(cg_span) * cap_spans); uint8_t *d2 = (uint8_t *)realloc(dig, (size_t)cap_spans * 32);
+    if (o2) out = o2;
+    if (s2) spans = s2;
+    if (d2) dig = d2;
+    if (!o2 || !s2 || !d2) { rc = CG_ERR_NOMEM; break; }
+    rc = cg_redact_one(rs, bytes, (uint32_t)nb, out, cap_bytes, &need, spans, cap_spans, &ns, dig);
+    if (rc == CG_ERR_CAPACITY && (need > cap_bytes || ns > cap_spans)) { if (need > cap_bytes) cap_bytes = need; if (ns > cap_spans) cap_spans = ns; continue; }
+    break;
+  }
+  if (rc != CG_OK) { free(out); free(spans); free(dig); napi_throw_error(env, NULL, rc == CG_ERR_NOMEM ? "out of host memory" : cg_last_error()); return NULL; }
+  napi_value res = NULL, b_arr = make_u8(env, out, (size_t)need), d_arr = make_u8(env, dig, (size_t)ns * 32), s_ab, s_arr = NULL; void *p;
+  int ok = b_arr && d_arr && napi_create_arraybuffer(env, (size_t)ns * sizeof(cg_span), &p, &s_ab) == napi_ok;
+  if (ok) { memcpy(p, spans, (size_t)ns * sizeof(cg_span)); ok = napi_create_typedarray(env, napi_uint32_array, (size_t)ns * 6, s_ab, 0, &s_arr) == napi_ok; }
+  free(out); free(spans); free(dig);
+  if (!ok || napi_create_object(env, &res) != napi_ok) { napi_throw_error(env, NULL, "N-API call failed"); return NULL; }
+  NAPI_CALL(env, napi_set_named_property(env, res, "bytes", b_arr));
+  NAPI_CALL(env, napi_set_named_property(env, res, "spans", s_arr)); NAPI_CALL(env, napi_set_named_property(env, res, "digests", d_arr));
+  return res;
+}
+
 static napi_value module_init(napi_env env, napi_value exports) {
   napi_property_descriptor d[] = {
 #define FN(name, fn) {name, NULL, fn, NULL, NULL, NULL, napi_default, NULL}
     FN("init", js_init), FN("shutdown", js_shutdown), FN("stats", js_stats), FN("ruleCheck", js_rule_check),
     FN("createRuleset", js_create_ruleset), FN("scanBatch", js_scan_batch), FN("scanOne", js_scan_one),
     FN("findMatchesBatch", js_find_matches_batch), FN("redactBatch", js_redact_batch),
+    FN("findMatchesOne", js_find_matches_one), FN("redactOne", js_redact_one),
     FN("setPolicy", js_set_policy), FN("verdictBatch", js_verdict_batch),
     FN("sha256Batch", js_sha256_batch), FN("merkleRoot", js_merkle_root),
     FN("logCreate", js_log_create), FN("logRestore", js_log_restore), FN("logAppend", js_log_append), FN("logAppendJsonl", js_log_append_jsonl),

@@ -54,7 +54,7 @@ EXPORTS = ["cg_init", "cg_shutdown", "cg_last_error", "cg_version", "cg_device_c
            "cg_merkle_log_append_jsonl", "cg_merkle_log_consistency", "cg_merkle_verify_consistency", "cg_merkle_log_reserve",
            "cg_shard_range", "cg_comm_unique_id", "cg_comm_init", "cg_comm_destroy", "cg_merkle_root_sharded_device",
            "cg_ruleset_create", "cg_ruleset_destroy", "cg_ruleset_get_info", "cg_rule_check", "cg_scan_batch",
-           "cg_scan_one", "cg_find_matches_batch", "cg_scan_batch_device", "cg_find_matches_batch_device", "cg_redact_batch_device", "cg_sha256_batch", "cg_merkle_root",
+           "cg_scan_one", "cg_find_matches_batch", "cg_find_matches_one", "cg_redact_one", "cg_scan_batch_device", "cg_find_matches_batch_device", "cg_redact_batch_device", "cg_sha256_batch", "cg_merkle_root",
            "cg_merkle_root_fixed", "cg_merkle_block_roots_device", "cg_merkle_fold", "cg_merkle_fold_device"]
 
 _lib = None
@@ -116,6 +116,8 @@ def load():
     L.cg_scan_batch.argtypes = [vp, vp, vp, u32, vp, vp, u32, C.POINTER(u32)]; L.cg_scan_batch.restype = i32
     L.cg_scan_one.argtypes = [vp, vp, u32, C.POINTER(u64), vp, u32, C.POINTER(u32)]; L.cg_scan_one.restype = i32
     L.cg_find_matches_batch.argtypes = [vp, vp, vp, u32, vp, u32, C.POINTER(u32)]; L.cg_find_matches_batch.restype = i32
+    L.cg_find_matches_one.argtypes = [vp, vp, u32, vp, u32, C.POINTER(u32)]; L.cg_find_matches_one.restype = i32
+    L.cg_redact_one.argtypes = [vp, vp, u32, vp, u64, C.POINTER(u64), vp, u32, C.POINTER(u32), vp]; L.cg_redact_one.restype = i32
     L.cg_scan_batch_device.argtypes = [vp, vp, vp, u32, vp, vp]; L.cg_scan_batch_device.restype = i32
     L.cg_find_matches_batch_device.argtypes = [vp, vp, vp, u32, vp, u32, vp, vp]; L.cg_find_matches_batch_device.restype = i32
     L.cg_redact_batch_device.argtypes = [vp, vp, vp, u32, vp, u64, vp, vp, u32, vp, vp, vp]; L.cg_redact_batch_device.restype = i32
@@ -237,6 +239,37 @@ class Ruleset:
                 continue
             check(rc)
             return spans[:ns.value]
+
+    def find_matches_one(self, msg: bytes):
+        """findMatches for one message, blocking (the synchronous hooks' path): -> spans structured array (msg = 0), as
+        find_matches_batch returns for a batch of one."""
+        ns = C.c_uint32(0)
+        cap = 64
+        while True:
+            spans = np.empty(cap, dtype=SPAN_DTYPE)
+            rc = load().cg_find_matches_one(self.handle, msg, len(msg), spans.ctypes.data, cap, C.byref(ns))
+            if rc == CG_ERR_CAPACITY and ns.value > cap:
+                cap = ns.value
+                continue
+            check(rc)
+            return spans[:ns.value]
+
+    def redact_one(self, msg: bytes):
+        """RedactionEngine.scanString for one message, blocking, spliced on the device.
+        -> (redacted bytes, resolved spans, digests uint8[ns, 32])"""
+        need, ns = C.c_uint64(0), C.c_uint32(0)
+        cap_bytes, cap_spans = len(msg) + 1024, 64
+        while True:
+            out = np.empty(cap_bytes, dtype=np.uint8)
+            spans = np.empty(cap_spans, dtype=SPAN_DTYPE)
+            dig = np.empty((cap_spans, 32), dtype=np.uint8)
+            rc = load().cg_redact_one(self.handle, msg, len(msg), out.ctypes.data, cap_bytes, C.byref(need), spans.ctypes.data,
+                                      cap_spans, C.byref(ns), dig.ctypes.data)
+            if rc == CG_ERR_CAPACITY and (need.value > cap_bytes or ns.value > cap_spans):
+                cap_bytes, cap_spans = max(cap_bytes, need.value), max(cap_spans, ns.value)
+                continue
+            check(rc)
+            return out[:need.value].tobytes(), spans[:ns.value], dig[:ns.value]
 
     def set_policy(self, rule_policy, rule_action):
         """rule i belongs to policy rule_policy[i] (evaluation order, non-decreasing) with effect rule_action[i] (0 allow, 1 audit, 2 deny)."""

@@ -120,16 +120,20 @@ struct cg_ruleset {
   uint64_t scratch_gen = 0;       // advanced by every change to what a captured step holds (scratch buffers, DevRuleset)
   // the device-resident step replayed as one CUDA graph (keyed on its arguments, the scratch generation and the verify grid)
   struct CachedGraph { int kernels = 0; cudaGraphExec_t exec = nullptr; const void* bytes = nullptr; const void* off = nullptr; void* words = nullptr; uint32_t n = 0; uint64_t gen = 0; int ctas = 0; uint64_t used = 0; };
-  // cg_scan_one: pinned staging + one device block ([offsets][message bytes] in, [word][counters][hit row] out) and the
-  // step as a graph over those fixed addresses (the message length is data, so one graph serves every message)
-  struct OnePath { cudaGraphExec_t exec = nullptr; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint64_t gen = 0; int ctas = 0; int kernels = 0; } one;
+  // cg_scan_one / cg_find_matches_one / cg_redact_one: pinned staging + one device block ([offsets][message bytes] in,
+  // [word][counters][hit row] out), for the span calls a second pair (the packed result, and on the device its scratch;
+  // capi.cu kOne*), and per mode the step as a graph over those fixed addresses (the message length is data, so one graph
+  // serves every message)
+  struct OneGraph { cudaGraphExec_t exec = nullptr; uint64_t gen = 0; int ctas = 0; int kernels = 0; };
+  struct OnePath { OneGraph g[3]; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint8_t* h_pack = nullptr; uint8_t* d_pack = nullptr; } one;
   CachedGraph graphs[2];          // two entries: callers that alternate between two input/output buffer sets replay, never re-capture
   uint64_t graph_clock = 0;
   ~cg_ruleset() {
     for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    if (one.exec) cudaGraphExecDestroy(one.exec);
+    for (auto& g : one.g) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (one.h_pin) cudaFreeHost(one.h_pin);
-    cudaFree(one.d_buf);
+    if (one.h_pack) cudaFreeHost(one.h_pack);
+    cudaFree(one.d_buf); cudaFree(one.d_pack);
     if (h_counters) cudaFreeHost(h_counters);
     for (auto& e : e_cnt) if (e) cudaEventDestroy(e);
     for (void* p : allocs) cudaFree(p);
@@ -430,6 +434,44 @@ int mirror_counters(cg_ruleset* rs, cudaStream_t st) {
   return CG_OK;
 }
 
+// The single-message staging block, host (pinned) and device: [offsets, 256 B][message bytes][64 zero bytes] in (kOneIn),
+// [word][counters][hit row] out (kOneOut).  The span calls add, on their first use, the packed result (kOnePack bytes,
+// layout in kernels.h) on both sides and, on the device only, the digests and the redacted bytes before the pack step
+// moves them behind the spans (kOnePack each).
+constexpr uint32_t kOneBytes = 16384, kOneRw = 128, kOneIn = 256 + kOneBytes + 64, kOneOut = (2 + kCounterWords + kOneRw) * 4;
+constexpr uint32_t kOnePack = 512 * 1024;
+// the resolver's capacities on this path: every resolved span (and, redacting, its digest and the output) must fit the block
+constexpr uint32_t kOneSpansFind = (kOnePack - kPackHeader) / 24, kOneSpansRedact = (kOnePack - kPackHeader) / 56;
+enum { kOneScan = 0, kOneFind = 1, kOneRedact = 2 };
+
+// (spans: also the span calls' packed result and scratch)
+int one_staging(cg_ruleset::OnePath& o, bool spans) {
+  if (!o.h_pin) { CU(cudaMallocHost((void**)&o.h_pin, kOneIn + kOneOut)); memset(o.h_pin, 0, kOneIn + kOneOut); }
+  if (!o.d_buf) { CU(cudaMalloc((void**)&o.d_buf, kOneIn + kOneOut)); CU(cudaMemset(o.d_buf, 0, kOneIn + kOneOut)); }
+  if (!spans) return CG_OK;
+  if (!o.h_pack) { CU(cudaMallocHost((void**)&o.h_pack, kOnePack)); memset(o.h_pack, 0, kOnePack); }
+  if (!o.d_pack) { CU(cudaMalloc((void**)&o.d_pack, 3 * (size_t)kOnePack)); CU(cudaMemset(o.d_pack, 0, 3 * (size_t)kOnePack)); }
+  return CG_OK;
+}
+// mode m's graph, captured again when the scratch or the verify grid changed since it was captured
+template <typename Enqueue>
+int one_graph(cg_ruleset* rs, int m, Enqueue&& enqueue) {
+  cg_ruleset::OneGraph& g = rs->one.g[m];
+  if (g.exec && g.gen == rs->scratch_gen && g.ctas == rs->verify_ctas) return CG_OK;
+  if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
+  if (int rc = capture(G.stream, enqueue, &g.exec, &g.kernels)) return rc;
+  g.gen = rs->scratch_gen; g.ctas = rs->verify_ctas;
+  return CG_OK;
+}
+// the message into the staging block (offsets {256, 256 + len}) and one H2D copy
+int stage_one(cg_ruleset::OnePath& o, const uint8_t* bytes, uint32_t len, cudaStream_t st) {
+  uint32_t* hoff = reinterpret_cast<uint32_t*>(o.h_pin); hoff[0] = 256; hoff[1] = 256 + len;
+  if (len) memcpy(o.h_pin + 256, bytes, len);
+  memset(o.h_pin + 256 + len, 0, 64);
+  CU(cudaMemcpyAsync(o.d_buf, o.h_pin, 256 + (size_t)len + 64, cudaMemcpyHostToDevice, st));
+  return CG_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -676,7 +718,6 @@ int cg_scan_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets,
 }
 
 namespace {
-constexpr uint32_t kOneBytes = 16384, kOneRw = 128, kOneIn = 256 + kOneBytes + 64, kOneOut = (2 + kCounterWords + kOneRw) * 4;
 // -> CG_OK, an error, or 1 = take the general path (long message, large rule set, a queue overflowed)
 int scan_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* out_word, uint32_t* out_rules, uint32_t rules_cap, uint32_t* out_nrules) {
   static const bool off_ = getenv("CG_ONE_FAST") && atoi(getenv("CG_ONE_FAST")) == 0;
@@ -684,27 +725,20 @@ int scan_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* 
   cg_ruleset::OnePath& o = rs->one;
   cudaStream_t st = G.stream;
   int rc;
-  if (!o.h_pin) { CU(cudaMallocHost((void**)&o.h_pin, kOneIn + kOneOut)); memset(o.h_pin, 0, kOneIn + kOneOut); CU(cudaMalloc((void**)&o.d_buf, kOneIn + kOneOut)); CU(cudaMemset(o.d_buf, 0, kOneIn + kOneOut)); }
+  if ((rc = one_staging(o, false))) return rc;
   if ((rc = prepare_step(rs, 1, false, st))) return rc;
   const uint8_t* d_bytes = o.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(o.d_buf);
   uint32_t* d_out = reinterpret_cast<uint32_t*>(o.d_buf + kOneIn); uint64_t* d_word = reinterpret_cast<uint64_t*>(o.d_buf + kOneIn + kOneOut - 8);   // (the word lands behind the hit row, then is packed to the front)
-  if (!o.exec || o.gen != rs->scratch_gen || o.ctas != rs->verify_ctas) {
-    if (o.exec) { cudaGraphExecDestroy(o.exec); o.exec = nullptr; }
-    if ((rc = capture(st, [&] {
-          const int r = run_scan_device(rs, d_bytes, d_off, 1, d_word, false, st);
-          if (r == CG_OK) count_launches(launch_pack_one(rs->dev, rs->work, d_word, d_out, kOneRw - 2, st));
-          return r;
-        }, &o.exec, &o.kernels))) return rc;
-    o.gen = rs->scratch_gen; o.ctas = rs->verify_ctas;
-  }
-  uint32_t* hoff = reinterpret_cast<uint32_t*>(o.h_pin); hoff[0] = 256; hoff[1] = 256 + len;
-  if (len) memcpy(o.h_pin + 256, bytes, len);
-  memset(o.h_pin + 256 + len, 0, 64);
-  CU(cudaMemcpyAsync(o.d_buf, o.h_pin, 256 + (size_t)len + 64, cudaMemcpyHostToDevice, st));
-  CU(cudaGraphLaunch(o.exec, st));
+  if ((rc = one_graph(rs, kOneScan, [&] {
+        const int r = run_scan_device(rs, d_bytes, d_off, 1, d_word, false, st);
+        if (r == CG_OK) count_launches(launch_pack_one(rs->dev, rs->work, d_word, d_out, kOneRw - 2, st));
+        return r;
+      }))) return rc;
+  if ((rc = stage_one(o, bytes, len, st))) return rc;
+  CU(cudaGraphLaunch(o.g[kOneScan].exec, st));
   CU(cudaMemcpyAsync(o.h_pin + kOneIn, d_out, (2 + kCounterWords + rs->dev.rw) * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  count_launches(o.kernels);
+  count_launches(o.g[kOneScan].kernels);
   const uint32_t* ho = reinterpret_cast<const uint32_t*>(o.h_pin + kOneIn);
   const uint32_t* hc = ho + 2;
   if ((rc = absorb_counters(rs, hc))) return rc;                 // 1: a queue overflowed, the general path retries with larger scratch
@@ -835,6 +869,100 @@ int cg_redact_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offset
   if (ns && out_digests32) CU(cudaMemcpyAsync(out_digests32, d_dig, (size_t)ns * 32, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
+}
+
+namespace {
+struct OneSpanOut { cg_span* spans; uint32_t spans_cap; uint32_t* nspans; uint8_t* bytes; uint64_t out_cap; uint64_t* need; uint8_t* digests; };
+// cg_find_matches_one / cg_redact_one on the staging block: one H2D copy, one graph (span-mode step, one-block resolver,
+// digests and splice when redacting, pack), one D2H copy of the header plus a window sized from len, one synchronise; a
+// second copy and synchronise only for a packed result longer than the window.  Outputs, statuses and statistics are those
+// of the batch call with n = 1.  -> CG_OK, an error, or 1 = take the batch path (an argument the batch call rejects, no
+// device, a long message, profiling, a queue overflowed, or a result longer than the staging block)
+int span_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, bool redact, const OneSpanOut& out) {
+  if (!G.ready || !rs || !bytes || len > kOneBytes || G.profiling) return 1;
+  cg_ruleset::OnePath& o = rs->one;
+  cudaStream_t st = G.stream;
+  int rc;
+  if ((rc = one_staging(o, true))) return rc;
+  if ((rc = prepare_step(rs, 1, true, st))) return rc;
+  const ScanWork& w = rs->work;
+  const uint8_t* d_bytes = o.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(o.d_buf);
+  uint32_t* d_pack = reinterpret_cast<uint32_t*>(o.d_pack);
+  uint32_t* d_dig = reinterpret_cast<uint32_t*>(o.d_pack + kOnePack);
+  uint8_t* d_out = o.d_pack + 2 * kOnePack;
+  const int m = redact ? kOneRedact : kOneFind;
+  if ((rc = one_graph(rs, m, [&] {
+        const int r = run_scan_device(rs, d_bytes, d_off, 1, w.words, true, st);
+        if (r != CG_OK) return r;
+        const SpanOutputs so{d_pack + kPackHeader / 4, redact ? kOneSpansRedact : kOneSpansFind, d_pack + kPackOffsets,
+                             redact ? (uint64_t)(kOnePack - kPackHeader) : 0ull, d_pack + kPackSizes, redact};
+        int k = launch_span_resolve_one(w, d_off, so, st);
+        if (redact) {
+          k += launch_redact_digests(d_bytes, w.sp_start, w.sp_len, w.counters + 21, d_dig, G.sm_count, st);
+          k += launch_redact_splice(d_bytes, d_off, d_pack + kPackOffsets, w.kept_begin, w.sp_start, w.sp_len, w.sp_cat, d_dig, d_out,
+                                    w.counters + 22, 1, G.sm_count, st);
+        }
+        k += launch_span_pack_one(w, d_dig, d_out, d_pack, kOnePack, redact, st);
+        count_launches(k);
+        CU(cudaGetLastError());
+        return CG_OK;
+      }))) return rc;
+  if ((rc = stage_one(o, bytes, len, st))) return rc;
+  CU(cudaGraphLaunch(o.g[m].exec, st));
+  // the window: the header, 1 KB and len / 2 bytes (find-matches) or 2 x len bytes (redaction) of the packed result
+  const uint32_t window = std::min<uint32_t>(kOnePack, kPackHeader + 1024 + (redact ? 2 * len : len / 2));
+  uint8_t* h_pack = o.h_pack;
+  CU(cudaMemcpyAsync(h_pack, d_pack, window, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  count_launches(o.g[m].kernels);
+  const uint32_t* hp = reinterpret_cast<const uint32_t*>(h_pack);
+  const uint32_t* hc = hp + kPackCounters;
+  if ((rc = absorb_counters(rs, hc))) return rc;                 // 1: a queue overflowed, the batch call retries with larger scratch
+  const uint32_t packed = hp[0];
+  if (!packed) return 1;                                         // longer than the staging block: the batch call has room
+  if (packed > window) {
+    CU(cudaMemcpyAsync(h_pack + window, reinterpret_cast<const uint8_t*>(d_pack) + window, packed - window, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+  }
+  G.stats.messages_scanned += 1; G.stats.bytes_scanned += len; G.stats.candidate_events += hc[1]; G.stats.verified_pairs += hc[1];
+  const uint8_t* body = h_pack + kPackHeader;
+  if (!redact) {
+    const uint32_t ns = hp[kPackSizes];
+    G.stats.spans += ns;
+    const uint32_t k = std::min(ns, out.spans_cap);
+    if (out.spans && k) memcpy(out.spans, body, (size_t)k * sizeof(cg_span));
+    if (out.nspans) *out.nspans = ns;
+    if (out.spans && ns > out.spans_cap) return fail(CG_ERR_CAPACITY, "out_spans too small");
+    return CG_OK;
+  }
+  uint64_t sizes[2];
+  memcpy(sizes, hp + kPackSizes, sizeof sizes);
+  const uint64_t need = sizes[0]; const uint32_t ns = (uint32_t)sizes[1];
+  G.stats.spans += ns;
+  if (out.need) *out.need = need;
+  if (out.nspans) *out.nspans = ns;
+  if (need >> 32) return fail(CG_ERR_TOO_LARGE, "redacted batch exceeds 4 GiB");
+  if ((out.spans && ns > out.spans_cap) || need > out.out_cap || !out.bytes) return fail(CG_ERR_CAPACITY, "output buffer too small (see *out_need / *out_nspans)");
+  G.stats.sha256_items += ns;
+  if (need) memcpy(out.bytes, body + (size_t)ns * (sizeof(cg_span) + 32), (size_t)need);
+  if (ns && out.spans) memcpy(out.spans, body, (size_t)ns * sizeof(cg_span));
+  if (ns && out.digests) memcpy(out.digests, body + (size_t)ns * sizeof(cg_span), (size_t)ns * 32);
+  return CG_OK;
+}
+}  // namespace
+
+int cg_find_matches_one(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans) {
+  { std::lock_guard<std::mutex> lk(g_mu); const int frc = span_one_fast(rs, bytes, len, false, OneSpanOut{out_spans, spans_cap, out_nspans, nullptr, 0, nullptr, nullptr}); if (frc != 1) return frc; }
+  const uint32_t off[2] = {0, len};
+  return cg_find_matches_batch(rs, bytes, off, 1, out_spans, spans_cap, out_nspans);
+}
+
+int cg_redact_one(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_need,
+                  cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans, uint8_t* out_digests32) {
+  { std::lock_guard<std::mutex> lk(g_mu); const int frc = span_one_fast(rs, bytes, len, true, OneSpanOut{out_spans, spans_cap, out_nspans, out_bytes, out_cap, out_need, out_digests32}); if (frc != 1) return frc; }
+  const uint32_t off[2] = {0, len};
+  uint32_t out_off[2] = {0, 0};
+  return cg_redact_batch(rs, bytes, off, 1, out_bytes, out_cap, out_need, out_off, out_spans, spans_cap, out_nspans, out_digests32);
 }
 
 int cg_scan_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_words, void* stream) {

@@ -145,6 +145,16 @@ struct SpanOutputs {
 // whatever the span count.  Redact also leaves the splice's input in w.sp_* / w.kept_begin and sets counters[21] / [22] to the
 // spans to digest / messages to splice (0 unless every output fits).
 int launch_span_resolve(const ScanWork& w, const uint32_t* d_off, uint32_t n, const SpanOutputs& o, int sm_count, cudaStream_t stream);
+// the same for a batch of one message in one block (one launch, any raw span count up to w.span_cap)
+int launch_span_resolve_one(const ScanWork& w, const uint32_t* d_off, const SpanOutputs& o, cudaStream_t stream);
+// single-message span path: the result packed into one block for one D2H copy, as u32 words:
+//   [0] packed bytes (0: the result is incomplete, not ok, or longer than pack_cap -- the caller takes the batch path)
+//   [1] resolver status  [2..5] sizes (SpanOutputs.sizes)  [6..7] output offsets  [8..39] counter block
+//   then from byte kPackHeader: spans (6 words each), digests (32 bytes each, redact), output bytes (redact)
+// The resolver writes the spans, sizes and offsets in place; the pack step adds the rest.
+constexpr uint32_t kPackSizes = 2, kPackOffsets = 6, kPackCounters = 8, kPackHeader = (kPackCounters + kCounterWords) * 4;
+int launch_span_pack_one(const ScanWork& w, const uint32_t* d_digests, const uint8_t* d_out, uint32_t* d_packed, uint32_t pack_cap, bool redact,
+                         cudaStream_t stream);
 
 // SHA-256 / Merkle
 int launch_sha256_batch(const uint8_t* d_bytes, const uint64_t* d_off, uint32_t n, uint8_t* d_out, cudaStream_t stream);

@@ -10,6 +10,9 @@
 // the raw spans were queued in.  An empty match sets last_end to its own start: empty spans at one position are all kept.
 //
 // Every launch geometry depends on n and the SM count only; the span count is read from device memory.
+//
+// A batch of one message (cg_find_matches_one / cg_redact_one) skips the chain: span_resolve_one_kernel builds the keys,
+// sorts, keeps and emits in one block, through the same sort_keep_segment as the long segments of a batch.
 #include <algorithm>
 #include <cstdint>
 
@@ -132,6 +135,64 @@ __device__ __forceinline__ int64_t splice_delta(const ScanWork& w, const uint32_
   return (int64_t)(20u + ((0x0603090au >> (8u * cat)) & 0xffu)) - (int64_t)(s[3] - s[2]);
 }
 
+// Sort the segment sorted[s0, s0 + c) (any length) and keep greedily, one block: runs of kBlockSort bitonic-sorted in shared
+// memory, pairwise merges in HBM (through sort_tmp), the greedy walk by one thread.  The kept keys move to the segment's
+// front.  Returns the number kept and, redacting, *delta = the bytes their placeholders add (both on every thread).
+// Call from block-uniform code with blockDim.x == kSortBlock.
+__device__ uint32_t sort_keep_segment(const ScanWork& w, const uint32_t* __restrict__ category, uint32_t s0, uint32_t c, int redact,
+                                      long long* delta) {
+  __shared__ uint4 sk[kBlockSort];
+  __shared__ long long red[32];
+  __shared__ uint32_t kept_sh;
+  uint4* cur = w.sorted + s0; uint4* alt = w.sort_tmp + s0;
+  for (uint32_t base = 0; base < c; base += kBlockSort) {             // runs of kBlockSort: bitonic sort in shared memory
+    const uint32_t cc = min(kBlockSort, c - base);
+    uint32_t P = 64; while (P < cc) P <<= 1;
+    for (uint32_t i = threadIdx.x; i < P; i += blockDim.x) sk[i] = i < cc ? cur[base + i] : pad_key();
+    __syncthreads();
+    for (uint32_t k = 2; k <= P; k <<= 1)
+      for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+        for (uint32_t i = threadIdx.x; i < P; i += blockDim.x) {
+          const uint32_t p = i ^ j;
+          if (p > i) {
+            const uint4 a = sk[i], b = sk[p];
+            if (((i & k) == 0) ? key_less(b, a) : key_less(a, b)) { sk[i] = b; sk[p] = a; }
+          }
+        }
+        __syncthreads();
+      }
+    for (uint32_t i = threadIdx.x; i < cc; i += blockDim.x) cur[base + i] = sk[i];
+    __syncthreads();
+  }
+  for (uint64_t width = kBlockSort; width < c; width *= 2) {           // pairwise merges in HBM: each key finds its place by rank
+    for (uint32_t i = threadIdx.x; i < c; i += blockDim.x) {
+      const uint64_t a0 = (uint64_t)i / (2 * width) * (2 * width);
+      const uint32_t a1 = (uint32_t)min(a0 + width, (uint64_t)c), b1 = (uint32_t)min(a0 + 2 * width, (uint64_t)c);
+      const uint4 x = cur[i];
+      const uint32_t pos = i < a1 ? (i - (uint32_t)a0) + rank_in(cur + a1, b1 - a1, x, false)
+                                  : (i - a1) + rank_in(cur + a0, a1 - (uint32_t)a0, x, true);
+      alt[a0 + pos] = x;
+    }
+    __syncthreads();
+    uint4* t = cur; cur = alt; alt = t;
+  }
+  if (threadIdx.x == 0) {                                              // the greedy walk: kept keys to the segment's front
+    long long last_end = -1;
+    uint32_t k = 0;
+    for (uint32_t j = 0; j < c; j++) {
+      const uint4 x = cur[j];
+      if ((long long)x.x >= last_end) { w.sorted[s0 + k++] = x; last_end = key_end(x); }
+    }
+    kept_sh = k;
+  }
+  __syncthreads();
+  const uint32_t kc = kept_sh;
+  long long d = 0;
+  if (redact) for (uint32_t j = threadIdx.x; j < kc; j += blockDim.x) d += splice_delta(w, category, w.sorted[s0 + j]);
+  *delta = block_sum(d, red);
+  return kc;
+}
+
 // ---------------------------------------------------------------------------------------------- kernels
 __global__ void __launch_bounds__(256) span_count_kernel(ScanWork w) {
   const uint32_t ns = min(w.counters[2], w.span_cap);
@@ -153,9 +214,6 @@ __global__ void __launch_bounds__(256) span_scatter_kernel(ScanWork w, const uin
 // out_len[m] = the message's redacted length (redact only).
 __global__ void __launch_bounds__(kSortBlock) span_sort_keep_kernel(ScanWork w, const uint32_t* __restrict__ category, const uint32_t* __restrict__ off,
                                                                     uint32_t n, int redact) {
-  __shared__ uint4 sk[kBlockSort];
-  __shared__ long long red[32];
-  __shared__ uint32_t kept_sh;
   const uint32_t lane = threadIdx.x & 31;
   if (blockIdx.x == 0 && threadIdx.x == 0) { w.kept_cnt[n] = 0; w.out_len[n] = 0; }
 
@@ -193,55 +251,78 @@ __global__ void __launch_bounds__(kSortBlock) span_sort_keep_kernel(ScanWork w, 
   for (uint32_t m = blockIdx.x; m < n; m += gridDim.x) {
     const uint32_t s0 = w.seg_begin[m], c = w.seg_begin[m + 1] - s0;
     if (c <= kWarpSort) continue;
-    uint4* cur = w.sorted + s0; uint4* alt = w.sort_tmp + s0;
-    for (uint32_t base = 0; base < c; base += kBlockSort) {           // runs of kBlockSort: bitonic sort in shared memory
-      const uint32_t cc = min(kBlockSort, c - base);
-      uint32_t P = 64; while (P < cc) P <<= 1;
-      for (uint32_t i = threadIdx.x; i < P; i += blockDim.x) sk[i] = i < cc ? cur[base + i] : pad_key();
-      __syncthreads();
-      for (uint32_t k = 2; k <= P; k <<= 1)
-        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-          for (uint32_t i = threadIdx.x; i < P; i += blockDim.x) {
-            const uint32_t p = i ^ j;
-            if (p > i) {
-              const uint4 a = sk[i], b = sk[p];
-              if (((i & k) == 0) ? key_less(b, a) : key_less(a, b)) { sk[i] = b; sk[p] = a; }
-            }
-          }
-          __syncthreads();
-        }
-      for (uint32_t i = threadIdx.x; i < cc; i += blockDim.x) cur[base + i] = sk[i];
-      __syncthreads();
-    }
-    for (uint64_t width = kBlockSort; width < c; width *= 2) {         // pairwise merges in HBM: each key finds its place by rank
-      for (uint32_t i = threadIdx.x; i < c; i += blockDim.x) {
-        const uint64_t a0 = (uint64_t)i / (2 * width) * (2 * width);
-        const uint32_t a1 = (uint32_t)min(a0 + width, (uint64_t)c), b1 = (uint32_t)min(a0 + 2 * width, (uint64_t)c);
-        const uint4 x = cur[i];
-        const uint32_t pos = i < a1 ? (i - (uint32_t)a0) + rank_in(cur + a1, b1 - a1, x, false)
-                                    : (i - a1) + rank_in(cur + a0, a1 - (uint32_t)a0, x, true);
-        alt[a0 + pos] = x;
-      }
-      __syncthreads();
-      uint4* t = cur; cur = alt; alt = t;
-    }
-    if (threadIdx.x == 0) {                                            // the greedy walk: kept keys to the segment's front
-      long long last_end = -1;
-      uint32_t k = 0;
-      for (uint32_t j = 0; j < c; j++) {
-        const uint4 x = cur[j];
-        if ((long long)x.x >= last_end) { w.sorted[s0 + k++] = x; last_end = key_end(x); }
-      }
-      kept_sh = k;
-    }
-    __syncthreads();
-    const uint32_t kc = kept_sh;
     long long delta = 0;
-    if (redact) for (uint32_t j = threadIdx.x; j < kc; j += blockDim.x) delta += splice_delta(w, category, w.sorted[s0 + j]);
-    delta = block_sum(delta, red);
+    const uint32_t kc = sort_keep_segment(w, category, s0, c, redact, &delta);
     if (threadIdx.x == 0) { w.kept_cnt[m] = kc; if (redact) w.out_len[m] = (uint64_t)((long long)(off[m + 1] - off[m]) + delta); }
     __syncthreads();
   }
+}
+
+// The whole resolver for a batch of one message (cg_find_matches_one / cg_redact_one), one block: every raw span belongs to
+// message 0, so the keys are built straight from w.spans (no count, scan or scatter), sorted and kept by sort_keep_segment,
+// and everything span_emit_kernel writes is written here for n = 1.  The span count is read from device memory only.
+__global__ void __launch_bounds__(kSortBlock) span_resolve_one_kernel(ScanWork w, const uint32_t* __restrict__ category,
+                                                                      const uint32_t* __restrict__ rank, const uint32_t* __restrict__ off,
+                                                                      SpanOutputs o) {
+  const bool incomplete = w.counters[3] != 0;
+  const uint32_t c = incomplete ? 0u : min(w.counters[2], w.span_cap);
+  for (uint32_t i = threadIdx.x; i < c; i += blockDim.x) {
+    const uint32_t* s = w.spans + (size_t)i * 6;
+    w.sorted[i] = make_uint4(s[4], ~(s[5] - s[4]), rank[s[1]], i);
+  }
+  __syncthreads();
+  long long delta = 0;
+  const uint32_t total = sort_keep_segment(w, category, 0, c, o.redact ? 1 : 0, &delta);
+  const uint64_t need = o.redact ? (uint64_t)((long long)(off[1] - off[0]) + delta) : 0;
+  uint32_t status = kResolveOk;
+  if (!incomplete) {
+    if (o.redact && (need >> 32)) status = kResolveTooLarge;
+    else if (total > o.spans_cap || (o.redact && need > o.out_cap)) status = kResolveCapacity;
+  }
+  const bool go = !incomplete && status == kResolveOk;
+  for (uint32_t r = threadIdx.x; r < total; r += blockDim.x) {
+    const uint4 k = w.sorted[r];
+    const uint32_t* s = w.spans + (size_t)k.w * 6;
+    const uint32_t rule = s[1], sb = s[2], eb = s[3];
+    if (r < o.spans_cap) {
+      uint32_t* d = o.spans + (size_t)r * 6;
+      d[0] = 0; d[1] = rule; d[2] = sb; d[3] = eb; d[4] = s[4]; d[5] = s[5];
+    }
+    if (o.redact) { w.sp_start[r] = off[0] + sb; w.sp_len[r] = eb - sb; w.sp_cat[r] = category[rule]; }
+  }
+  if (threadIdx.x == 0) {
+    w.kept_begin[0] = 0; w.kept_begin[1] = total;
+    if (o.redact) {
+      w.out_off[0] = 0; w.out_off[1] = need;
+      o.out_offsets[0] = 0; o.out_offsets[1] = (uint32_t)need;
+      uint64_t* z = reinterpret_cast<uint64_t*>(o.sizes); z[0] = incomplete ? ~0ull : need; z[1] = incomplete ? ~0ull : total;
+    } else *reinterpret_cast<uint32_t*>(o.sizes) = incomplete ? ~0u : total;
+    w.counters[16] = status;
+    w.counters[20] = incomplete ? 0u : total;
+    w.counters[21] = go && o.redact ? total : 0u;
+    w.counters[22] = go && o.redact ? 1u : 0u;
+  }
+}
+
+// The one-message result made contiguous for one D2H copy (layout: kernels.h, launch_span_pack_one).  The spans and sizes
+// are already in place (the resolver wrote them there); this adds the status, the packed length, the counter block and,
+// redacting, the digests and the output bytes behind the spans -- when all of it fits in pack_cap bytes.
+__global__ void __launch_bounds__(512) span_pack_one_kernel(ScanWork w, const uint32_t* __restrict__ digests, const uint8_t* __restrict__ out,
+                                                            uint32_t* __restrict__ packed, uint32_t pack_cap, int redact) {
+  const uint32_t flags = w.counters[3], status = w.counters[16];
+  uint32_t ns = 0; uint64_t need = 0;
+  if (redact) { const uint64_t* z = reinterpret_cast<const uint64_t*>(packed + kPackSizes); need = z[0]; ns = (uint32_t)z[1]; }
+  else ns = packed[kPackSizes];
+  const uint64_t len = (uint64_t)kPackHeader + (uint64_t)ns * 24 + (redact ? (uint64_t)ns * 32 + need : 0);
+  const bool fits = !flags && status == kResolveOk && len <= pack_cap;
+  if (fits && redact) {
+    uint32_t* dd = packed + kPackHeader / 4 + (size_t)ns * 6;
+    for (uint32_t i = threadIdx.x; i < ns * 8; i += blockDim.x) dd[i] = digests[i];
+    uint8_t* ob = reinterpret_cast<uint8_t*>(dd + (size_t)ns * 8);
+    for (uint32_t i = threadIdx.x; i < need; i += blockDim.x) ob[i] = out[i];
+  }
+  if (threadIdx.x < kCounterWords) packed[kPackCounters + threadIdx.x] = w.counters[threadIdx.x];
+  if (threadIdx.x == 0) { packed[0] = fits ? (uint32_t)len : 0u; packed[1] = status; }
 }
 
 // Resolved span r = the (r - kept_begin[m])-th kept key of message m; sizes, status and the output offsets.
@@ -304,6 +385,17 @@ int launch_span_resolve(const ScanWork& w, const uint32_t* d_off, uint32_t n, co
   span_emit_kernel<<<sm_count * 4, 256, 0, stream>>>(w, w.rule_category, d_off, n, o);
   k++;
   return k;
+}
+
+int launch_span_resolve_one(const ScanWork& w, const uint32_t* d_off, const SpanOutputs& o, cudaStream_t stream) {
+  span_resolve_one_kernel<<<1, kSortBlock, 0, stream>>>(w, w.rule_category, w.rule_rank, d_off, o);
+  return 1;
+}
+
+int launch_span_pack_one(const ScanWork& w, const uint32_t* d_digests, const uint8_t* d_out, uint32_t* d_packed, uint32_t pack_cap, bool redact,
+                         cudaStream_t stream) {
+  span_pack_one_kernel<<<1, 512, 0, stream>>>(w, d_digests, d_out, d_packed, pack_cap, redact ? 1 : 0);
+  return 1;
 }
 
 }  // namespace cg

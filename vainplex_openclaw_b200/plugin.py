@@ -6,7 +6,7 @@ TypeScript equivalent a maintainer would ship is sketched in INTEGRATION.md).  E
 matches or hashes goes through the C ABI (include/openclaw_gov.h) to the CUDA kernels; this file
 only holds the host logic the reference also keeps on the host:
 
-  PatternRegistry    gov/src/redaction/registry.ts:165-316   (findMatches -> cg_find_matches_batch)
+  PatternRegistry    gov/src/redaction/registry.ts:165-316   (findMatches -> cg_find_matches_one / cg_redact_one)
   RedactionVault     gov/src/redaction/vault.ts:39-258        (sha256 -> cg_sha256_batch)
   RedactionEngine    gov/src/redaction/engine.ts:38-191
   evaluate_allowlist gov/src/redaction/allowlist.ts:35-85
@@ -23,7 +23,7 @@ from __future__ import annotations
 import json
 import re
 import time
-from typing import Any, Callable, Dict, Iterable, List, Optional, Sequence, Tuple
+from typing import Any, Callable, Dict, Iterable, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -111,8 +111,45 @@ class PatternRegistry:
             out[int(sp["msg"])].append({"pattern": self.patterns[int(sp["rule"])], "match": _slice16(s, a, b), "start": a, "end": b})
         return out
 
-    def find_matches(self, input: str) -> List[dict]:
-        return self.find_matches_batch([input])[0]
+    def find_matches(self, input: str, redact: bool = False) -> "Matches":
+        """findMatches for one string: one blocking device call.  The result is the list findMatches returns.
+
+        redact=False: cg_find_matches_one.  redact=True (RedactionEngine's scanString path): cg_redact_one, which finds the
+        same matches and also splices the default placeholders and hashes every match on the device; the result then carries
+        that in .redacted (see Matches).  Both go through this method so that a failing device call surfaces here, where
+        the reference's engine calls findMatches."""
+        rs = self._rs()
+        if rs is None:
+            return Matches()
+        enc = N.js_utf8(input)
+        if redact:
+            out_bytes, spans, digests = rs.redact_one(enc)
+            redacted = RedactedString(enc, out_bytes, spans, digests)
+        else:
+            spans, redacted = rs.find_matches_one(enc), None
+        out = Matches(redacted=redacted)
+        for sp in spans:
+            a, b = int(sp["start16"]), int(sp["end16"])
+            out.append({"pattern": self.patterns[int(sp["rule"])], "match": _slice16(input, a, b), "start": a, "end": b})
+        return out
+
+
+class RedactedString(NamedTuple):
+    """what cg_redact_one returns for one string: its UTF-8 bytes, the redacted bytes with the default placeholders, the
+    resolved spans and the SHA-256 of every match"""
+    enc: bytes
+    out: bytes
+    spans: np.ndarray
+    digests: np.ndarray
+
+
+class Matches(list):
+    """PatternRegistry.find_matches' result: the list findMatches returns; .redacted is the device's RedactedString when
+    it was asked for (redact=True), else None."""
+
+    def __init__(self, items=(), redacted: Optional[RedactedString] = None):
+        super().__init__(items)
+        self.redacted = redacted
 
 
 # ------------------------------------------------------------------------------------- vault
@@ -260,47 +297,74 @@ class RedactionEngine:
 
     def scan_strings(self, inputs: Sequence[str]) -> List[dict]:
         """scanString (engine.ts:74-85) for many strings with the splice done on the device (cg_redact_batch): matches,
-        SHA-256 of every match and the redacted text come back from one call; the vault learns the originals here.
-        A string whose placeholder the vault would issue in its 12-digit form (another live value shares hash8,
-        vault.ts:85-104) is re-spliced on the host."""
+        SHA-256 of every match and the redacted text come back from one call; the vault learns the originals here, in the
+        same loop as scan_string (_store_and_splice), so both give scanString's result.  A string is spliced on the host,
+        with the placeholders the vault returned (vault.store runs once per match), when the vault issues its 12-digit form
+        (another live value shares hash8, vault.ts:85-104), when the string has a lone surrogate or a match splits a
+        surrogate pair, or when several empty matches share a position (applyReplacements puts the last one first)."""
         rs = self.registry._rs()
         if rs is None or not inputs:
             return [{"output": s, "redactionCount": 0, "categories": set()} for s in inputs]
-        data, off = N.pack([N.js_utf8(s) for s in inputs])
+        enc = [N.js_utf8(s) for s in inputs]
+        data, off = N.pack(enc)
         out, out_off, spans, digests = rs.redact_batch(data, off)
         res = [{"output": s, "redactionCount": 0, "categories": set()} for s in inputs]
-        by_msg: Dict[int, list] = {}
-        for sp, dg in zip(spans, digests):
-            by_msg.setdefault(int(sp["msg"]), []).append((sp, bytes(dg).hex()))
-        for m, lst in by_msg.items():
-            s = inputs[m]
-            short = True
-            for sp, h in reversed(lst):                          # vault.store order of applyReplacements: last match first
-                cat = self.registry.patterns[int(sp["rule"])]["category"]
-                ph = self.vault.store(_slice16(s, int(sp["start16"]), int(sp["end16"])), cat, h)
-                short = short and ph == "[REDACTED:%s:%s]" % (cat, h[:8])
-                res[m]["redactionCount"] += 1
-                res[m]["categories"].add(cat)
-            if short:
-                res[m]["output"] = bytes(out[int(out_off[m]):int(out_off[m + 1])]).decode("utf-8", "surrogatepass")
-            else:
-                cats, count = set(), [0]
-                res[m]["output"] = self._redact_string(s, cats, count)
+        first = np.searchsorted(spans["msg"], np.arange(len(inputs) + 1)) if len(spans) else None
+        for m in (np.unique(spans["msg"]) if len(spans) else ()):
+            m = int(m)
+            a, b = int(first[m]), int(first[m + 1])
+            r = res[m]
+            r["output"] = self._store_and_splice(inputs[m], enc[m], bytes(out[int(out_off[m]):int(out_off[m + 1])]), spans[a:b], digests[a:b],
+                                                 r["categories"], r)
         return res
 
     def _redact_string(self, input: str, cats, count) -> str:
-        matches = self.registry.find_matches(input)
+        """scanString's splice for one string: one blocking device call (cg_redact_one) gives the spans, the SHA-256 of every
+        match and the redacted text; the vault learns the originals here."""
+        matches = self.registry.find_matches(input, redact=True)
         if not matches:
             return input
-        # applyReplacements (engine.ts:165-181): right to left; vault.store is called for the LAST match first
-        ordered = sorted(matches, key=lambda m: -m["start"])
-        hashes = sha256_hex([m["match"] for m in ordered])        # one batched device call
-        result = input
-        for m, h in zip(ordered, hashes):
-            ph = self.vault.store(m["match"], m["pattern"]["category"], h)
-            result = _slice16(result, 0, m["start"]) + ph + _slice16(result, m["end"], _js_len(result))
-            count[0] += 1
-            cats.add(m["pattern"]["category"])
+        r = matches.redacted
+        counter = {"redactionCount": 0}
+        result = self._store_and_splice(input, r.enc, r.out, r.spans, r.digests, cats, counter)
+        count[0] += counter["redactionCount"]
+        return result
+
+    def _store_and_splice(self, s: str, enc: bytes, out: bytes, spans, digests, cats, counter: dict) -> str:
+        """applyReplacements (engine.ts:165-181) for the resolved spans of one string s (enc = its UTF-8 bytes, out = the
+        device's redacted bytes): vault.store for every match, last match first, with the device's SHA-256 of the match.
+        The device text is the answer unless the vault issued a placeholder other than the default 8-digit one (another live
+        value shares hash8, vault.ts:85-104), or the bytes cannot stand for the JS string (a lone surrogate, a match that
+        splits a surrogate pair, several empty matches at one position): then s is spliced on the host, right to left, with
+        the placeholders the vault returned."""
+        starts = [int(x) for x in spans["start16"]]
+        order = sorted(range(len(starts)), key=lambda i: -starts[i])          # the reference's order: by start, descending, stable
+        device_text = len(set(starts)) == len(starts)
+        try:
+            device_text = device_text and s.encode("utf-8") == enc
+        except UnicodeEncodeError:
+            device_text = False
+        reps = []
+        for i in order:
+            sp = spans[i]
+            a, b = starts[i], int(sp["end16"])
+            match = _slice16(s, a, b)
+            if N.js_utf8(match) == enc[int(sp["start_byte"]):int(sp["end_byte"])]:
+                h = bytes(digests[i]).hex()
+            else:                                                            # the device hashed other bytes than createHash() would
+                h = sha256_hex([match])[0]
+                device_text = False
+            cat = self.registry.patterns[int(sp["rule"])]["category"]
+            ph = self.vault.store(match, cat, h)
+            device_text = device_text and ph == "[REDACTED:%s:%s]" % (cat, h[:8])
+            reps.append((a, b, ph))
+            counter["redactionCount"] += 1
+            cats.add(cat)
+        if device_text:
+            return out.decode("utf-8", "surrogatepass")
+        result = s
+        for a, b, ph in reps:
+            result = _slice16(result, 0, a) + ph + _slice16(result, b, _js_len(result))
         return result
 
 
