@@ -13,7 +13,9 @@
  * CUDA device every compute call fails with CG_ERR_CUDA / CG_ERR_NOT_INITIALIZED.
  *
  * Text encoding: message bytes are UTF-8 as produced by Buffer.from(str,'utf8') (lone
- * surrogates already replaced by U+FFFD).  All span offsets are reported both in bytes and in
+ * surrogates already replaced by U+FFFD).  Ill-formed bytes decode as TextDecoder decodes them:
+ * each maximal subpart of an ill-formed sequence becomes one U+FFFD (WHATWG Encoding, UTF-8
+ * decoder), and a sequence cut at a message's end never continues into the next message.  All span offsets are reported both in bytes and in
  * UTF-16 code units, the unit the reference's m.index / lastIndex use (registry.ts:226-231).
  */
 #ifndef OPENCLAW_GOV_H

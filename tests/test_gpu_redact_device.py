@@ -117,7 +117,8 @@ def find_device(N, torch, rs, data, off, cap=None):
 
 
 def splice_python(msgs, rules, spans, dig):
-    """applyReplacements restated: right to left, [REDACTED:<category>:<hash8>]"""
+    """applyReplacements restated: the spans in findMatches order, stably sorted by start, descending (several empty
+    matches at one position are inserted one in front of the other), [REDACTED:<category>:<hash8>]"""
     by_msg = {}
     for s, d in zip(spans, dig):
         m = msgs[int(s["msg"])][int(s["start_byte"]):int(s["end_byte"])]
@@ -126,7 +127,7 @@ def splice_python(msgs, rules, spans, dig):
     out = []
     for i, m in enumerate(msgs):
         e = bytearray(m)
-        for a, b, cat, h8 in sorted(by_msg.get(i, []), reverse=True):
+        for a, b, cat, h8 in sorted(by_msg.get(i, []), key=lambda r: -r[0]):
             e[a:b] = ("[REDACTED:%s:%s]" % (cat, h8)).encode()
         out.append(bytes(e))
     return out

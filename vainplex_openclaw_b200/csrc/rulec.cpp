@@ -511,7 +511,9 @@ struct Compiler {
   // literal is its UTF-8 bytes; any other set with members >= 0x80 is over-approximated by the three
   // byte shapes one decoded unit can have (1 byte; 2 bytes incl. half an astral pair or a truncated
   // sequence; 3 bytes) -- sound for ill-formed input too, since every U+FFFD the decoder emits
-  // covers 1-3 bytes of exactly these shapes.  *tight is cleared when the view over-approximates.
+  // covers 1-3 bytes of exactly these shapes.  U+FFFD itself therefore takes the three shapes even
+  // as a single literal: EF BF BD is only one of the byte strings it decodes from.  *tight is
+  // cleared when the view over-approximates.
   bool unit_bytes(int n, std::vector<FactorSeq>* seqs, bool* tight) const {
     Ranges r = unit_ranges(n);
     *tight = true;
@@ -520,7 +522,7 @@ struct Compiler {
     if (ascii_only) { if (lo.empty()) return false; seqs->push_back({lo}); return true; }
     if (r.size() == 1 && r[0].first == r[0].second) {      // single non-ASCII literal: its UTF-8 bytes
       int c = r[0].first;
-      if (!(c >= 0xd800 && c <= 0xdfff)) {
+      if (!(c >= 0xd800 && c <= 0xdfff) && c != 0xfffd) {
         FactorSeq s; ByteSet b0, b1, b2;
         if (c < 0x800) { b0.set(0xc0 | (c >> 6)); b1.set(0x80 | (c & 0x3f)); s = {b0, b1}; }
         else { b0.set(0xe0 | (c >> 12)); b1.set(0x80 | ((c >> 6) & 0x3f)); b2.set(0x80 | (c & 0x3f)); s = {b0, b1, b2}; }

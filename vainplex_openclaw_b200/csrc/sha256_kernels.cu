@@ -426,7 +426,9 @@ __constant__ char kCatName[4][12] = {"credential", "financial", "pii", "custom"}
 __constant__ uint8_t kCatLen[4] = {10, 9, 3, 6};
 
 // One warp per message: the text between spans is copied, every span is replaced by its placeholder.
-// span_begin[msg] .. span_begin[msg+1] index the (position-sorted, non-overlapping) spans of the message.
+// span_begin[msg] .. span_begin[msg+1] index the (position-sorted, non-overlapping) spans of the message.  Several empty
+// matches at one position come out last one first: applyReplacements sorts the matches by start, descending, with a stable
+// sort, and each of them is inserted in front of the ones before it.
 __global__ void __launch_bounds__(256) redact_splice_kernel(const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off,
                                                              const uint32_t* __restrict__ out_off, const uint32_t* __restrict__ span_begin,
                                                              const uint32_t* __restrict__ span_start, const uint32_t* __restrict__ span_len,
@@ -441,24 +443,29 @@ __global__ void __launch_bounds__(256) redact_splice_kernel(const uint8_t* __res
       for (uint32_t i = lane; i < stop - src; i += 32u) out[dst + i] = bytes[src + i];
       dst += stop - src;
       if (k == ke) break;
-      const uint32_t cat = span_cat[k] & 3u, cl = kCatLen[cat];
-      // "[REDACTED:" cat ":" hhhhhhhh "]"   = 10 + cl + 1 + 8 + 1 bytes, one byte per lane
-      const uint32_t plen = 20u + cl;
-      if (lane < plen) {
-        uint8_t ch;
-        if (lane < 10u) ch = (uint8_t)"[REDACTED:"[lane];
-        else if (lane < 10u + cl) ch = (uint8_t)kCatName[cat][lane - 10u];
-        else if (lane == 10u + cl) ch = ':';
-        else if (lane < 19u + cl) {
-          const uint32_t d = lane - (11u + cl);                   // hex digit 0..7 of the digest (bytes 0..3)
-          const uint32_t word = digests[(size_t)k * 8];           // stored big-endian byte order in memory: byte j = (word >> 8j) & 0xff
-          const uint32_t byte = (word >> (8u * (d >> 1))) & 0xffu, nib = (d & 1u) ? (byte & 15u) : (byte >> 4);
-          ch = (uint8_t)(nib < 10u ? '0' + nib : 'a' + nib - 10u);
-        } else ch = ']';
-        out[dst + lane] = ch;
+      uint32_t last = k;                                          // spans k .. last: one span, or a run of empty ones at one position
+      if (span_len[k] == 0u) while (last + 1u < ke && span_len[last + 1u] == 0u && span_start[last + 1u] == span_start[k]) last++;
+      for (uint32_t t = last + 1u; t-- > k;) {
+        const uint32_t cat = span_cat[t] & 3u, cl = kCatLen[cat];
+        // "[REDACTED:" cat ":" hhhhhhhh "]"   = 10 + cl + 1 + 8 + 1 bytes, one byte per lane
+        const uint32_t plen = 20u + cl;
+        if (lane < plen) {
+          uint8_t ch;
+          if (lane < 10u) ch = (uint8_t)"[REDACTED:"[lane];
+          else if (lane < 10u + cl) ch = (uint8_t)kCatName[cat][lane - 10u];
+          else if (lane == 10u + cl) ch = ':';
+          else if (lane < 19u + cl) {
+            const uint32_t d = lane - (11u + cl);                 // hex digit 0..7 of the digest (bytes 0..3)
+            const uint32_t word = digests[(size_t)t * 8];         // stored big-endian byte order in memory: byte j = (word >> 8j) & 0xff
+            const uint32_t byte = (word >> (8u * (d >> 1))) & 0xffu, nib = (d & 1u) ? (byte & 15u) : (byte >> 4);
+            ch = (uint8_t)(nib < 10u ? '0' + nib : 'a' + nib - 10u);
+          } else ch = ']';
+          out[dst + lane] = ch;
+        }
+        dst += plen;
       }
-      dst += plen;
       src = span_start[k] + span_len[k];
+      k = last;
     }
   }
 }
