@@ -265,6 +265,32 @@ CG_API int cg_merkle_verify_consistency(uint64_t first_size, uint64_t second_siz
 CG_API int cg_merkle_verify_proof(const uint8_t *leaf_bytes, uint64_t leaf_len, uint64_t index, uint64_t tree_size,
                                   const uint8_t *path32, uint32_t path_len, const uint8_t root[32], int *out_ok);
 
+/* ---- proofs at any tree size, in batches.  An auditor holds the root and size of an earlier day's log (the frontier
+ * persisted next to YYYY-MM-DD.jsonl, src/audit-trail.ts:151-179) and asks today's log for receipts against it, as RFC 6962 /
+ * CT get-proof-by-hash does with its tree_size.  A log made by cg_merkle_log_create_tree keeps its leaf digests and every
+ * complete aligned node MTH(D[j 2^h, (j + 1) 2^h)) -- fewer than n more digests, filled by the appends' own folds and frontier
+ * carries -- so a proof is a gather of at most 64 stored digests instead of a re-hash of the tree.  Its roots, frontiers and
+ * sizes equal those of a keep_leaf_digests = 1 log, and so do its appends' kernel launches; cg_merkle_log_proof and
+ * cg_merkle_log_consistency on it return the same bytes from the store.  Logs from cg_merkle_log_restore keep no nodes. */
+CG_API int cg_merkle_log_create_tree(cg_merkle_log **out);
+/* RFC 6962 2.1.1 PATH(index, D[0:tree_size]) for m indices; needs a log made by cg_merkle_log_create_tree.
+ * tree_size <= size of the log.  Path i (leaf level first) at out_paths32 + i * path_stride * 32, its length in out_lens[i];
+ * the stride's unused digests are zero.  Checked before anything is written: no node store -> CG_ERR_UNSUPPORTED; tree_size 0
+ * or past the log, or an index >= tree_size -> CG_ERR_INVALID_ARG; path_stride < ceil(log2 tree_size) -> CG_ERR_CAPACITY;
+ * m = 0 -> CG_OK with nothing written. */
+CG_API int cg_merkle_log_proofs(cg_merkle_log *log, const uint64_t *indices, uint32_t m, uint64_t tree_size,
+                                uint8_t *out_paths32, uint32_t path_stride, uint32_t *out_lens);
+/* RFC 6962 2.1.2 PROOF(first_size, D[0:second_size]) with second_size <= size of the log (1 <= first_size <= second_size);
+ * at most ceil(log2 second_size) + 1 digests.  Errors as for cg_merkle_log_proofs, *out_len and the path untouched. */
+CG_API int cg_merkle_log_consistency_between(cg_merkle_log *log, uint64_t first_size, uint64_t second_size,
+                                             uint8_t *out_path32, uint32_t path_cap, uint32_t *out_len);
+/* RFC 9162 2.1.3.2 for m (leaf, index, path) triples against one (tree_size, root): out_ok[i] = 1 iff proof i holds -- exactly
+ * when cg_merkle_verify_proof says so.  leaves: bytes/offsets as cg_merkle_root (ragged); paths at path_stride digests,
+ * lengths in path_lens (each <= 64 and <= path_stride, else CG_ERR_INVALID_ARG). */
+CG_API int cg_merkle_verify_proofs(const uint8_t *leaf_bytes, const uint64_t *leaf_offsets, const uint64_t *indices, uint32_t m,
+                                   uint64_t tree_size, const uint8_t *paths32, uint32_t path_stride, const uint32_t *path_lens,
+                                   const uint8_t root[32], uint8_t *out_ok);
+
 #ifdef __cplusplus
 }
 #endif

@@ -41,6 +41,11 @@ type Addon = {
   logFrontier(log: unknown): Uint8Array;
   logProof(log: unknown, index: bigint): Uint8Array;
   logConsistency(log: unknown, firstSize: bigint): Uint8Array;
+  logCreateTree(): unknown;
+  logProofs(log: unknown, indices: BigUint64Array, treeSize: bigint): { paths: Uint8Array; lens: Uint32Array };
+  logConsistencyBetween(log: unknown, firstSize: bigint, secondSize: bigint): Uint8Array;
+  verifyProofs(leafBytes: Uint8Array, leafOffsets: BigUint64Array, indices: BigUint64Array, treeSize: bigint, paths: Uint8Array,
+               lens: Uint32Array, stride: number, root: Uint8Array): Uint8Array;
 };
 
 const addon: Addon = require("./openclaw_gov.node");
@@ -153,4 +158,35 @@ export class AuditMerkleLog {
   state(): { size: bigint; frontier: Uint8Array } { return { size: addon.logSize(this.log), frontier: addon.logFrontier(this.log) }; }
   inclusionProof(index: bigint): Uint8Array { return addon.logProof(this.log, index); }
   consistencyProof(firstSize: bigint): Uint8Array { return addon.logConsistency(this.log, firstSize); }
+}
+
+/** The same log keeping every complete subtree node (logCreateTree): an auditor holding yesterday's (size, root) gets receipts
+ * for any records against that size, many per call, and checks a day's receipts in one call (RFC 6962 / RFC 9162). */
+export class AuditMerkleTreeLog {
+  private readonly log: unknown = addon.logCreateTree();
+  append(flushedBytes: Uint8Array): bigint { return addon.logAppendJsonl(this.log, flushedBytes); }
+  root(): string { return Buffer.from(addon.logRoot(this.log)).toString("hex"); }
+  /** one audit path per index against the tree of the first treeSize records, leaf level first */
+  inclusionProofs(indices: bigint[], treeSize: bigint): Uint8Array[] {
+    const { paths, lens } = addon.logProofs(this.log, BigUint64Array.from(indices), treeSize);
+    const stride = indices.length ? paths.length / 32 / indices.length : 0;
+    return indices.map((_, i) => paths.subarray(32 * stride * i, 32 * (stride * i + lens[i])));
+  }
+  consistencyProof(firstSize: bigint, secondSize: bigint): Uint8Array { return addon.logConsistencyBetween(this.log, firstSize, secondSize); }
+}
+
+/** RFC 9162 2.1.3.2 for many receipts against one (treeSize, root): records as written by flush() (one JSON line each,
+ * without its "\n"), their indices and paths -> per receipt whether it holds. */
+export function verifyInclusionProofs(records: string[], indices: bigint[], treeSize: bigint, paths: Uint8Array[], root: Uint8Array): boolean[] {
+  const parts = records.map((t) => enc.encode(t));
+  const offsets = new BigUint64Array(parts.length + 1);
+  parts.forEach((p, i) => (offsets[i + 1] = offsets[i] + BigInt(p.length)));
+  const bytes = new Uint8Array(Number(offsets[parts.length]) + 64);
+  parts.forEach((p, i) => bytes.set(p, Number(offsets[i])));
+  const stride = Math.max(1, ...paths.map((p) => p.length / 32));
+  const flat = new Uint8Array(paths.length * stride * 32);
+  paths.forEach((p, i) => flat.set(p, 32 * stride * i));
+  const lens = Uint32Array.from(paths.map((p) => p.length / 32));
+  const ok = addon.verifyProofs(bytes, offsets, BigUint64Array.from(indices), treeSize, flat, lens, stride, root);
+  return Array.from(ok, (v) => v !== 0);
 }

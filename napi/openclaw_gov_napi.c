@@ -30,6 +30,10 @@
  *   logProof(log, index: bigint): Uint8Array ; logConsistency(log, firstSize: bigint): Uint8Array      // 32 bytes per path node
  *   verifyProof(leaf: Uint8Array, index, treeSize, path: Uint8Array, root: Uint8Array): boolean
  *   verifyConsistency(firstSize, secondSize, rootFirst, rootSecond, path): boolean
+ *   logCreateTree(): External  // keeps every complete subtree node: receipts against any earlier size, in batches
+ *   logProofs(log, indices: BigUint64Array, treeSize): {paths: Uint8Array, lens: Uint32Array}  // stride max(1, ceil(log2 treeSize)) nodes
+ *   logConsistencyBetween(log, firstSize, secondSize): Uint8Array
+ *   verifyProofs(leafBytes, leafOffsets: BigUint64Array, indices: BigUint64Array, treeSize, paths, lens: Uint32Array, stride, root): Uint8Array (0/1)
  * Every failure throws a JS Error carrying cg_last_error(); the reference's try/catch + failMode
  * blocks (src/hooks.ts:232-241, src/redaction/hooks.ts:193-204) decide what happens next.
  * Offsets are validated here (non-decreasing, last one within the byte array): the C ABI trusts its caller.
@@ -262,6 +266,11 @@ static napi_value js_log_create(napi_env env, napi_callback_info info) {
   CG_CALL(env, cg_merkle_log_create(&L, keep ? 1 : 0));
   return wrap_log(env, L);
 }
+static napi_value js_log_create_tree(napi_env env, napi_callback_info info) {
+  (void)info; cg_merkle_log *L = NULL;
+  CG_CALL(env, cg_merkle_log_create_tree(&L));
+  return wrap_log(env, L);
+}
 static napi_value js_log_restore(napi_env env, napi_callback_info info) {
   ARGS(env, info, 2)
   uint64_t n; uint8_t *f; size_t nf; cg_merkle_log *L = NULL;
@@ -334,6 +343,52 @@ static napi_value js_verify_proof(napi_env env, napi_callback_info info) {
     napi_throw_type_error(env, NULL, "verifyProof(leaf, index, treeSize, path, root)"); return NULL; }
   CG_CALL(env, cg_merkle_verify_proof(leaf, nl, index, size, path, (uint32_t)(np / 32), root, &ok));
   NAPI_CALL(env, napi_get_boolean(env, ok != 0, &out));
+  return out;
+}
+/* logProofs(log, BigUint64Array indices, treeSize) -> { paths: Uint8Array (m x stride x 32, stride = max(1, ceil(log2 treeSize))), lens: Uint32Array } */
+static napi_value js_log_proofs(napi_env env, napi_callback_info info) {
+  ARGS(env, info, 3)
+  cg_merkle_log *L; uint8_t *ip; size_t ni; uint64_t size; napi_value res, paths, lens_ab, lens; void *lens_data;
+  NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&L));
+  if (!get_ta(env, argv[1], &ip, &ni, napi_biguint64_array) || !get_u64(env, argv[2], &size) || ni / 8 > UINT32_MAX) {
+    napi_throw_type_error(env, NULL, "logProofs(log, BigUint64Array, treeSize)"); return NULL; }
+  const uint32_t m = (uint32_t)(ni / 8);
+  uint32_t stride = 1; while (stride < 64 && size > (1ull << stride)) stride++;          /* ceil(log2 treeSize), at least 1 */
+  uint8_t *tmp = (uint8_t *)malloc((size_t)m * stride * 32 + 32);
+  if (!tmp) { napi_throw_error(env, NULL, "out of memory"); return NULL; }
+  NAPI_CALL(env, napi_create_arraybuffer(env, (size_t)m * 4 + 4, &lens_data, &lens_ab));
+  int rc = cg_merkle_log_proofs(L, (const uint64_t *)ip, m, size, tmp, stride, (uint32_t *)lens_data);
+  if (rc != CG_OK) { free(tmp); napi_throw_error(env, NULL, cg_last_error()); return NULL; }
+  paths = make_u8(env, tmp, (size_t)m * stride * 32);
+  free(tmp);
+  if (!paths) { napi_throw_error(env, NULL, "N-API call failed"); return NULL; }
+  NAPI_CALL(env, napi_create_typedarray(env, napi_uint32_array, m, lens_ab, 0, &lens));
+  NAPI_CALL(env, napi_create_object(env, &res));
+  NAPI_CALL(env, napi_set_named_property(env, res, "paths", paths)); NAPI_CALL(env, napi_set_named_property(env, res, "lens", lens));
+  return res;
+}
+static napi_value js_log_consistency_between(napi_env env, napi_callback_info info) {
+  ARGS(env, info, 3)
+  cg_merkle_log *L; uint64_t a, b; uint8_t p[65 * 32]; uint32_t k = 0;
+  NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&L));
+  if (!get_u64(env, argv[1], &a) || !get_u64(env, argv[2], &b)) { napi_throw_type_error(env, NULL, "logConsistencyBetween(log, firstSize, secondSize)"); return NULL; }
+  CG_CALL(env, cg_merkle_log_consistency_between(L, a, b, p, 65, &k));
+  return make_u8(env, p, (size_t)k * 32);
+}
+/* verifyProofs(leafBytes, BigUint64Array leafOffsets, BigUint64Array indices, treeSize, paths, Uint32Array lens, stride, root) -> Uint8Array */
+static napi_value js_verify_proofs(napi_env env, napi_callback_info info) {
+  ARGS(env, info, 8)
+  uint8_t *bytes, *offp, *ip, *paths, *lp, *root; size_t ni, np, nl, nr; uint64_t size; uint32_t stride;
+  const int64_t nn = get_batch(env, argv[0], argv[1], 1, &bytes, &offp); if (nn < 0) return NULL;
+  if (!get_ta(env, argv[2], &ip, &ni, napi_biguint64_array) || !get_u64(env, argv[3], &size) || !get_ta(env, argv[4], &paths, &np, napi_uint8_array) ||
+      !get_ta(env, argv[5], &lp, &nl, napi_uint32_array) || napi_get_value_uint32(env, argv[6], &stride) != napi_ok ||
+      !get_ta(env, argv[7], &root, &nr, napi_uint8_array) || nr != 32 || ni / 8 != (size_t)nn || nl / 4 != (size_t)nn ||
+      np < (size_t)nn * stride * 32 || nn > UINT32_MAX) {
+    napi_throw_type_error(env, NULL, "verifyProofs(leafBytes, leafOffsets, indices, treeSize, paths, lens, stride, root)"); return NULL; }
+  napi_value ab, out; void *ok;
+  NAPI_CALL(env, napi_create_arraybuffer(env, (size_t)nn + 1, &ok, &ab));
+  CG_CALL(env, cg_merkle_verify_proofs(bytes, (const uint64_t *)offp, (const uint64_t *)ip, (uint32_t)nn, size, paths, stride, (const uint32_t *)lp, root, (uint8_t *)ok));
+  NAPI_CALL(env, napi_create_typedarray(env, napi_uint8_array, (size_t)nn, ab, 0, &out));
   return out;
 }
 static napi_value js_verify_consistency(napi_env env, napi_callback_info info) {
@@ -437,6 +492,8 @@ static napi_value module_init(napi_env env, napi_value exports) {
     FN("logCreate", js_log_create), FN("logRestore", js_log_restore), FN("logAppend", js_log_append), FN("logAppendJsonl", js_log_append_jsonl),
     FN("logReserve", js_log_reserve), FN("logSize", js_log_size), FN("logRoot", js_log_root), FN("logFrontier", js_log_frontier),
     FN("logProof", js_log_proof), FN("logConsistency", js_log_consistency), FN("verifyProof", js_verify_proof), FN("verifyConsistency", js_verify_consistency),
+    FN("logCreateTree", js_log_create_tree), FN("logProofs", js_log_proofs), FN("logConsistencyBetween", js_log_consistency_between),
+    FN("verifyProofs", js_verify_proofs),
 #undef FN
   };
   if (napi_define_properties(env, exports, sizeof d / sizeof d[0], d) != napi_ok) return NULL;

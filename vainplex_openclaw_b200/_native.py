@@ -55,7 +55,8 @@ EXPORTS = ["cg_init", "cg_shutdown", "cg_last_error", "cg_version", "cg_device_c
            "cg_shard_range", "cg_comm_unique_id", "cg_comm_init", "cg_comm_destroy", "cg_merkle_root_sharded_device",
            "cg_ruleset_create", "cg_ruleset_destroy", "cg_ruleset_get_info", "cg_rule_check", "cg_scan_batch",
            "cg_scan_one", "cg_find_matches_batch", "cg_find_matches_one", "cg_redact_one", "cg_scan_batch_device", "cg_find_matches_batch_device", "cg_redact_batch_device", "cg_sha256_batch", "cg_merkle_root",
-           "cg_merkle_root_fixed", "cg_merkle_block_roots_device", "cg_merkle_fold", "cg_merkle_fold_device"]
+           "cg_merkle_root_fixed", "cg_merkle_block_roots_device", "cg_merkle_fold", "cg_merkle_fold_device",
+           "cg_merkle_log_create_tree", "cg_merkle_log_proofs", "cg_merkle_log_consistency_between", "cg_merkle_verify_proofs"]
 
 _lib = None
 
@@ -127,6 +128,10 @@ def load():
     L.cg_merkle_block_roots_device.argtypes = [vp, u64, u64, u32, vp, vp]; L.cg_merkle_block_roots_device.restype = i32
     L.cg_merkle_fold.argtypes = [vp, u64, vp]; L.cg_merkle_fold.restype = i32
     L.cg_merkle_fold_device.argtypes = [vp, u64, vp, vp]; L.cg_merkle_fold_device.restype = i32
+    L.cg_merkle_log_create_tree.argtypes = [vp]; L.cg_merkle_log_create_tree.restype = i32
+    L.cg_merkle_log_proofs.argtypes = [vp, vp, u32, u64, vp, u32, vp]; L.cg_merkle_log_proofs.restype = i32
+    L.cg_merkle_log_consistency_between.argtypes = [vp, u64, u64, vp, u32, vp]; L.cg_merkle_log_consistency_between.restype = i32
+    L.cg_merkle_verify_proofs.argtypes = [vp, vp, vp, u32, u64, vp, u32, vp, vp, vp]; L.cg_merkle_verify_proofs.restype = i32
     _lib = L
     return L
 
@@ -406,6 +411,13 @@ class MerkleLog:
         self.handle = h
 
     @classmethod
+    def tree(cls):
+        """a log that keeps every complete aligned node as well (cg_merkle_log_create_tree): proofs at any tree size."""
+        h = C.c_void_p()
+        check(load().cg_merkle_log_create_tree(C.byref(h)))
+        return cls(_handle=h)
+
+    @classmethod
     def restore(cls, n: int, frontier: np.ndarray):
         f = np.ascontiguousarray(frontier, dtype=np.uint8)
         h = C.c_void_p()
@@ -465,6 +477,24 @@ class MerkleLog:
         check(load().cg_merkle_log_proof(self.handle, index, out.ctypes.data, 64, C.byref(k)))
         return [out[i].tobytes() for i in range(k.value)]
 
+    def proofs(self, indices, tree_size=None):
+        """RFC 6962 audit paths of many leaves in the tree of the first tree_size leaves (default: the whole log); needs
+        MerkleLog.tree().  Returns (paths uint8[m, stride, 32] with stride = max(1, ceil(log2 tree_size)), lens uint32[m])."""
+        idx = np.ascontiguousarray(indices, dtype=np.uint64).reshape(-1)
+        s = self.size() if tree_size is None else tree_size
+        stride = max(1, (s - 1).bit_length()) if s else 1
+        paths = np.zeros((len(idx), stride, 32), dtype=np.uint8)
+        lens = np.zeros(len(idx), dtype=np.uint32)
+        check(load().cg_merkle_log_proofs(self.handle, idx.ctypes.data, len(idx), s, paths.ctypes.data, stride, lens.ctypes.data))
+        return paths, lens
+
+    def consistency_between(self, first_size: int, second_size: int):
+        """RFC 6962 consistency proof of the tree of first_size leaves in that of second_size leaves; needs MerkleLog.tree()."""
+        out = np.zeros((65, 32), dtype=np.uint8)
+        k = C.c_uint32(0)
+        check(load().cg_merkle_log_consistency_between(self.handle, first_size, second_size, out.ctypes.data, 65, C.byref(k)))
+        return [out[i].tobytes() for i in range(k.value)]
+
     def close(self):
         if self.handle:
             load().cg_merkle_log_destroy(self.handle)
@@ -515,3 +545,30 @@ def merkle_verify_proof(leaf: bytes, index: int, tree_size: int, path, root: byt
     ok = C.c_int(0)
     check(load().cg_merkle_verify_proof(lb.ctypes.data, len(leaf), index, tree_size, p.ctypes.data, len(path), r.ctypes.data, C.byref(ok)))
     return bool(ok.value)
+
+
+def merkle_verify_proofs(leaves, indices, tree_size: int, paths, root: bytes) -> np.ndarray:
+    """cg_merkle_verify_proofs: bool[m], proof i = (leaves[i], indices[i], paths[i]) against (tree_size, root).  leaves: a list
+    of bytes or (data uint8, off64 uint64[m + 1]); paths: a list of lists of 32-byte digests or (uint8[m, stride, 32], lens)
+    as MerkleLog.proofs returns them."""
+    if isinstance(leaves, tuple):
+        data, off = np.ascontiguousarray(leaves[0], dtype=np.uint8), np.ascontiguousarray(leaves[1], dtype=np.uint64)
+    else:
+        off = np.zeros(len(leaves) + 1, dtype=np.uint64)
+        off[1:] = np.cumsum([len(x) for x in leaves])
+        data = np.frombuffer(b"".join(leaves) + b"\0", dtype=np.uint8).copy()
+    if isinstance(paths, tuple):
+        p, lens = np.ascontiguousarray(paths[0], dtype=np.uint8), np.ascontiguousarray(paths[1], dtype=np.uint32)
+    else:
+        lens = np.array([len(x) for x in paths], dtype=np.uint32)
+        p = np.zeros((len(paths), max(1, int(lens.max()) if len(paths) else 1), 32), dtype=np.uint8)
+        for i, x in enumerate(paths):
+            if x:
+                p[i, :len(x)] = np.frombuffer(b"".join(x), dtype=np.uint8).reshape(-1, 32)
+    idx = np.ascontiguousarray(indices, dtype=np.uint64).reshape(-1)
+    m = len(idx)
+    r = np.frombuffer(root, dtype=np.uint8).copy()
+    ok = np.zeros(max(m, 1), dtype=np.uint8)
+    check(load().cg_merkle_verify_proofs(data.ctypes.data, off.ctypes.data, idx.ctypes.data, m, tree_size, p.ctypes.data, p.shape[1],
+                                         lens.ctypes.data, r.ctypes.data, ok.ctypes.data))
+    return ok[:m].astype(bool)

@@ -1216,7 +1216,16 @@ struct cg_merkle_log {
   uint32_t* d_leaves = nullptr; uint64_t cap_leaves = 0;     // keep: n leaf digests
   uint32_t* d_new = nullptr; size_t cap_new = 0;             // !keep: the current batch's leaf digests
   uint32_t* d_a = nullptr; size_t cap_a = 0; uint32_t* d_b = nullptr; size_t cap_b = 0;   // level ping-pong
-  ~cg_merkle_log() { cudaFree(d_slots); cudaFree(d_tmp); cudaFree(d_leaves); cudaFree(d_new); cudaFree(d_a); cudaFree(d_b); }
+  // tree (cg_merkle_log_create_tree): every complete aligned node as well -- level h >= 1 holds floor(n / 2^h) nodes at
+  // d_lvl[h] (node j covers leaves [j 2^h, (j + 1) 2^h)), each level sized cap_leaves >> h, so the store is smaller than the
+  // leaf digests; d_spine: 64 x 8 words, the suffix roots of the tree size of the last proof call (log_spine)
+  bool tree = false;
+  uint32_t* d_lvl[64] = {}; uint64_t cap_lvl[64] = {};
+  uint32_t* d_spine = nullptr;
+  ~cg_merkle_log() {
+    cudaFree(d_slots); cudaFree(d_tmp); cudaFree(d_leaves); cudaFree(d_new); cudaFree(d_a); cudaFree(d_b); cudaFree(d_spine);
+    for (uint32_t* p : d_lvl) cudaFree(p);
+  }
 };
 
 namespace {
@@ -1248,18 +1257,30 @@ int log_root_device(cg_merkle_log* L, cudaStream_t st) {
   count_launches(k);
   return CG_OK;
 }
+// node j of level h of a tree log (level 0: leaf digest j)
+uint32_t* log_node(cg_merkle_log* L, uint32_t h, uint64_t j) { return (h ? L->d_lvl[h] : L->d_leaves) + 8 * (size_t)j; }
+
+int log_new(cg_merkle_log** out, bool keep, bool tree) {
+  if (int rc = require_ready()) return rc;
+  if (!out) return fail(CG_ERR_INVALID_ARG, "null argument");
+  std::unique_ptr<cg_merkle_log> L(new cg_merkle_log());
+  L->keep = keep; L->tree = tree;
+  CU(cudaMalloc((void**)&L->d_slots, 64 * 32)); CU(cudaMalloc((void**)&L->d_tmp, 66 * 32));
+  CU(cudaMemset(L->d_slots, 0, 64 * 32));
+  if (tree) CU(cudaMalloc((void**)&L->d_spine, 64 * 32));
+  *out = L.release();
+  return CG_OK;
+}
 }  // namespace
 
 int cg_merkle_log_create(cg_merkle_log** out, int keep_leaf_digests) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (int rc = require_ready()) return rc;
-  if (!out) return fail(CG_ERR_INVALID_ARG, "null argument");
-  std::unique_ptr<cg_merkle_log> L(new cg_merkle_log());
-  L->keep = keep_leaf_digests != 0;
-  CU(cudaMalloc((void**)&L->d_slots, 64 * 32)); CU(cudaMalloc((void**)&L->d_tmp, 66 * 32));
-  CU(cudaMemset(L->d_slots, 0, 64 * 32));
-  *out = L.release();
-  return CG_OK;
+  return log_new(out, keep_leaf_digests != 0, false);
+}
+
+int cg_merkle_log_create_tree(cg_merkle_log** out) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return log_new(out, true, true);
 }
 void cg_merkle_log_destroy(cg_merkle_log* L) { std::lock_guard<std::mutex> lk(g_mu); if (L) { if (G.ready) cudaStreamSynchronize(G.stream); delete L; } }
 int cg_merkle_log_size(const cg_merkle_log* L, uint64_t* out_n) { if (!L || !out_n) return fail(CG_ERR_INVALID_ARG, "null argument"); *out_n = L->n; return CG_OK; }
@@ -1295,7 +1316,16 @@ int log_digest_room(cg_merkle_log* L, uint64_t m, cudaStream_t st, uint32_t** ou
       uint64_t cap = std::max<uint64_t>(L->n + m, L->cap_leaves * 2); uint32_t* nd = nullptr;
       CU(cudaMalloc((void**)&nd, (size_t)cap * 32));
       if (L->n) CU(cudaMemcpyAsync(nd, L->d_leaves, (size_t)L->n * 32, cudaMemcpyDeviceToDevice, st));
+      // a tree log's node levels follow: level h holds up to cap >> h nodes
+      uint32_t* nl[64] = {};
+      for (uint32_t h = 1; L->tree && h < 64 && (cap >> h); h++) {
+        if ((cap >> h) <= L->cap_lvl[h]) continue;
+        cudaError_t e = cudaMalloc((void**)&nl[h], (size_t)(cap >> h) * 32);
+        if (e != cudaSuccess) { cudaStreamSynchronize(st); cudaFree(nd); for (uint32_t* p : nl) cudaFree(p); return cuda_fail(e, "cudaMalloc"); }
+        if (L->n >> h) CU(cudaMemcpyAsync(nl[h], L->d_lvl[h], (size_t)(L->n >> h) * 32, cudaMemcpyDeviceToDevice, st));
+      }
       CU(cudaStreamSynchronize(st)); cudaFree(L->d_leaves); L->d_leaves = nd; L->cap_leaves = cap;
+      for (uint32_t h = 1; h < 64; h++) if (nl[h]) { cudaFree(L->d_lvl[h]); L->d_lvl[h] = nl[h]; L->cap_lvl[h] = cap >> h; }
     }
     *out = L->d_leaves + (size_t)L->n * 8;
   } else {
@@ -1312,9 +1342,24 @@ int log_absorb(cg_merkle_log* L, const uint32_t* d_dig, uint64_t m, cudaStream_t
   while (rem) {
     uint64_t s = pos ? (pos & (~pos + 1)) : (1ull << 63);
     while (s > rem) s >>= 1;
+    int h = 0; while ((1ull << h) < s) h++;
+    if (L->tree) {
+      // the block's fold writes its levels into the store (its root is node (h, pos >> h)); every carry above it makes the
+      // complete node (top, pos >> top) for the next occupied slot
+      uint32_t* lv[64] = {};
+      for (int l = 1; l <= h; l++) lv[l] = log_node(L, l, pos >> l);
+      const uint32_t* unused;
+      count_launches(launch_merkle_fold(log_node(L, 0, pos), s, 64, nullptr, nullptr, st, &unused, lv));
+      const uint32_t* acc = log_node(L, h, pos >> h);
+      ChainOperands ops{}; uint32_t nl = 0; int top = h;
+      while ((pos >> top) & 1ull) { ops.left[nl] = L->d_slots + 8 * top; top++; ops.keep[nl] = log_node(L, top, pos >> top); nl++; }
+      if (nl) { k = launch_merkle_chain_keep(ops, nl, acc, L->d_slots + 8 * top, st); count_launches(k); }
+      else CU(cudaMemcpyAsync(L->d_slots + 8 * top, acc, 32, cudaMemcpyDeviceToDevice, st));
+      pos += s; rem -= s;
+      continue;
+    }
     uint32_t* acc = L->d_tmp + 8 * 64;
     if ((rc = log_range_root(L, d_dig + (size_t)(pos - L->n) * 8, s, acc, st))) return rc;
-    int h = 0; while ((1ull << h) < s) h++;
     uint32_t nl = 0; int top = h;                           // slots h, h+1, ... that are occupied merge into the new subtree
     while ((pos >> top) & 1ull) { CU(cudaMemcpyAsync(L->d_tmp + 8 * nl, L->d_slots + 8 * top, 32, cudaMemcpyDeviceToDevice, st)); nl++; top++; }
     if (nl) { k = launch_merkle_chain(L->d_tmp, nl, acc, L->d_slots + 8 * top, st); count_launches(k); }
@@ -1419,12 +1464,87 @@ int cg_merkle_log_root(cg_merkle_log* L, uint8_t out_root[32]) {
   }
 }
 
+namespace {
+// Proofs on a tree log.  Every sibling range of RFC 6962's recursion over D[0:s] is a complete aligned node of the store or a
+// suffix D[a:s] whose root is a right-to-left fold of s's frontier subtrees: the spine.  spine[h] (h a set bit of s above its
+// lowest) = MTH(D[s with bits <= h cleared : s]), made by one chain over the frontier subtrees, which are stored nodes.
+int log_spine(cg_merkle_log* L, uint64_t s, cudaStream_t st) {
+  const int lowest = __builtin_ctzll(s);
+  ChainOperands ops{}; uint32_t nl = 0;
+  for (int h = lowest + 1; h < 64; h++) if ((s >> h) & 1ull) { ops.left[nl] = log_node(L, h, (s >> h) - 1); ops.keep[nl] = L->d_spine + 8 * h; nl++; }
+  count_launches(launch_merkle_chain_keep(ops, nl, log_node(L, lowest, (s >> lowest) - 1), nullptr, st));
+  return CG_OK;
+}
+NodeStore log_store(cg_merkle_log* L) {
+  NodeStore ns{};
+  for (uint32_t h = 0; h < 64; h++) ns.lvl[h] = h ? L->d_lvl[h] : L->d_leaves;
+  return ns;
+}
+// path lengths (host side of the gather's rule): inclusion of leaf i, and PROOF(first, D[0:size])
+uint32_t inclusion_len(uint64_t i, uint64_t size) { return (uint32_t)__builtin_popcountll(merkle_path_levels(i, size, 0)); }
+uint32_t consistency_len(uint64_t first, uint64_t size) {
+  if (first == size) return 0;
+  return (uint32_t)__builtin_popcountll(merkle_path_levels(first - 1, size, __builtin_ctzll(first))) + ((first & (first - 1)) ? 1u : 0u);
+}
+// the spine of `size`, then m paths (leaf indices h_idx, or one consistency proof from `first` when h_idx is null) at `stride`
+// digests each -> out_paths32 (host), their lengths -> out_lens (host, may be null).  Two launches, whatever m and size.
+int log_gather(cg_merkle_log* L, const uint64_t* h_idx, uint32_t m, uint64_t size, uint64_t first, uint8_t* out_paths32, uint32_t stride,
+               uint32_t* out_lens) {
+  cudaStream_t st = G.stream; int rc;
+  const size_t path_words = (size_t)m * stride * 8, lens_words = ((size_t)m + 7) / 8 * 8;
+  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], path_words + lens_words))) return rc;
+  if (h_idx && (rc = grow(&G.d_off64, &G.cap_off64, (size_t)m))) return rc;
+  uint32_t* d_paths = G.d_dig[0]; uint32_t* d_lens = d_paths + path_words;
+  if (h_idx) CU(cudaMemcpyAsync(G.d_off64, h_idx, (size_t)m * 8, cudaMemcpyHostToDevice, st));
+  if ((rc = log_spine(L, size, st))) return rc;
+  count_launches(launch_merkle_gather(log_store(L), L->d_spine, size, h_idx ? G.d_off64 : nullptr, first, m, stride, d_paths, d_lens, G.sm_count, st));
+  CU(cudaGetLastError());
+  if (path_words) CU(cudaMemcpyAsync(out_paths32, d_paths, path_words * 4, cudaMemcpyDeviceToHost, st));
+  if (out_lens) CU(cudaMemcpyAsync(out_lens, d_lens, (size_t)m * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return CG_OK;
+}
+}  // namespace
+
+int cg_merkle_log_proofs(cg_merkle_log* L, const uint64_t* indices, uint32_t m, uint64_t tree_size, uint8_t* out_paths32, uint32_t path_stride,
+                         uint32_t* out_lens) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  int rc = log_check(L); if (rc) return rc;
+  if (!L->tree) return fail(CG_ERR_UNSUPPORTED, "proofs at any tree size need a log made by cg_merkle_log_create_tree");
+  if (tree_size == 0 || tree_size > L->n) return fail(CG_ERR_INVALID_ARG, "tree_size must be in [1, size of the log]");
+  if (!m) return CG_OK;
+  if (!indices || !out_lens || (path_stride && !out_paths32)) return fail(CG_ERR_INVALID_ARG, "null argument");
+  for (uint32_t i = 0; i < m; i++) if (indices[i] >= tree_size) return fail(CG_ERR_INVALID_ARG, "leaf index out of range");
+  const uint32_t longest = tree_size > 1 ? 64 - (uint32_t)__builtin_clzll(tree_size - 1) : 0;       // ceil(log2 tree_size)
+  if (path_stride < longest) return fail(CG_ERR_CAPACITY, "path_stride is below ceil(log2 tree_size)");
+  return log_gather(L, indices, m, tree_size, 0, out_paths32, path_stride, out_lens);
+}
+
+int cg_merkle_log_consistency_between(cg_merkle_log* L, uint64_t first_size, uint64_t second_size, uint8_t* out_path32, uint32_t path_cap, uint32_t* out_len) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  int rc = log_check(L); if (rc) return rc;
+  if (!out_len) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (!L->tree) return fail(CG_ERR_UNSUPPORTED, "proofs at any tree size need a log made by cg_merkle_log_create_tree");
+  if (second_size == 0 || second_size > L->n || first_size == 0 || first_size > second_size)
+    return fail(CG_ERR_INVALID_ARG, "need 1 <= first_size <= second_size <= size of the log");
+  const uint32_t len = consistency_len(first_size, second_size);
+  if (len > path_cap || (len && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
+  *out_len = len;
+  return len ? log_gather(L, nullptr, 1, second_size, first_size, out_path32, len, nullptr) : CG_OK;
+}
+
 int cg_merkle_log_proof(cg_merkle_log* L, uint64_t index, uint8_t* out_path32, uint32_t path_cap, uint32_t* out_len) {
   std::lock_guard<std::mutex> lk(g_mu);
   int rc = log_check(L); if (rc) return rc;
   if (!out_len) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (!L->keep) return fail(CG_ERR_UNSUPPORTED, "log was created without leaf digests (or restored from a frontier): no proofs");
   if (index >= L->n) return fail(CG_ERR_INVALID_ARG, "leaf index out of range");
+  if (L->tree) {                                            // from the node store: the same path, two launches
+    const uint32_t len = inclusion_len(index, L->n);
+    *out_len = len;
+    if (len > path_cap || (len && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
+    return len ? log_gather(L, &index, 1, L->n, 0, out_path32, len, nullptr) : CG_OK;
+  }
   // RFC 6962 2.1.1: PATH(m, D[n]) -- the sibling subtree at every split on the way down, returned leaf level first
   std::vector<std::pair<uint64_t, uint64_t>> sib;
   uint64_t lo = 0, hi = L->n;
@@ -1451,6 +1571,12 @@ int cg_merkle_log_consistency(cg_merkle_log* L, uint64_t first_size, uint8_t* ou
   if (!out_len) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (!L->keep) return fail(CG_ERR_UNSUPPORTED, "log was created without leaf digests (or restored from a frontier): no proofs");
   if (first_size == 0 || first_size > L->n) return fail(CG_ERR_INVALID_ARG, "first_size must be in [1, size of the log]");
+  if (L->tree) {                                            // from the node store: the same proof, two launches
+    const uint32_t len = consistency_len(first_size, L->n);
+    *out_len = len;
+    if (len > path_cap || len > 64 || (len && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
+    return len ? log_gather(L, nullptr, 1, L->n, first_size, out_path32, len, nullptr) : CG_OK;
+  }
   // SUBPROOF(m, D[lo:hi], b): k = largest power of two < hi - lo; m <= k: recurse left, then MTH(D[lo+k:hi]);
   // else recurse right with b = false, then MTH(D[lo:lo+k]); m == hi - lo: {} if b else {MTH(D[lo:hi])}
   std::vector<std::pair<uint64_t, uint64_t>> ranges;      // in proof order
@@ -1521,6 +1647,46 @@ int cg_merkle_verify_proof(const uint8_t* leaf_bytes, uint64_t leaf_len, uint64_
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
   *out_ok = (int)ok;
+  return CG_OK;
+}
+
+/* m proofs against one (tree_size, root): the leaves are hashed by the word-granular leaf kernel over the staging buffer, then
+ * one thread per proof walks its path (the walk of the single-proof verifier).  Two launches, whatever m. */
+int cg_merkle_verify_proofs(const uint8_t* leaf_bytes, const uint64_t* leaf_offsets, const uint64_t* indices, uint32_t m, uint64_t tree_size,
+                            const uint8_t* paths32, uint32_t path_stride, const uint32_t* path_lens, const uint8_t root[32], uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  if (!m) return CG_OK;
+  if (!leaf_offsets || !indices || !path_lens || !root || !out_ok || (path_stride && !paths32)) return fail(CG_ERR_INVALID_ARG, "null argument");
+  for (uint32_t i = 0; i < m; i++) {
+    if (leaf_offsets[i + 1] < leaf_offsets[i]) return fail(CG_ERR_INVALID_ARG, "offsets must be non-decreasing");
+    if (path_lens[i] > 64 || path_lens[i] > path_stride) return fail(CG_ERR_INVALID_ARG, "a path is longer than 64 digests or than path_stride");
+  }
+  const size_t total = leaf_offsets[m];
+  if (total && !leaf_bytes) return fail(CG_ERR_INVALID_ARG, "null argument");
+  int rc; cudaStream_t st = G.stream;
+  // d_dig[0]: leaf digests | root ; d_dig[1]: paths | indices | lengths | verdicts (every region a multiple of 32 bytes)
+  const size_t leaf_words = (size_t)m * 8, path_words = (size_t)m * path_stride * 8, idx_words = ((size_t)m * 2 + 7) / 8 * 8,
+               len_words = ((size_t)m + 7) / 8 * 8, ok_words = ((size_t)m + 31) / 32 * 8;
+  if ((rc = grow_bytes(total + 64))) return rc;
+  if ((rc = grow(&G.d_off64, &G.cap_off64, (size_t)m + 1))) return rc;
+  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], leaf_words + 8))) return rc;
+  if ((rc = grow(&G.d_dig[1], &G.cap_dig[1], path_words + idx_words + len_words + ok_words))) return rc;
+  uint32_t* d_leaf = G.d_dig[0]; uint32_t* d_root = d_leaf + leaf_words;
+  uint32_t* d_paths = G.d_dig[1]; uint64_t* d_idx = reinterpret_cast<uint64_t*>(d_paths + path_words);
+  uint32_t* d_lens = d_paths + path_words + idx_words; uint8_t* d_ok = reinterpret_cast<uint8_t*>(d_lens + len_words);
+  if (total) CU(cudaMemcpyAsync(G.d_bytes, leaf_bytes, total, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(G.d_off64, leaf_offsets, ((size_t)m + 1) * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_root, root, 32, cudaMemcpyHostToDevice, st));
+  if (path_words) CU(cudaMemcpyAsync(d_paths, paths32, path_words * 4, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_idx, indices, (size_t)m * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_lens, path_lens, (size_t)m * 4, cudaMemcpyHostToDevice, st));
+  int k = launch_merkle_leaves_var(G.d_bytes, G.d_off64, m, d_leaf, st);
+  k += launch_merkle_verify_batch(d_leaf, d_idx, m, tree_size, d_paths, path_stride, d_lens, d_root, d_ok, G.sm_count, st);
+  count_launches(k);
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(out_ok, d_ok, m, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   return CG_OK;
 }
 

@@ -180,7 +180,37 @@ int launch_newline_starts(const uint8_t* d_bytes, uint64_t len, const uint32_t* 
 int launch_merkle_consistency(uint64_t first, uint64_t second, const uint32_t* d_first32, const uint32_t* d_second32, const uint32_t* d_path, uint32_t path_len, uint32_t* d_ok, cudaStream_t stream);
 // fold the n nodes at d_in (16-byte aligned) level by level until one is left or max_levels levels are done; the first level
 // writes d_a, later ones d_b, d_a, ...; only the first reads d_in (d_b may be d_in).  *d_result = the folded nodes.
+// d_levels (a host array, indexed by level): level l >= 1 goes to d_levels[l] instead, every level of the fold kept.
 int launch_merkle_fold(const uint32_t* d_in, uint64_t n, uint32_t max_levels, uint32_t* d_a, uint32_t* d_b, cudaStream_t stream,
-                       const uint32_t** d_result);
+                       const uint32_t** d_result, uint32_t* const* d_levels = nullptr);
+
+// Logs that keep their complete aligned nodes (cg_merkle_log_create_tree).  Kernel arguments by value:
+struct FoldLevels { uint32_t* p[5]; };                                  // merkle_reduce_kernel: intermediate level s + 1 -> p[s]
+struct ChainOperands { const uint32_t* left[64]; uint32_t* keep[64]; };  // chain step k: acc = node(*left[k], acc) -> keep[k]
+struct NodeStore { const uint32_t* lvl[64]; };                          // level h of the store (level 0: the leaf digests)
+// acc = node(left[k], acc) for k < n_left, keeping every intermediate (frontier carries into the store, the spine of a size)
+int launch_merkle_chain_keep(const ChainOperands& ops, uint32_t n_left, const uint32_t* d_acc_in, uint32_t* d_acc_out, cudaStream_t stream);
+
+// The levels at which PATH(i, D[0:size]) (RFC 6962 2.1.1) has an element, from level lo up: bit l set <=> one element at level
+// l, the sibling range of i's level-l ancestor.  Below inner = bit length of i ^ (size - 1) the ancestor of i is left of that of
+// leaf size - 1, so every level has a sibling (the one at level inner - 1 ends at size); from inner up the two ancestors are
+// the same node and only a left sibling (bit l of i set) exists -- a right one would lie past the end and is promoted.
+__host__ __device__ inline uint64_t merkle_path_levels(uint64_t i, uint64_t size, uint32_t lo) {
+  const uint64_t x = i ^ (size - 1);
+  uint32_t inner = 0;
+  while (inner < 64 && (x >> inner)) inner++;
+  const uint64_t below = inner >= 64 ? ~0ull : (1ull << inner) - 1;
+  return (below | (i & ~below)) & ~((1ull << lo) - 1);
+}
+// paths from the store: one warp per path, kGatherWarps per block, at most kGatherBlocksPerSm blocks per SM (grid-stride);
+// d_idx = leaf indices, or null: one consistency proof PROOF(first, D[0:size]).  d_spine: spine of `size` (chain_keep).
+constexpr uint32_t kGatherWarps = 8, kGatherBlocksPerSm = 8;
+int launch_merkle_gather(const NodeStore& st, const uint32_t* d_spine, uint64_t size, const uint64_t* d_idx, uint64_t first, uint32_t m, uint32_t stride,
+                         uint32_t* d_out, uint32_t* d_lens, int sm_count, cudaStream_t stream);
+// RFC 9162 2.1.3.2 for m proofs against one (size, root): one thread per proof, kProofVerifyBlock threads per block, at most
+// kProofVerifyBlocksPerSm blocks per SM (grid-stride); d_ok[i] = 1 iff proof i holds
+constexpr uint32_t kProofVerifyBlock = 128, kProofVerifyBlocksPerSm = 16;
+int launch_merkle_verify_batch(const uint32_t* d_leaf32, const uint64_t* d_idx, uint32_t m, uint64_t size, const uint32_t* d_paths, uint32_t stride,
+                               const uint32_t* d_lens, const uint32_t* d_root32, uint8_t* d_ok, int sm_count, cudaStream_t stream);
 
 }  // namespace cg

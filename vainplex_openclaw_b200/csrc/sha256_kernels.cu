@@ -241,16 +241,27 @@ __global__ void merkle_chain_kernel(const uint32_t* __restrict__ left, uint32_t 
     for (int t = 0; t < 8; t++) r[t] = h[t]; }
   store_digest(acc_out, r);
 }
-// RFC 9162 2.1.3.2: does `path` prove that the leaf with digest leaf32 is entry `index` of the tree of `size` leaves with root `root32`?
-__global__ void merkle_verify_kernel(const uint32_t* __restrict__ leaf32, unsigned long long index, unsigned long long size,
-                                     const uint32_t* __restrict__ path, uint32_t path_len, const uint32_t* __restrict__ root32, uint32_t* __restrict__ ok) {
+// The same chain with its left operands anywhere (ops.left[k]), keeping the accumulator after step k at ops.keep[k] too:
+// the frontier carries of a log that keeps its nodes (each intermediate accumulator is a complete aligned node) and the
+// spine of a tree size (each intermediate is the root of a suffix of the leaves).  acc_out may be null.
+__global__ void merkle_chain_keep_kernel(ChainOperands ops, uint32_t n_left, const uint32_t* __restrict__ acc_in, uint32_t* __restrict__ acc_out) {
   if (threadIdx.x || blockIdx.x) return;
-  *ok = 0;
-  if (index >= size) return;
+  uint32_t r[8]; load_digest(acc_in, r);
+  for (uint32_t k = 0; k < n_left; k++) { uint32_t l[8], h[8]; load_digest(ops.left[k], l); merkle_node(l, r, h);
+#pragma unroll
+    for (int t = 0; t < 8; t++) r[t] = h[t];
+    store_digest(ops.keep[k], r); }
+  if (acc_out) store_digest(acc_out, r);
+}
+// RFC 9162 2.1.3.2: does `path` prove that the leaf with digest leaf32 is entry `index` of the tree of `size` leaves with root
+// `root32`?  At most path_len node hashes; the single-proof and the batched verifier both ask this function.
+__device__ bool merkle_verify_path(const uint32_t* __restrict__ leaf32, unsigned long long index, unsigned long long size,
+                                   const uint32_t* __restrict__ path, uint32_t path_len, const uint32_t* __restrict__ root32) {
+  if (index >= size) return false;
   unsigned long long fn = index, sn = size - 1;
   uint32_t r[8]; load_digest(leaf32, r);
   for (uint32_t k = 0; k < path_len; k++) {
-    if (sn == 0) return;
+    if (sn == 0) return false;
     uint32_t p[8], h[8]; load_digest(path + 8 * k, p);
     if ((fn & 1ull) || fn == sn) {
       merkle_node(p, r, h);
@@ -260,12 +271,64 @@ __global__ void merkle_verify_kernel(const uint32_t* __restrict__ leaf32, unsign
     for (int t = 0; t < 8; t++) r[t] = h[t];
     fn >>= 1; sn >>= 1;
   }
-  if (sn != 0) return;
+  if (sn != 0) return false;
   uint32_t q[8]; load_digest(root32, q);
   bool eq = true;
 #pragma unroll
   for (int t = 0; t < 8; t++) eq = eq && q[t] == r[t];
-  *ok = eq ? 1u : 0u;
+  return eq;
+}
+__global__ void merkle_verify_kernel(const uint32_t* __restrict__ leaf32, unsigned long long index, unsigned long long size,
+                                     const uint32_t* __restrict__ path, uint32_t path_len, const uint32_t* __restrict__ root32, uint32_t* __restrict__ ok) {
+  if (threadIdx.x || blockIdx.x) return;
+  *ok = merkle_verify_path(leaf32, index, size, path, path_len, root32) ? 1u : 0u;
+}
+// m proofs against one (size, root), one thread per proof: proof i = leaf digest leaf32[i], index idx[i], the path_lens[i]
+// digests at paths + 8 i stride.  Grid-stride over the proofs.
+__global__ void __launch_bounds__(128) merkle_verify_batch_kernel(const uint32_t* __restrict__ leaf32, const uint64_t* __restrict__ idx, uint32_t m,
+                                                                  unsigned long long size, const uint32_t* __restrict__ paths, uint32_t stride,
+                                                                  const uint32_t* __restrict__ path_lens, const uint32_t* __restrict__ root32, uint8_t* __restrict__ ok) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x)
+    ok[i] = merkle_verify_path(leaf32 + 8 * (size_t)i, idx[i], size, paths + (size_t)i * stride * 8, path_lens[i], root32) ? 1 : 0;
+}
+
+// Paths from a log's node store.  Element `pos` of the path of leaf i in the tree of `size` leaves (merkle_path_levels: the
+// element at level l is the sibling range of i's level-l ancestor, [b, min(b + 2^l, size)) with b = ((i >> l) ^ 1) << l).  A
+// range of 2^h leaves is a complete aligned node, read from level h of the store; any other range ends at `size` and is the
+// suffix root spine[msb of its width].  Consistency proofs (first != 0) are the path of leaf first - 1 from level
+// ctz(first) up, behind the node (ctz(first), (first - 1) >> ctz(first)) unless first is a power of two.
+__device__ __forceinline__ const uint32_t* merkle_path_element(const NodeStore& st, const uint32_t* spine, uint64_t size, uint64_t i,
+                                                               uint64_t levels, uint32_t lo, bool seed, uint32_t pos) {
+  if (seed && pos == 0) return st.lvl[lo] + 8 * (i >> lo);
+  for (uint32_t q = pos - (seed ? 1u : 0u); q; q--) levels &= levels - 1;      // the q-th set level
+  const uint32_t l = __ffsll((long long)levels) - 1;
+  const uint64_t b = ((i >> l) ^ 1ull) << l, w = (size - b) < (1ull << l) ? size - b : (1ull << l);
+  const uint32_t h = 63 - __clzll(w);
+  return (w & (w - 1)) ? spine + 8 * h : st.lvl[h] + 8 * (b >> h);
+}
+// One warp per path (grid-stride): lane p copies elements p, p + 32, ... into out + 8 (item stride + p) and zeros the
+// stride's unused tail; lens[item] = the path's length.  idx: leaf indices; null: one consistency proof from `first`.
+__global__ void __launch_bounds__(256) merkle_gather_kernel(NodeStore st, const uint32_t* __restrict__ spine, uint64_t size, const uint64_t* __restrict__ idx,
+                                                            uint64_t first, uint32_t m, uint32_t stride, uint32_t* __restrict__ out, uint32_t* __restrict__ lens) {
+  const uint32_t lane = threadIdx.x & 31u, wpb = blockDim.x >> 5;
+  for (uint32_t item = blockIdx.x * wpb + (threadIdx.x >> 5); item < m; item += gridDim.x * wpb) {
+    uint64_t i; uint32_t lo = 0; bool seed = false;
+    if (idx) i = idx[item];
+    else { i = first - 1; lo = __ffsll((long long)first) - 1; seed = (first & (first - 1)) != 0; }
+    uint64_t levels = merkle_path_levels(i, size, lo);
+    if (!idx && first == size) { levels = 0; seed = false; }
+    const uint32_t len = __popcll(levels) + (seed ? 1u : 0u);
+    for (uint32_t p = lane; p < stride; p += 32u) {
+      uint4 a = make_uint4(0, 0, 0, 0), b = a;
+      if (p < len) {
+        const uint4* src = reinterpret_cast<const uint4*>(merkle_path_element(st, spine, size, i, levels, lo, seed, p));
+        a = src[0]; b = src[1];
+      }
+      uint4* dst = reinterpret_cast<uint4*>(out + ((size_t)item * stride + p) * 8);
+      dst[0] = a; dst[1] = b;
+    }
+    if (lane == 0) lens[item] = len;
+  }
 }
 // RFC 9162 2.1.4.2: does `path` prove that the tree of `first` leaves with root first32 is a prefix of the tree of
 // `second` leaves with root second32?
@@ -301,8 +364,11 @@ __global__ void merkle_consistency_kernel(unsigned long long first, unsigned lon
 // pairwise reduction runs through shuffles -- at step s the lanes with (i mod 2^(s+1)) == 0 hash their node with the one
 // 2^s lanes up, an unpaired node is promoted unchanged -- and only the group's root goes back to HBM.  Used for the small
 // upper levels of every tree and for the short trees of log appends, where a kernel launch per level costs more than the
-// idle lanes do (the large lower levels keep every lane busy in merkle_level_kernel).
-__global__ void __launch_bounds__(256) merkle_reduce_kernel(const uint32_t* __restrict__ in, uint64_t n_in, uint32_t levels, uint32_t* __restrict__ out) {
+// idle lanes do (the large lower levels keep every lane busy in merkle_level_kernel).  kKeep: every intermediate level s + 1
+// (s + 1 < levels) goes to keep.p[s] as well, node j of that level at keep.p[s] + 8 j (a log's node store).
+template <bool kKeep>
+__global__ void __launch_bounds__(256) merkle_reduce_kernel(const uint32_t* __restrict__ in, uint64_t n_in, uint32_t levels, uint32_t* __restrict__ out,
+                                                            FoldLevels keep) {
   const uint32_t lane = threadIdx.x & 31u, span = 1u << levels;                   // nodes per group (<= 32)
   const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint32_t gpw = 32u >> levels;                                             // groups per warp
@@ -321,6 +387,7 @@ __global__ void __launch_bounds__(256) merkle_reduce_kernel(const uint32_t* __re
 #pragma unroll
       for (int t = 0; t < 8; t++) d[t] = h[t];
     }
+    if (kKeep && s + 1 < levels && ((lane & (span - 1)) & ((2u << s) - 1u)) == 0 && have) store_digest(keep.p[s] + 8 * (node >> (s + 1)), d);
   }
   if ((lane & (span - 1)) == 0 && have) store_digest(out + 8 * group, d);
 }
@@ -404,6 +471,24 @@ int launch_merkle_chain(const uint32_t* d_left, uint32_t n_left, const uint32_t*
 }
 int launch_merkle_verify(const uint32_t* d_leaf32, uint64_t index, uint64_t size, const uint32_t* d_path, uint32_t path_len, const uint32_t* d_root32, uint32_t* d_ok, cudaStream_t stream) {
   merkle_verify_kernel<<<1, 32, 0, stream>>>(d_leaf32, index, size, d_path, path_len, d_root32, d_ok);
+  return 1;
+}
+int launch_merkle_chain_keep(const ChainOperands& ops, uint32_t n_left, const uint32_t* d_acc_in, uint32_t* d_acc_out, cudaStream_t stream) {
+  merkle_chain_keep_kernel<<<1, 32, 0, stream>>>(ops, n_left, d_acc_in, d_acc_out);
+  return 1;
+}
+int launch_merkle_verify_batch(const uint32_t* d_leaf32, const uint64_t* d_idx, uint32_t m, uint64_t size, const uint32_t* d_paths, uint32_t stride,
+                               const uint32_t* d_lens, const uint32_t* d_root32, uint8_t* d_ok, int sm_count, cudaStream_t stream) {
+  if (!m) return 0;
+  const uint32_t grid = std::min<uint32_t>((m + kProofVerifyBlock - 1) / kProofVerifyBlock, (uint32_t)sm_count * kProofVerifyBlocksPerSm);
+  merkle_verify_batch_kernel<<<grid, kProofVerifyBlock, 0, stream>>>(d_leaf32, d_idx, m, size, d_paths, stride, d_lens, d_root32, d_ok);
+  return 1;
+}
+int launch_merkle_gather(const NodeStore& st, const uint32_t* d_spine, uint64_t size, const uint64_t* d_idx, uint64_t first, uint32_t m, uint32_t stride,
+                         uint32_t* d_out, uint32_t* d_lens, int sm_count, cudaStream_t stream) {
+  if (!m) return 0;
+  const uint32_t grid = std::min<uint32_t>((m + kGatherWarps - 1) / kGatherWarps, (uint32_t)sm_count * kGatherBlocksPerSm);
+  merkle_gather_kernel<<<grid, kGatherWarps * 32, 0, stream>>>(st, d_spine, size, d_idx, first, m, stride, d_out, d_lens);
   return 1;
 }
 
@@ -519,22 +604,33 @@ static int launch_merkle_level(const uint32_t* d_in, uint64_t n_in, uint32_t* d_
   merkle_level_kernel<<<(unsigned)((n_out + 127) / 128), 128, 0, stream>>>(d_in, n_in, d_out);
   return 1;
 }
-static int launch_merkle_reduce(const uint32_t* d_in, uint64_t n_in, uint32_t levels, uint32_t* d_out, cudaStream_t stream) {
+// keep: where levels 1 .. levels - 1 of the launch go as well (nullptr: only the last level, at d_out)
+static int launch_merkle_reduce(const uint32_t* d_in, uint64_t n_in, uint32_t levels, uint32_t* d_out, uint32_t* const* keep, cudaStream_t stream) {
   if (!n_in || levels == 0 || levels > 5) return 0;
   const uint64_t n_groups = (n_in + (1ull << levels) - 1) >> levels, warps = (n_groups + (32u >> levels) - 1) / (32u >> levels);
-  merkle_reduce_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, stream>>>(d_in, n_in, levels, d_out);
+  const unsigned grid = (unsigned)((warps + 7) / 8);
+  FoldLevels kl{};
+  if (keep) {
+    for (uint32_t s = 0; s + 1 < levels; s++) kl.p[s] = keep[s];
+    merkle_reduce_kernel<true><<<grid, 256, 0, stream>>>(d_in, n_in, levels, d_out, kl);
+  } else {
+    merkle_reduce_kernel<false><<<grid, 256, 0, stream>>>(d_in, n_in, levels, d_out, kl);
+  }
   return 1;
 }
 // Above 2^15 nodes a level is one launch of merkle_level_kernel (every lane busy); from 2^15 nodes down merkle_reduce_kernel
 // folds min(5, levels left under max_levels, ceil(log2 n)) levels per launch, where a launch costs more than idle lanes do.
+// With d_levels every level l >= 1 is written to d_levels[l] instead of the d_a / d_b ping-pong, the reductions' intermediate
+// levels included: the launches are the same, only where the nodes land differs.
 int launch_merkle_fold(const uint32_t* d_in, uint64_t n, uint32_t max_levels, uint32_t* d_a, uint32_t* d_b, cudaStream_t stream,
-                       const uint32_t** d_result) {
+                       const uint32_t** d_result, uint32_t* const* d_levels) {
   int k = 0;
   const uint32_t* src = d_in; uint32_t* dst = d_a;
   for (uint32_t lv = 0; n > 1 && lv < max_levels;) {
     uint32_t step = 1;
     if (n <= (1u << 15)) { step = std::min(5u, max_levels - lv); while (step > 1 && (1ull << (step - 1)) >= n) step--; }
-    k += step > 1 ? launch_merkle_reduce(src, n, step, dst, stream) : launch_merkle_level(src, n, dst, stream);
+    if (d_levels) dst = d_levels[lv + step];
+    k += step > 1 ? launch_merkle_reduce(src, n, step, dst, d_levels ? d_levels + lv + 1 : nullptr, stream) : launch_merkle_level(src, n, dst, stream);
     n = (n + (1ull << step) - 1) >> step; lv += step;
     src = dst; dst = dst == d_a ? d_b : d_a;
   }
