@@ -109,7 +109,7 @@ def main():
             N.check(lib.cg_merkle_log_proofs(tree.handle, idx.data_ptr(), m, s, paths.data_ptr(), stride, plens.data_ptr()))
         call()
         ms = median_ms(call, args.reps)
-        kern = kernel_ms(torch, call, ["merkle_gather_kernel", "merkle_chain_keep_kernel"])
+        kern = kernel_ms(torch, call, ["merkle_gather_kernel", "merkle_chain_kernel"])
         proofs[label] = {"tree_size": s, "proofs": m, "stride": stride, "call_ms": ms, "proofs_per_s_call": m / ms * 1e3,
                          "d2h_bytes": m * stride * 32 + 4 * m, "kernel_ms": kern,
                          "proofs_per_s_gather_kernel": m / kern.get("merkle_gather_kernel", float("nan")) * 1e3}

@@ -1,6 +1,6 @@
 """GPU tier, proofs from a log's node store (cg_merkle_log_create_tree): audit paths and consistency proofs at any tree size,
 in batches, against the oracle's RFC 6962 recursion and the CT vectors; the store filled across the fold's switch points;
-the gather and batch-verify kernels past their grids; batched verification rejecting exactly what the single-proof verifier
+the gather and batch-verify kernels past their grids; batched verification rejecting exactly what the oracle's RFC 9162 walk
 rejects; errors before any output byte changes.  Run on an H100: pytest -m gpu."""
 import ctypes as C
 import json
@@ -226,10 +226,9 @@ def root_at(N, large, s):
         lg.close()
 
 
-def test_batched_verification_rejects_what_the_single_verifier_rejects(N, oracle, large):
+def test_batched_verification_rejects_what_the_oracle_rejects(N, oracle, large):
     """100k valid proofs all hold; copies with one change each (a flipped leaf byte, index ^ 1, tree_size +- 1, a path element
-    dropped or added, an older root, an index >= tree_size) give the single-proof verifier's bit on every copy and the
-    oracle's on a sample"""
+    dropped or added, an older root, an index >= tree_size) give the oracle's bit on every copy"""
     tree, leaves, roots = large["tree"], large["leaves"], large["roots"]
     n = tree.size()
     rng = np.random.default_rng(6)
@@ -259,11 +258,8 @@ def test_batched_verification_rejects_what_the_single_verifier_rejects(N, oracle
         got = np.zeros(len(items), dtype=bool)
         for (s, r), ks in by_size.items():
             got[ks] = N.merkle_verify_proofs([items[k][0] for k in ks], [items[k][1] for k in ks], s, [items[k][2] for k in ks], r)
-        single = np.array([N.merkle_verify_proof(lf, i, s, p, r) for lf, i, p, s, r in items])
-        assert np.array_equal(got, single), name
-        for k in range(0, len(items), 64):
-            lf, i, p, s, r = items[k]
-            assert got[k] == oracle.merkle_verify_path(lf, i, s, p, r), (name, k)
+        want = np.array([oracle.merkle_verify_path(lf, i, s, p, r) for lf, i, p, s, r in items], dtype=bool)
+        assert np.array_equal(got, want), name
 
 
 def test_verification_over_every_leaf_length_and_start_offset(N, oracle):

@@ -1212,7 +1212,7 @@ struct cg_merkle_log {
   uint64_t n = 0;                 // leaves so far; bit h of n set <=> slot h holds the root of a perfect 2^h subtree
   bool keep = false;              // keep every leaf digest in HBM (needed for inclusion proofs)
   uint32_t* d_slots = nullptr;    // 64 x 8 words
-  uint32_t* d_tmp = nullptr;      // 66 x 8 words: [0..63] gathered left operands, [64] accumulator, [65] result
+  uint32_t* d_tmp = nullptr;      // 65 x 8 words: [0..63] a proof folded from the leaf digests, [64] the root
   uint32_t* d_leaves = nullptr; uint64_t cap_leaves = 0;     // keep: n leaf digests
   uint32_t* d_new = nullptr; size_t cap_new = 0;             // !keep: the current batch's leaf digests
   uint32_t* d_a = nullptr; size_t cap_a = 0; uint32_t* d_b = nullptr; size_t cap_b = 0;   // level ping-pong
@@ -1229,12 +1229,16 @@ struct cg_merkle_log {
 };
 
 namespace {
+// room in the level ping-pong for a fold of cnt > 1 nodes
+int log_fold_room(cg_merkle_log* L, uint64_t cnt) {
+  int rc = grow(&L->d_a, &L->cap_a, (size_t)(cnt + 1) / 2 * 8 + 8);
+  return rc ? rc : grow(&L->d_b, &L->cap_b, (size_t)(cnt + 3) / 4 * 8 + 8);
+}
 // MTH of `cnt` consecutive leaf digests starting at d_in (level-wise, unpaired node promoted) -> d_out (32 bytes)
 int log_range_root(cg_merkle_log* L, const uint32_t* d_in, uint64_t cnt, uint32_t* d_out, cudaStream_t st) {
   int rc;
   if (cnt == 1) { CU(cudaMemcpyAsync(d_out, d_in, 32, cudaMemcpyDeviceToDevice, st)); return CG_OK; }
-  if ((rc = grow(&L->d_a, &L->cap_a, (size_t)(cnt + 1) / 2 * 8 + 8))) return rc;
-  if ((rc = grow(&L->d_b, &L->cap_b, (size_t)(cnt + 3) / 4 * 8 + 8))) return rc;
+  if ((rc = log_fold_room(L, cnt))) return rc;
   const uint32_t* d_root;
   count_launches(launch_merkle_fold(d_in, cnt, 64, L->d_a, L->d_b, st, &d_root));
   CU(cudaMemcpyAsync(d_out, d_root, 32, cudaMemcpyDeviceToDevice, st));
@@ -1245,16 +1249,13 @@ int log_check(cg_merkle_log* L) {
   if (!L) return fail(CG_ERR_INVALID_ARG, "null argument");
   return CG_OK;
 }
-// root of the current tree -> d_tmp[65]
+// root of the current tree -> d_tmp[64]
 int log_root_device(cg_merkle_log* L, cudaStream_t st) {
   // fold the frontier from the smallest subtree upwards: r = slot[lowest]; r = node(slot[h], r) for every higher set bit
-  uint32_t nl = 0; int lowest = -1;
-  for (int h = 0; h < 64; h++) if ((L->n >> h) & 1ull) {
-    if (lowest < 0) { lowest = h; continue; }
-    CU(cudaMemcpyAsync(L->d_tmp + 8 * nl, L->d_slots + 8 * h, 32, cudaMemcpyDeviceToDevice, st)); nl++;
-  }
-  int k = launch_merkle_chain(L->d_tmp, nl, L->d_slots + 8 * lowest, L->d_tmp + 8 * 65, st);
-  count_launches(k);
+  const int lowest = __builtin_ctzll(L->n);
+  ChainOperands ops{}; uint32_t nl = 0;
+  for (int h = lowest + 1; h < 64; h++) if ((L->n >> h) & 1ull) ops.left[nl++] = L->d_slots + 8 * h;
+  count_launches(launch_merkle_chain_keep(ops, nl, L->d_slots + 8 * lowest, L->d_tmp + 8 * 64, st));
   return CG_OK;
 }
 // node j of level h of a tree log (level 0: leaf digest j)
@@ -1265,7 +1266,7 @@ int log_new(cg_merkle_log** out, bool keep, bool tree) {
   if (!out) return fail(CG_ERR_INVALID_ARG, "null argument");
   std::unique_ptr<cg_merkle_log> L(new cg_merkle_log());
   L->keep = keep; L->tree = tree;
-  CU(cudaMalloc((void**)&L->d_slots, 64 * 32)); CU(cudaMalloc((void**)&L->d_tmp, 66 * 32));
+  CU(cudaMalloc((void**)&L->d_slots, 64 * 32)); CU(cudaMalloc((void**)&L->d_tmp, 65 * 32));
   CU(cudaMemset(L->d_slots, 0, 64 * 32));
   if (tree) CU(cudaMalloc((void**)&L->d_spine, 64 * 32));
   *out = L.release();
@@ -1335,34 +1336,23 @@ int log_digest_room(cg_merkle_log* L, uint64_t m, cudaStream_t st, uint32_t** ou
   return CG_OK;
 }
 // m new leaf digests at d_dig: cut [n, n+m) into aligned perfect blocks (block size <= lowest set bit of its position),
-// reduce each, carry into the frontier
+// reduce each, carry into the frontier.  On a tree log the block's fold writes its levels into the store (its root is node
+// (h, pos >> h)) and every carry makes the complete node (top, pos >> top) under the next occupied slot.
 int log_absorb(cg_merkle_log* L, const uint32_t* d_dig, uint64_t m, cudaStream_t st) {
-  int rc, k;
+  int rc;
   uint64_t pos = L->n, rem = m;
   while (rem) {
     uint64_t s = pos ? (pos & (~pos + 1)) : (1ull << 63);
     while (s > rem) s >>= 1;
     int h = 0; while ((1ull << h) < s) h++;
-    if (L->tree) {
-      // the block's fold writes its levels into the store (its root is node (h, pos >> h)); every carry above it makes the
-      // complete node (top, pos >> top) for the next occupied slot
-      uint32_t* lv[64] = {};
-      for (int l = 1; l <= h; l++) lv[l] = log_node(L, l, pos >> l);
-      const uint32_t* unused;
-      count_launches(launch_merkle_fold(log_node(L, 0, pos), s, 64, nullptr, nullptr, st, &unused, lv));
-      const uint32_t* acc = log_node(L, h, pos >> h);
-      ChainOperands ops{}; uint32_t nl = 0; int top = h;
-      while ((pos >> top) & 1ull) { ops.left[nl] = L->d_slots + 8 * top; top++; ops.keep[nl] = log_node(L, top, pos >> top); nl++; }
-      if (nl) { k = launch_merkle_chain_keep(ops, nl, acc, L->d_slots + 8 * top, st); count_launches(k); }
-      else CU(cudaMemcpyAsync(L->d_slots + 8 * top, acc, 32, cudaMemcpyDeviceToDevice, st));
-      pos += s; rem -= s;
-      continue;
-    }
-    uint32_t* acc = L->d_tmp + 8 * 64;
-    if ((rc = log_range_root(L, d_dig + (size_t)(pos - L->n) * 8, s, acc, st))) return rc;
-    uint32_t nl = 0; int top = h;                           // slots h, h+1, ... that are occupied merge into the new subtree
-    while ((pos >> top) & 1ull) { CU(cudaMemcpyAsync(L->d_tmp + 8 * nl, L->d_slots + 8 * top, 32, cudaMemcpyDeviceToDevice, st)); nl++; top++; }
-    if (nl) { k = launch_merkle_chain(L->d_tmp, nl, acc, L->d_slots + 8 * top, st); count_launches(k); }
+    uint32_t* lv[64] = {};
+    if (L->tree) for (int l = 1; l <= h; l++) lv[l] = log_node(L, l, pos >> l);
+    else if (s > 1 && (rc = log_fold_room(L, s))) return rc;
+    const uint32_t* acc;                                    // the block's root (a block of one leaf: the leaf digest, no launch)
+    count_launches(launch_merkle_fold(d_dig + (size_t)(pos - L->n) * 8, s, 64, L->d_a, L->d_b, st, &acc, L->tree ? lv : nullptr));
+    ChainOperands ops{}; uint32_t nl = 0; int top = h;     // slots h, h+1, ... that are occupied merge into the new subtree
+    while ((pos >> top) & 1ull) { ops.left[nl] = L->d_slots + 8 * top; top++; ops.keep[nl] = L->tree ? log_node(L, top, pos >> top) : nullptr; nl++; }
+    if (nl) count_launches(launch_merkle_chain_keep(ops, nl, acc, L->d_slots + 8 * top, st));
     else CU(cudaMemcpyAsync(L->d_slots + 8 * top, acc, 32, cudaMemcpyDeviceToDevice, st));
     pos += s; rem -= s;
   }
@@ -1456,7 +1446,7 @@ int cg_merkle_log_root(cg_merkle_log* L, uint8_t out_root[32]) {
     if (!out_root) return fail(CG_ERR_INVALID_ARG, "null argument");
     if (L->n) {
       if ((rc = log_root_device(L, G.stream))) return rc;
-      CU(cudaMemcpyAsync(out_root, L->d_tmp + 8 * 65, 32, cudaMemcpyDeviceToHost, G.stream));
+      CU(cudaMemcpyAsync(out_root, L->d_tmp + 8 * 64, 32, cudaMemcpyDeviceToHost, G.stream));
       CU(cudaStreamSynchronize(G.stream));
       return CG_OK;
     }
@@ -1480,11 +1470,23 @@ NodeStore log_store(cg_merkle_log* L) {
   for (uint32_t h = 0; h < 64; h++) ns.lvl[h] = h ? L->d_lvl[h] : L->d_leaves;
   return ns;
 }
-// path lengths (host side of the gather's rule): inclusion of leaf i, and PROOF(first, D[0:size])
-uint32_t inclusion_len(uint64_t i, uint64_t size) { return (uint32_t)__builtin_popcountll(merkle_path_levels(i, size, 0)); }
-uint32_t consistency_len(uint64_t first, uint64_t size) {
-  if (first == size) return 0;
-  return (uint32_t)__builtin_popcountll(merkle_path_levels(first - 1, size, __builtin_ctzll(first))) + ((first & (first - 1)) ? 1u : 0u);
+// The leaf ranges [a, b) of PATH(i, D[0:size]) (RFC 6962 2.1.1; first == 0), or of PROOF(first, D[0:size]) (2.1.2; i unused),
+// in proof order -- the gather kernel's rule (merkle_path_element): a consistency proof is the node (ctz first, (first - 1) >>
+// ctz first) unless first is a power of two, then the path of leaf first - 1 from level ctz first up (nothing when first == size).
+std::vector<std::pair<uint64_t, uint64_t>> proof_ranges(uint64_t i, uint64_t size, uint64_t first) {
+  std::vector<std::pair<uint64_t, uint64_t>> r;
+  uint32_t lo = 0;
+  if (first) {
+    if (first == size) return r;
+    i = first - 1; lo = (uint32_t)__builtin_ctzll(first);
+    if (first & (first - 1)) r.push_back({first - (1ull << lo), first});
+  }
+  for (uint64_t levels = merkle_path_levels(i, size, lo); levels; levels &= levels - 1) {
+    const uint32_t l = (uint32_t)__builtin_ctzll(levels);
+    const uint64_t b = ((i >> l) ^ 1ull) << l;
+    r.push_back({b, b + std::min<uint64_t>(size - b, 1ull << l)});
+  }
+  return r;
 }
 // the spine of `size`, then m paths (leaf indices h_idx, or one consistency proof from `first` when h_idx is null) at `stride`
 // digests each -> out_paths32 (host), their lengths -> out_lens (host, may be null).  Two launches, whatever m and size.
@@ -1501,6 +1503,17 @@ int log_gather(cg_merkle_log* L, const uint64_t* h_idx, uint32_t m, uint64_t siz
   CU(cudaGetLastError());
   if (path_words) CU(cudaMemcpyAsync(out_paths32, d_paths, path_words * 4, cudaMemcpyDeviceToHost, st));
   if (out_lens) CU(cudaMemcpyAsync(out_lens, d_lens, (size_t)m * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return CG_OK;
+}
+// one proof at the log's size, whose ranges are `ranges` (proof_ranges) -> out_path32 (host): gathered from the node store on a
+// tree log, else every range folded from the leaf digests.  The path of leaf *h_idx, or PROOF(first, ...) when h_idx is null.
+int log_proof(cg_merkle_log* L, const std::vector<std::pair<uint64_t, uint64_t>>& ranges, const uint64_t* h_idx, uint64_t first, uint8_t* out_path32) {
+  if (L->tree) return ranges.empty() ? CG_OK : log_gather(L, h_idx, 1, L->n, first, out_path32, (uint32_t)ranges.size(), nullptr);
+  cudaStream_t st = G.stream; int rc;
+  for (size_t i = 0; i < ranges.size(); i++)
+    if ((rc = log_range_root(L, L->d_leaves + (size_t)ranges[i].first * 8, ranges[i].second - ranges[i].first, L->d_tmp + 8 * i, st))) return rc;
+  if (!ranges.empty()) CU(cudaMemcpyAsync(out_path32, L->d_tmp, ranges.size() * 32, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
 }
@@ -1527,7 +1540,7 @@ int cg_merkle_log_consistency_between(cg_merkle_log* L, uint64_t first_size, uin
   if (!L->tree) return fail(CG_ERR_UNSUPPORTED, "proofs at any tree size need a log made by cg_merkle_log_create_tree");
   if (second_size == 0 || second_size > L->n || first_size == 0 || first_size > second_size)
     return fail(CG_ERR_INVALID_ARG, "need 1 <= first_size <= second_size <= size of the log");
-  const uint32_t len = consistency_len(first_size, second_size);
+  const uint32_t len = (uint32_t)proof_ranges(0, second_size, first_size).size();
   if (len > path_cap || (len && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
   *out_len = len;
   return len ? log_gather(L, nullptr, 1, second_size, first_size, out_path32, len, nullptr) : CG_OK;
@@ -1539,29 +1552,10 @@ int cg_merkle_log_proof(cg_merkle_log* L, uint64_t index, uint8_t* out_path32, u
   if (!out_len) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (!L->keep) return fail(CG_ERR_UNSUPPORTED, "log was created without leaf digests (or restored from a frontier): no proofs");
   if (index >= L->n) return fail(CG_ERR_INVALID_ARG, "leaf index out of range");
-  if (L->tree) {                                            // from the node store: the same path, two launches
-    const uint32_t len = inclusion_len(index, L->n);
-    *out_len = len;
-    if (len > path_cap || (len && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
-    return len ? log_gather(L, &index, 1, L->n, 0, out_path32, len, nullptr) : CG_OK;
-  }
-  // RFC 6962 2.1.1: PATH(m, D[n]) -- the sibling subtree at every split on the way down, returned leaf level first
-  std::vector<std::pair<uint64_t, uint64_t>> sib;
-  uint64_t lo = 0, hi = L->n;
-  while (hi - lo > 1) {
-    uint64_t k = 1; while (k * 2 < hi - lo) k *= 2;       // largest power of two < hi - lo
-    if (index < lo + k) { sib.push_back({lo + k, hi}); hi = lo + k; } else { sib.push_back({lo, lo + k}); lo = lo + k; }
-  }
-  *out_len = (uint32_t)sib.size();
-  if (sib.size() > path_cap || (sib.size() && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
-  cudaStream_t st = G.stream;
-  for (size_t i = 0; i < sib.size(); i++) {
-    const auto& r = sib[sib.size() - 1 - i];
-    if ((rc = log_range_root(L, L->d_leaves + (size_t)r.first * 8, r.second - r.first, L->d_tmp + 8 * i, st))) return rc;
-  }
-  if (!sib.empty()) CU(cudaMemcpyAsync(out_path32, L->d_tmp, sib.size() * 32, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  return CG_OK;
+  const auto ranges = proof_ranges(index, L->n, 0);
+  *out_len = (uint32_t)ranges.size();
+  if (ranges.size() > path_cap || (ranges.size() && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
+  return log_proof(L, ranges, &index, 0, out_path32);
 }
 
 /* RFC 6962 2.1.2: PROOF(m, D[n]) -- the nodes that show the tree of the first m leaves is a prefix of the current one. */
@@ -1571,34 +1565,10 @@ int cg_merkle_log_consistency(cg_merkle_log* L, uint64_t first_size, uint8_t* ou
   if (!out_len) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (!L->keep) return fail(CG_ERR_UNSUPPORTED, "log was created without leaf digests (or restored from a frontier): no proofs");
   if (first_size == 0 || first_size > L->n) return fail(CG_ERR_INVALID_ARG, "first_size must be in [1, size of the log]");
-  if (L->tree) {                                            // from the node store: the same proof, two launches
-    const uint32_t len = consistency_len(first_size, L->n);
-    *out_len = len;
-    if (len > path_cap || len > 64 || (len && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
-    return len ? log_gather(L, nullptr, 1, L->n, first_size, out_path32, len, nullptr) : CG_OK;
-  }
-  // SUBPROOF(m, D[lo:hi], b): k = largest power of two < hi - lo; m <= k: recurse left, then MTH(D[lo+k:hi]);
-  // else recurse right with b = false, then MTH(D[lo:lo+k]); m == hi - lo: {} if b else {MTH(D[lo:hi])}
-  std::vector<std::pair<uint64_t, uint64_t>> ranges;      // in proof order
-  {
-    std::vector<std::pair<uint64_t, uint64_t>> tail;       // appended after the recursion, innermost first
-    uint64_t lo = 0, hi = L->n, m = first_size; bool b = true;
-    while (m != hi - lo) {
-      uint64_t k = 1; while (k * 2 < hi - lo) k *= 2;
-      if (m <= k) { tail.push_back({lo + k, hi}); hi = lo + k; }
-      else { tail.push_back({lo, lo + k}); lo += k; m -= k; b = false; }
-    }
-    if (!b) ranges.push_back({lo, hi});
-    for (size_t i = tail.size(); i-- > 0;) ranges.push_back(tail[i]);
-  }
+  const auto ranges = proof_ranges(0, L->n, first_size);
   *out_len = (uint32_t)ranges.size();
   if (ranges.size() > path_cap || ranges.size() > 64 || (ranges.size() && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
-  cudaStream_t st = G.stream;
-  for (size_t i = 0; i < ranges.size(); i++)
-    if ((rc = log_range_root(L, L->d_leaves + (size_t)ranges[i].first * 8, ranges[i].second - ranges[i].first, L->d_tmp + 8 * i, st))) return rc;
-  if (!ranges.empty()) CU(cudaMemcpyAsync(out_path32, L->d_tmp, ranges.size() * 32, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  return CG_OK;
+  return log_proof(L, ranges, nullptr, first_size, out_path32);
 }
 
 /* RFC 9162 2.1.4.2: *out_ok = 1 iff `path` proves that the tree with root_first over first_size leaves is a prefix of the tree
@@ -1624,38 +1594,11 @@ int cg_merkle_verify_consistency(uint64_t first_size, uint64_t second_size, cons
   return CG_OK;
 }
 
-int cg_merkle_verify_proof(const uint8_t* leaf_bytes, uint64_t leaf_len, uint64_t index, uint64_t tree_size, const uint8_t* path32, uint32_t path_len,
-                           const uint8_t root[32], int* out_ok) {
-  std::lock_guard<std::mutex> lk(g_mu);
-  if (int rc = require_ready()) return rc;
-  if (!out_ok || !root || (leaf_len && !leaf_bytes) || (path_len && !path32) || path_len > 64) return fail(CG_ERR_INVALID_ARG, "bad argument");
-  int rc; cudaStream_t st = G.stream;
-  if ((rc = grow_bytes((size_t)leaf_len + 64))) return rc;
-  if ((rc = grow(&G.d_off64, &G.cap_off64, 2))) return rc;
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)(path_len + 4) * 8))) return rc;
-  uint64_t off[2] = {0, leaf_len};
-  if (leaf_len) CU(cudaMemcpyAsync(G.d_bytes, leaf_bytes, leaf_len, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(G.d_off64, off, 16, cudaMemcpyHostToDevice, st));
-  uint32_t* d_leaf = G.d_dig[0]; uint32_t* d_root = d_leaf + 8; uint32_t* d_ok = d_root + 8; uint32_t* d_path = d_ok + 8;
-  int k = launch_merkle_leaves_var(G.d_bytes, G.d_off64, 1, d_leaf, st);
-  CU(cudaMemcpyAsync(d_root, root, 32, cudaMemcpyHostToDevice, st));
-  if (path_len) CU(cudaMemcpyAsync(d_path, path32, (size_t)path_len * 32, cudaMemcpyHostToDevice, st));
-  k += launch_merkle_verify(d_leaf, index, tree_size, d_path, path_len, d_root, d_ok, st);
-  count_launches(k);
-  uint32_t ok = 0;
-  CU(cudaMemcpyAsync(&ok, d_ok, 4, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  CU(cudaGetLastError());
-  *out_ok = (int)ok;
-  return CG_OK;
-}
-
+namespace {
 /* m proofs against one (tree_size, root): the leaves are hashed by the word-granular leaf kernel over the staging buffer, then
- * one thread per proof walks its path (the walk of the single-proof verifier).  Two launches, whatever m. */
-int cg_merkle_verify_proofs(const uint8_t* leaf_bytes, const uint64_t* leaf_offsets, const uint64_t* indices, uint32_t m, uint64_t tree_size,
-                            const uint8_t* paths32, uint32_t path_stride, const uint32_t* path_lens, const uint8_t root[32], uint8_t* out_ok) {
-  std::lock_guard<std::mutex> lk(g_mu);
-  if (int rc = require_ready()) return rc;
+ * one thread per proof walks its path (RFC 9162 2.1.3.2).  Two launches, whatever m. */
+int verify_proofs(const uint8_t* leaf_bytes, const uint64_t* leaf_offsets, const uint64_t* indices, uint32_t m, uint64_t tree_size,
+                  const uint8_t* paths32, uint32_t path_stride, const uint32_t* path_lens, const uint8_t root[32], uint8_t* out_ok) {
   if (!m) return CG_OK;
   if (!leaf_offsets || !indices || !path_lens || !root || !out_ok || (path_stride && !paths32)) return fail(CG_ERR_INVALID_ARG, "null argument");
   for (uint32_t i = 0; i < m; i++) {
@@ -1688,6 +1631,25 @@ int cg_merkle_verify_proofs(const uint8_t* leaf_bytes, const uint64_t* leaf_offs
   CU(cudaMemcpyAsync(out_ok, d_ok, m, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
+}
+}  // namespace
+
+int cg_merkle_verify_proof(const uint8_t* leaf_bytes, uint64_t leaf_len, uint64_t index, uint64_t tree_size, const uint8_t* path32, uint32_t path_len,
+                           const uint8_t root[32], int* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  if (!out_ok || !root || (leaf_len && !leaf_bytes) || (path_len && !path32) || path_len > 64) return fail(CG_ERR_INVALID_ARG, "bad argument");
+  const uint64_t off[2] = {0, leaf_len}; uint8_t ok = 0;
+  int rc = verify_proofs(leaf_bytes, off, &index, 1, tree_size, path32, path_len, &path_len, root, &ok);
+  if (!rc) *out_ok = ok;
+  return rc;
+}
+
+int cg_merkle_verify_proofs(const uint8_t* leaf_bytes, const uint64_t* leaf_offsets, const uint64_t* indices, uint32_t m, uint64_t tree_size,
+                            const uint8_t* paths32, uint32_t path_stride, const uint32_t* path_lens, const uint8_t root[32], uint8_t* out_ok) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  return verify_proofs(leaf_bytes, leaf_offsets, indices, m, tree_size, paths32, path_stride, path_lens, root, out_ok);
 }
 
 // ---------------------------------------------------------------------------------- multi-GPU: one process per GPU

@@ -158,9 +158,6 @@ int launch_span_pack_one(const ScanWork& w, const uint32_t* d_digests, const uin
 
 // SHA-256 / Merkle
 int launch_sha256_batch(const uint8_t* d_bytes, const uint64_t* d_off, uint32_t n, uint8_t* d_out, cudaStream_t stream);
-// Merkle log: acc = node(left[k], acc) chains; audit-path verification
-int launch_merkle_chain(const uint32_t* d_left, uint32_t n_left, const uint32_t* d_acc_in, uint32_t* d_acc_out, cudaStream_t stream);
-int launch_merkle_verify(const uint32_t* d_leaf32, uint64_t index, uint64_t size, const uint32_t* d_path, uint32_t path_len, const uint32_t* d_root32, uint32_t* d_ok, cudaStream_t stream);
 // redacted output: SHA-256 of every span, then copy + placeholder splice (one warp per message).  Both read their item
 // count from device memory (*d_ns spans, *d_n <= n_max messages), so that the resolver decides on the device whether they run.
 // d_out digests: 16-byte aligned.
@@ -184,11 +181,12 @@ int launch_merkle_consistency(uint64_t first, uint64_t second, const uint32_t* d
 int launch_merkle_fold(const uint32_t* d_in, uint64_t n, uint32_t max_levels, uint32_t* d_a, uint32_t* d_b, cudaStream_t stream,
                        const uint32_t** d_result, uint32_t* const* d_levels = nullptr);
 
-// Logs that keep their complete aligned nodes (cg_merkle_log_create_tree).  Kernel arguments by value:
+// Merkle log kernel arguments by value (merkle_reduce_kernel's levels and the node store: logs made by cg_merkle_log_create_tree):
 struct FoldLevels { uint32_t* p[5]; };                                  // merkle_reduce_kernel: intermediate level s + 1 -> p[s]
-struct ChainOperands { const uint32_t* left[64]; uint32_t* keep[64]; };  // chain step k: acc = node(*left[k], acc) -> keep[k]
+struct ChainOperands { const uint32_t* left[64]; uint32_t* keep[64]; };  // chain step k: acc = node(*left[k], acc) -> keep[k] (if not null)
 struct NodeStore { const uint32_t* lvl[64]; };                          // level h of the store (level 0: the leaf digests)
-// acc = node(left[k], acc) for k < n_left, keeping every intermediate (frontier carries into the store, the spine of a size)
+// acc = node(*left[k], acc) for k < n_left, keeping the intermediates asked for: frontier carries (into the store on a tree
+// log), the root fold, the spine of a size.  One launch.
 int launch_merkle_chain_keep(const ChainOperands& ops, uint32_t n_left, const uint32_t* d_acc_in, uint32_t* d_acc_out, cudaStream_t stream);
 
 // The levels at which PATH(i, D[0:size]) (RFC 6962 2.1.1) has an element, from level lo up: bit l set <=> one element at level
@@ -203,7 +201,7 @@ __host__ __device__ inline uint64_t merkle_path_levels(uint64_t i, uint64_t size
   return (below | (i & ~below)) & ~((1ull << lo) - 1);
 }
 // paths from the store: one warp per path, kGatherWarps per block, at most kGatherBlocksPerSm blocks per SM (grid-stride);
-// d_idx = leaf indices, or null: one consistency proof PROOF(first, D[0:size]).  d_spine: spine of `size` (chain_keep).
+// d_idx = leaf indices, or null: one consistency proof PROOF(first, D[0:size]).  d_spine: spine of `size` (one chain launch).
 constexpr uint32_t kGatherWarps = 8, kGatherBlocksPerSm = 8;
 int launch_merkle_gather(const NodeStore& st, const uint32_t* d_spine, uint64_t size, const uint64_t* d_idx, uint64_t first, uint32_t m, uint32_t stride,
                          uint32_t* d_out, uint32_t* d_lens, int sm_count, cudaStream_t stream);

@@ -232,29 +232,20 @@ __global__ void __launch_bounds__(128) merkle_level_kernel(const uint32_t* __res
 // Merkle log helpers (append-only log: frontier carries, root fold, audit-path check) -- a handful of node hashes
 // per call, run by one thread on the device (the product computes no hash on the CPU)
 // ------------------------------------------------------------------------------------------
-// acc = node(left[k], acc) for k = 0..n_left-1 : frontier carry chains and the root fold.  left: n_left digests.
-__global__ void merkle_chain_kernel(const uint32_t* __restrict__ left, uint32_t n_left, const uint32_t* __restrict__ acc_in, uint32_t* __restrict__ acc_out) {
-  if (threadIdx.x || blockIdx.x) return;
-  uint32_t r[8]; load_digest(acc_in, r);
-  for (uint32_t k = 0; k < n_left; k++) { uint32_t l[8], h[8]; load_digest(left + 8 * k, l); merkle_node(l, r, h);
-#pragma unroll
-    for (int t = 0; t < 8; t++) r[t] = h[t]; }
-  store_digest(acc_out, r);
-}
-// The same chain with its left operands anywhere (ops.left[k]), keeping the accumulator after step k at ops.keep[k] too:
-// the frontier carries of a log that keeps its nodes (each intermediate accumulator is a complete aligned node) and the
-// spine of a tree size (each intermediate is the root of a suffix of the leaves).  acc_out may be null.
-__global__ void merkle_chain_keep_kernel(ChainOperands ops, uint32_t n_left, const uint32_t* __restrict__ acc_in, uint32_t* __restrict__ acc_out) {
+// acc = node(*ops.left[k], acc) for k = 0..n_left-1, the accumulator after step k kept at ops.keep[k] unless that is null:
+// frontier carries (on a log that keeps its nodes each intermediate accumulator is a complete aligned node), the root fold,
+// and the spine of a tree size (each intermediate is the root of a suffix of the leaves).  acc_out may be null.
+__global__ void merkle_chain_kernel(ChainOperands ops, uint32_t n_left, const uint32_t* __restrict__ acc_in, uint32_t* __restrict__ acc_out) {
   if (threadIdx.x || blockIdx.x) return;
   uint32_t r[8]; load_digest(acc_in, r);
   for (uint32_t k = 0; k < n_left; k++) { uint32_t l[8], h[8]; load_digest(ops.left[k], l); merkle_node(l, r, h);
 #pragma unroll
     for (int t = 0; t < 8; t++) r[t] = h[t];
-    store_digest(ops.keep[k], r); }
+    if (ops.keep[k]) store_digest(ops.keep[k], r); }
   if (acc_out) store_digest(acc_out, r);
 }
 // RFC 9162 2.1.3.2: does `path` prove that the leaf with digest leaf32 is entry `index` of the tree of `size` leaves with root
-// `root32`?  At most path_len node hashes; the single-proof and the batched verifier both ask this function.
+// `root32`?  At most path_len node hashes.
 __device__ bool merkle_verify_path(const uint32_t* __restrict__ leaf32, unsigned long long index, unsigned long long size,
                                    const uint32_t* __restrict__ path, uint32_t path_len, const uint32_t* __restrict__ root32) {
   if (index >= size) return false;
@@ -277,11 +268,6 @@ __device__ bool merkle_verify_path(const uint32_t* __restrict__ leaf32, unsigned
 #pragma unroll
   for (int t = 0; t < 8; t++) eq = eq && q[t] == r[t];
   return eq;
-}
-__global__ void merkle_verify_kernel(const uint32_t* __restrict__ leaf32, unsigned long long index, unsigned long long size,
-                                     const uint32_t* __restrict__ path, uint32_t path_len, const uint32_t* __restrict__ root32, uint32_t* __restrict__ ok) {
-  if (threadIdx.x || blockIdx.x) return;
-  *ok = merkle_verify_path(leaf32, index, size, path, path_len, root32) ? 1u : 0u;
 }
 // m proofs against one (size, root), one thread per proof: proof i = leaf digest leaf32[i], index idx[i], the path_lens[i]
 // digests at paths + 8 i stride.  Grid-stride over the proofs.
@@ -465,16 +451,8 @@ int launch_merkle_consistency(uint64_t first, uint64_t second, const uint32_t* d
   merkle_consistency_kernel<<<1, 32, 0, stream>>>(first, second, d_first32, d_second32, d_path, path_len, d_ok);
   return 1;
 }
-int launch_merkle_chain(const uint32_t* d_left, uint32_t n_left, const uint32_t* d_acc_in, uint32_t* d_acc_out, cudaStream_t stream) {
-  merkle_chain_kernel<<<1, 32, 0, stream>>>(d_left, n_left, d_acc_in, d_acc_out);
-  return 1;
-}
-int launch_merkle_verify(const uint32_t* d_leaf32, uint64_t index, uint64_t size, const uint32_t* d_path, uint32_t path_len, const uint32_t* d_root32, uint32_t* d_ok, cudaStream_t stream) {
-  merkle_verify_kernel<<<1, 32, 0, stream>>>(d_leaf32, index, size, d_path, path_len, d_root32, d_ok);
-  return 1;
-}
 int launch_merkle_chain_keep(const ChainOperands& ops, uint32_t n_left, const uint32_t* d_acc_in, uint32_t* d_acc_out, cudaStream_t stream) {
-  merkle_chain_keep_kernel<<<1, 32, 0, stream>>>(ops, n_left, d_acc_in, d_acc_out);
+  merkle_chain_kernel<<<1, 32, 0, stream>>>(ops, n_left, d_acc_in, d_acc_out);
   return 1;
 }
 int launch_merkle_verify_batch(const uint32_t* d_leaf32, const uint64_t* d_idx, uint32_t m, uint64_t size, const uint32_t* d_paths, uint32_t stride,
