@@ -122,7 +122,8 @@ CG_API int cg_rule_check(const char *source, uint32_t source_len, uint32_t flags
  *   bytes/offsets : n messages, message i = bytes[offsets[i] .. offsets[i+1])
  *   out_words[n]  : hit ? 1<<63 | (#distinct rules hit)<<32 | lowest hit rule index : 0
  *   out_hits      : optional sparse list sorted by (msg, rule); hits_cap entries available;
- *                   *out_nhits = number of hits (CG_ERR_CAPACITY when it exceeds hits_cap). */
+ *                   *out_nhits = number of hits (CG_ERR_CAPACITY when it exceeds hits_cap; CG_ERR_TOO_LARGE at 2^32
+ *                   hits or more).  Built on the device, as cg_scan_hits_batch_device builds it. */
 CG_API int cg_scan_batch(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, uint32_t n,
                          uint64_t *out_words, cg_hit *out_hits, uint32_t hits_cap, uint32_t *out_nhits);
 /* single message, blocking: the path for the synchronous hooks before_message_write /
@@ -195,9 +196,27 @@ CG_API int cg_find_matches_batch_device(cg_ruleset *rs, const void *d_bytes, con
 CG_API int cg_redact_batch_device(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, uint32_t n,
                                   void *d_out_bytes, uint64_t out_cap, void *d_out_offsets,
                                   void *d_out_spans, uint32_t spans_cap, void *d_out_digests32, void *d_out_sizes, void *stream);
-/* Waits for `stream` and returns the status of every device-path batch (scan, find-matches, redact) issued since the
- * previous join: CG_OK, CG_ERR_CAPACITY (see above) or CG_ERR_TOO_LARGE (the VM ran out of thread-list space; words all
- * ones as well; or a redacted batch of 4 GiB or more). */
+/* Every (message, rule) hit of a batch in HBM: the rule lists that matchesAny (src/conditions/context.ts:9-34, messageContains
+ * / conversationContains and the tool-param `matches` rules), aggregateMatches (src/policy-evaluator.ts:110-146) and the
+ * response gate's mustMatch / mustNotMatch (src/response-gate.ts:105-147) test per text, built on the device.  Same input rules as
+ * cg_scan_batch_device.  d_out_words[n]: the result words of cg_scan_batch_device; d_out_hits: cg_hit[hits_cap] sorted by
+ * (msg, rule), 4-byte aligned (may be NULL when hits_cap is 0); d_out_nhits: one uint32 = hits of the batch, 4-byte aligned.
+ * Asynchronous and in order on `stream`; its status comes from cg_scan_join: CG_ERR_CAPACITY when the batch has more than
+ * hits_cap hits (the first hits_cap are written), CG_ERR_TOO_LARGE at 2^32 - 1 hits or more, and CG_ERR_CAPACITY once after
+ * an internal queue overflow (then *d_out_nhits = 0xffffffff, no hit is written, the scratch grows: issue the batch again).
+ * n = 0 writes 0 to *d_out_nhits and enqueues nothing else. */
+CG_API int cg_scan_hits_batch_device(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, uint32_t n,
+                                     void *d_out_words, void *d_out_hits, uint32_t hits_cap, void *d_out_nhits, void *stream);
+/* cg_policy_verdict_batch for a batch in HBM (aggregateMatches / matchPolicy, src/policy-evaluator.ts:44-146): one verdict
+ * (uint32, 4-byte aligned) per message into d_out_verdicts.  CG_ERR_INVALID_ARG before anything is enqueued when
+ * cg_ruleset_set_policy has not been called.  Asynchronous and in order on `stream`, status from cg_scan_join; after an
+ * internal queue overflow every verdict of the batch is 0xffffffff (no verdict has action 3) and the join reports
+ * CG_ERR_CAPACITY once: issue the batch again. */
+CG_API int cg_policy_verdict_batch_device(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, uint32_t n,
+                                          void *d_out_verdicts, void *stream);
+/* Waits for `stream` and returns the status of every device-path batch (scan, hits, verdicts, find-matches, redact) issued
+ * since the previous join: CG_OK, CG_ERR_CAPACITY (see above) or CG_ERR_TOO_LARGE (the VM ran out of thread-list space; words
+ * all ones as well; a redacted batch of 4 GiB or more; a hit list of 2^32 - 1 hits or more). */
 CG_API int cg_scan_join(cg_ruleset *rs, void *stream);
 
 /* ---- SHA-256.  Replaces createHash("sha256").update(s).digest() at src/util.ts:77-79,

@@ -54,7 +54,8 @@ EXPORTS = ["cg_init", "cg_shutdown", "cg_last_error", "cg_version", "cg_device_c
            "cg_merkle_log_append_jsonl", "cg_merkle_log_consistency", "cg_merkle_verify_consistency", "cg_merkle_log_reserve",
            "cg_shard_range", "cg_comm_unique_id", "cg_comm_init", "cg_comm_destroy", "cg_merkle_root_sharded_device",
            "cg_ruleset_create", "cg_ruleset_destroy", "cg_ruleset_get_info", "cg_rule_check", "cg_scan_batch",
-           "cg_scan_one", "cg_find_matches_batch", "cg_find_matches_one", "cg_redact_one", "cg_scan_batch_device", "cg_find_matches_batch_device", "cg_redact_batch_device", "cg_sha256_batch", "cg_merkle_root",
+           "cg_scan_one", "cg_find_matches_batch", "cg_find_matches_one", "cg_redact_one", "cg_scan_batch_device", "cg_find_matches_batch_device", "cg_redact_batch_device",
+           "cg_scan_hits_batch_device", "cg_policy_verdict_batch_device", "cg_sha256_batch", "cg_merkle_root",
            "cg_merkle_root_fixed", "cg_merkle_block_roots_device", "cg_merkle_fold", "cg_merkle_fold_device",
            "cg_merkle_log_create_tree", "cg_merkle_log_proofs", "cg_merkle_log_consistency_between", "cg_merkle_verify_proofs"]
 
@@ -122,6 +123,8 @@ def load():
     L.cg_scan_batch_device.argtypes = [vp, vp, vp, u32, vp, vp]; L.cg_scan_batch_device.restype = i32
     L.cg_find_matches_batch_device.argtypes = [vp, vp, vp, u32, vp, u32, vp, vp]; L.cg_find_matches_batch_device.restype = i32
     L.cg_redact_batch_device.argtypes = [vp, vp, vp, u32, vp, u64, vp, vp, u32, vp, vp, vp]; L.cg_redact_batch_device.restype = i32
+    L.cg_scan_hits_batch_device.argtypes = [vp, vp, vp, u32, vp, vp, u32, vp, vp]; L.cg_scan_hits_batch_device.restype = i32
+    L.cg_policy_verdict_batch_device.argtypes = [vp, vp, vp, u32, vp, vp]; L.cg_policy_verdict_batch_device.restype = i32
     L.cg_sha256_batch.argtypes = [vp, vp, u32, vp]; L.cg_sha256_batch.restype = i32
     L.cg_merkle_root.argtypes = [vp, vp, u64, vp]; L.cg_merkle_root.restype = i32
     L.cg_merkle_root_fixed.argtypes = [vp, u64, u64, vp]; L.cg_merkle_root_fixed.restype = i32
@@ -335,6 +338,16 @@ class Ruleset:
         uint64[2] = (bytes needed, resolved spans) into d_sizes."""
         check(load().cg_redact_batch_device(self.handle, d_bytes, d_off, n, d_out or None, out_cap, d_out_off, d_spans or None,
                                             spans_cap, d_digests or None, d_sizes, stream))
+
+    def scan_hits_batch_device(self, d_bytes: int, d_off: int, n: int, d_words: int, d_hits: int, hits_cap: int, d_nhits: int, stream: int = 0):
+        """cg_scan_hits_batch_device on raw device pointers (asynchronous; status from scan_join): result words (uint64[n])
+        into d_words, the (msg, rule) hits (HIT_DTYPE, sorted, at most hits_cap) into d_hits, their number (uint32) into d_nhits."""
+        check(load().cg_scan_hits_batch_device(self.handle, d_bytes, d_off, n, d_words, d_hits or None, hits_cap, d_nhits, stream))
+
+    def verdict_batch_device(self, d_bytes: int, d_off: int, n: int, d_verdicts: int, stream: int = 0):
+        """cg_policy_verdict_batch_device on raw device pointers (asynchronous; status from scan_join): one uint32 verdict per
+        message into d_verdicts, as verdict_batch returns them (0xffffffff each after an internal queue overflow)."""
+        check(load().cg_policy_verdict_batch_device(self.handle, d_bytes, d_off, n, d_verdicts, stream))
 
 
 def sha256_batch(data: np.ndarray, off64: np.ndarray) -> np.ndarray:

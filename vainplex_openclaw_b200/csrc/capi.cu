@@ -47,6 +47,7 @@ struct Ctx {
   cg_span* d_spans = nullptr; size_t cap_spans = 0;
   uint8_t* d_redact_out = nullptr; size_t cap_redact_out = 0; uint32_t* d_redact_meta = nullptr; size_t cap_redact_meta = 0;
   uint32_t* d_verdicts = nullptr; size_t cap_verdicts = 0;
+  uint32_t* d_hits = nullptr; size_t cap_hits = 0;          // cg_scan_batch's hit list: [count][(msg, rule) pairs]
 } G;
 
 int fail(int code, const std::string& msg) { g_err = msg; return code; }
@@ -241,14 +242,15 @@ void default_caps(const cg_ruleset* rs, uint32_t n, bool spans, uint32_t* l1, ui
   *ev = std::max(std::max<uint32_t>(std::max<uint32_t>(n, 4096), rs->work.event_cap), rs->grow_ev);
   *span = spans ? std::max(std::max<uint32_t>(std::max<uint32_t>(n, 4096), rs->work.span_cap), rs->grow_span) : 1;
 }
-// the verify grid and the scratch of a step over n messages; growing waits for st (nothing may still use a replaced buffer)
-int prepare_step(cg_ruleset* rs, uint32_t n, bool spans, cudaStream_t st) {
+// the verify grid and the scratch of a step over n messages; growing waits for st (nothing may still use a replaced buffer).
+// per_msg: the step is followed by a hit list or verdicts, which need the per-message scratch of span-mode steps.
+int prepare_step(cg_ruleset* rs, uint32_t n, bool spans, cudaStream_t st, bool per_msg = false) {
   rs->size_verify_grid();
   const ScanWork& w = rs->work;
   uint32_t l1, slot, ev, span;
   default_caps(rs, n, spans, &l1, &slot, &ev, &span);
   n = std::max<uint32_t>(n, 1);
-  const uint32_t res = spans ? n : 0;
+  const uint32_t res = spans || per_msg ? n : 0;
   if (n <= w.msg_cap && l1 <= w.l1_cap && slot <= w.slot_cap && ev <= w.event_cap && span <= w.span_cap && res <= w.res_cap) return CG_OK;
   CU(cudaStreamSynchronize(st));
   return ensure_work(rs, rs->work, n, l1, slot, ev, span, res);
@@ -288,7 +290,7 @@ int capture(cudaStream_t st, Enqueue&& enqueue, cudaGraphExec_t* exec, int* kern
   return CG_OK;
 }
 // the rules of one hit row (rw words), lowest first: put(i, rule) for the i-th rule of the output while i < cap; returns nh
-// plus the number of rules in the row
+// plus the number of rules in the row (cg_scan_one's single row; batches build their hit list on the device)
 template <typename Put>
 uint32_t append_hit_row(const uint32_t* row, uint32_t rw, uint32_t nh, uint32_t cap, Put&& put) {
   for (uint32_t k = 0; k < rw; k++)
@@ -297,7 +299,7 @@ uint32_t append_hit_row(const uint32_t* row, uint32_t rw, uint32_t nh, uint32_t 
 }
 
 struct HostScan {
-  std::vector<uint32_t> counters, slot_msg, hit, spans;
+  std::vector<uint32_t> counters;
 };
 
 int check_offsets(const uint32_t* offsets, uint32_t n) {
@@ -305,8 +307,9 @@ int check_offsets(const uint32_t* offsets, uint32_t n) {
   return CG_OK;
 }
 
-// full host-buffer scan with capacity retry; leaves words in G.d_words (a span-mode step: in the rule set's scratch)
-int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, bool spans, HostScan* hs) {
+// full host-buffer scan with capacity retry; leaves words in G.d_words (a span-mode step: in the rule set's scratch).
+// per_msg: see prepare_step.
+int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, bool spans, HostScan* hs, bool per_msg = false) {
   if (int rc = require_ready()) return rc;
   if (!rs || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
   int rc;
@@ -323,7 +326,7 @@ int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uin
   }
   hs->counters.assign(kCounterWords, 0);
   for (int attempt = 0; attempt < 10; attempt++) {
-    if ((rc = prepare_step(rs, n, spans, st))) return rc;
+    if ((rc = prepare_step(rs, n, spans, st, per_msg))) return rc;
     CU(cudaEventRecord(G.ev0, st));
     if (n) { if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32, n, spans ? rs->work.words : G.d_words, spans, st))) return rc; }
     else CU(cudaMemsetAsync(rs->work.counters, 0, kCounterWords * sizeof(uint32_t), st));
@@ -412,7 +415,7 @@ void poll_mirrors(cg_ruleset* rs, bool wait) {
     const uint32_t* hc = rs->h_counters + (size_t)i * kCounterWords;
     rs->sticky_flags |= hc[3];
     if (!hc[3]) rs->sticky_status |= hc[16] ? 1u << hc[16] : 0u;
-    G.stats.spans += hc[20]; G.stats.sha256_items += hc[21];     // (zero for words-only steps)
+    G.stats.spans += hc[20]; G.stats.sha256_items += hc[21]; G.stats.hits += hc[23];     // (zero for steps without them)
     absorb_counters(rs, hc);                                // (cg_scan_join reports the flags)
   }
 }
@@ -472,6 +475,22 @@ int stage_one(cg_ruleset::OnePath& o, const uint8_t* bytes, uint32_t len, cudaSt
   return CG_OK;
 }
 
+// cg_scan_hits_batch_device / cg_policy_verdict_batch_device: a policy-mode step over a batch in HBM (result words to
+// d_words, or to the rule set's scratch when it is null), the per-message work enqueue(scratch) puts on st, then the counter
+// block into the mirror ring.  Launched directly (no graph); never waits for the device except when the scratch must grow.
+template <typename Enqueue>
+int policy_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, uint64_t* d_words, cudaStream_t st, Enqueue&& enqueue) {
+  int rc;
+  if ((rc = ensure_mirrors(rs))) return rc;
+  poll_mirrors(rs, false);                                  // (an earlier batch overflowed?  grow before this one runs)
+  if ((rc = prepare_step(rs, n, false, st, true))) return rc;
+  if ((rc = run_scan_device(rs, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, n, d_words ? d_words : rs->work.words, false, st))) return rc;
+  count_launches(enqueue(rs->work));
+  CU(cudaGetLastError());
+  G.stats.messages_scanned += n;
+  return mirror_counters(rs, st);
+}
+
 }  // namespace
 
 extern "C" {
@@ -509,7 +528,7 @@ void cg_shutdown(void) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!G.ready) return;
   cudaDeviceSynchronize();
-  cudaFree(G.d_spans); cudaFree(G.d_redact_out); cudaFree(G.d_redact_meta); cudaFree(G.d_verdicts);
+  cudaFree(G.d_spans); cudaFree(G.d_redact_out); cudaFree(G.d_redact_meta); cudaFree(G.d_verdicts); cudaFree(G.d_hits);
   if (G.h_chunk_counters) cudaFreeHost(G.h_chunk_counters);
   if (G.s_h2d) { cudaStreamDestroy(G.s_h2d); cudaStreamDestroy(G.s_d2h); for (int c = 0; c < Ctx::kChunks; c++) { cudaEventDestroy(G.e_h2d[c]); cudaEventDestroy(G.e_done[c]); } }
   cudaFree(G.d_bytes_raw); cudaFree(G.d_off32); cudaFree(G.d_off64); cudaFree(G.d_words); cudaFree(G.d_dig[0]); cudaFree(G.d_dig[1]);
@@ -689,27 +708,28 @@ int cg_scan_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets,
     }
     // rc == 1: a queue overflowed in some piece; capacities have been raised -- run the batch in one piece below
   }
-  rc = scan_host(rs, bytes, offsets, n, false, &hs);
+  const bool want_hits = out_hits || out_nhits;
+  rc = scan_host(rs, bytes, offsets, n, false, &hs, want_hits);
   if (rc) return rc;
   cudaStream_t st = G.stream;
   if (out_words && n) CU(cudaMemcpyAsync(out_words, G.d_words, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
-  uint32_t n_slots = hs.counters[0], rw = rs->dev.rw;
-  uint32_t nh = 0;
-  if ((out_hits || out_nhits) && n_slots) {
-    hs.slot_msg.resize(n_slots); hs.hit.resize((size_t)n_slots * rw);
-    CU(cudaMemcpyAsync(hs.slot_msg.data(), rs->work.slot_msg, (size_t)n_slots * 4, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(hs.hit.data(), rs->work.hit, (size_t)n_slots * rw * 4, cudaMemcpyDeviceToHost, st));
+  // the hit list on the device (as cg_scan_hits_batch_device builds it): counts and their scan, the total to the host, then
+  // the first min(total, hits_cap) pairs into a staging buffer and back
+  uint64_t total = 0;
+  if (want_hits && n) {
+    count_launches(launch_hit_count(rs->work, G.d_words, n, G.sm_count, st));
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(&total, rs->work.out_off + n, 8, cudaMemcpyDeviceToHost, st));
   }
   CU(cudaStreamSynchronize(st));
-  if ((out_hits || out_nhits) && n_slots) {
-    std::vector<uint32_t> order(n_slots);
-    for (uint32_t i = 0; i < n_slots; i++) order[i] = i;
-    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return hs.slot_msg[a] < hs.slot_msg[b]; });
-    for (uint32_t oi = 0; oi < n_slots; oi++) {
-      uint32_t s = order[oi];
-      if (hs.slot_msg[s] == 0xffffffffu) continue;
-      nh = append_hit_row(&hs.hit[(size_t)s * rw], rw, nh, out_hits ? hits_cap : 0, [&](uint32_t i, uint32_t r) { out_hits[i].msg = hs.slot_msg[s]; out_hits[i].rule = r; });
-    }
+  if (total >> 32) { if (out_nhits) *out_nhits = 0xffffffffu; return fail(CG_ERR_TOO_LARGE, "2^32 hits or more in one batch"); }
+  const uint32_t nh = (uint32_t)total, k = out_hits ? std::min(nh, hits_cap) : 0u;
+  if (k) {
+    if ((rc = grow(&G.d_hits, &G.cap_hits, 2 * (size_t)k + 1))) return rc;      // [count][pairs]
+    count_launches(launch_hit_emit(rs->dev, rs->work, n, G.d_hits + 1, k, G.d_hits, G.sm_count, st));
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(out_hits, G.d_hits + 1, (size_t)k * sizeof(cg_hit), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
   }
   if (out_nhits) *out_nhits = nh;
   G.stats.hits += nh;
@@ -836,7 +856,7 @@ int cg_policy_verdict_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t
   uint32_t* d_verdicts = G.d_verdicts;
   cudaStream_t st = G.stream;
   CU(cudaMemsetAsync(d_verdicts, 0, (size_t)n * 4, st));
-  int k = launch_verdicts(rs->dev, rs->work, d_verdicts, G.sm_count, st);
+  int k = launch_verdicts(rs->dev, rs->work, d_verdicts, n, G.sm_count, st);
   count_launches(k);
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(out_verdicts, d_verdicts, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
@@ -1011,9 +1031,9 @@ int cg_scan_join(cg_ruleset* rs, void* stream) {
   poll_mirrors(rs, true);
   const uint32_t flags = rs->sticky_flags, status = rs->sticky_status; rs->sticky_flags = rs->sticky_status = 0;
   if (flags & (ERR_VM_STACK | ERR_VM_LIST)) return fail(CG_ERR_TOO_LARGE, std::string(kVmOverflow) + " (result words of that batch are all ones)");
-  if (status & (1u << kResolveTooLarge)) return fail(CG_ERR_TOO_LARGE, "redacted batch exceeds 4 GiB");
+  if (status & (1u << kResolveTooLarge)) return fail(CG_ERR_TOO_LARGE, "redacted batch exceeds 4 GiB, or a batch has 2^32 - 1 hits or more");
   if (flags) return fail(CG_ERR_CAPACITY, "a candidate queue overflowed: the result words (or sizes) of that batch are all ones; the scratch has been grown, scan the batch again");
-  if (status & (1u << kResolveCapacity)) return fail(CG_ERR_CAPACITY, "output buffer too small: the sizes a batch needs are in its d_out_sizes / d_out_nspans");
+  if (status & (1u << kResolveCapacity)) return fail(CG_ERR_CAPACITY, "output buffer too small: the sizes a batch needs are in its d_out_sizes / d_out_nspans / d_out_nhits");
   return CG_OK;
 }
 
@@ -1066,6 +1086,37 @@ int cg_redact_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_of
   if ((uintptr_t)d_out_digests32 & 15u) return fail(CG_ERR_INVALID_ARG, "d_out_digests32 must be 16-byte aligned");
   const SpanOutputs o{(uint32_t*)d_out_spans, spans_cap, (uint32_t*)d_out_offsets, d_out_bytes ? out_cap : 0ull, d_out_sizes, true};
   return spans_device(rs, d_bytes, d_offsets, n, o, d_out_bytes, d_out_digests32, stream);
+}
+
+int cg_scan_hits_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_words, void* d_out_hits,
+                              uint32_t hits_cap, void* d_out_nhits, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  if (!rs || !d_bytes || !d_offsets || !d_out_words || !d_out_nhits || (hits_cap && !d_out_hits)) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if ((uintptr_t)d_bytes & 15u) return fail(CG_ERR_INVALID_ARG, "d_bytes must be 16-byte aligned");
+  if (((uintptr_t)d_offsets | (uintptr_t)d_out_hits | (uintptr_t)d_out_nhits) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets, d_out_hits and d_out_nhits must be 4-byte aligned");
+  if ((uintptr_t)d_out_words & 7u) return fail(CG_ERR_INVALID_ARG, "d_out_words must be 8-byte aligned");
+  cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
+  if (!n) { CU(cudaMemsetAsync(d_out_nhits, 0, 4, st)); return CG_OK; }
+  uint64_t* words = (uint64_t*)d_out_words;
+  return policy_device(rs, d_bytes, d_offsets, n, words, st, [&](const ScanWork& w) {
+    return launch_hit_count(w, words, n, G.sm_count, st) +
+           launch_hit_emit(rs->dev, w, n, (uint32_t*)d_out_hits, d_out_hits ? hits_cap : 0u, (uint32_t*)d_out_nhits, G.sm_count, st);
+  });
+}
+
+int cg_policy_verdict_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_verdicts, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  if (!rs || !d_bytes || !d_offsets || !d_out_verdicts) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (!rs->dev.rule_policy) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy has not been called");
+  if ((uintptr_t)d_bytes & 15u) return fail(CG_ERR_INVALID_ARG, "d_bytes must be 16-byte aligned");
+  if (((uintptr_t)d_offsets | (uintptr_t)d_out_verdicts) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets and d_out_verdicts must be 4-byte aligned");
+  cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
+  if (!n) return CG_OK;
+  uint32_t* verdicts = (uint32_t*)d_out_verdicts;
+  CU(cudaMemsetAsync(verdicts, 0, (size_t)n * 4, st));       // (verdict_kernel writes the messages that hit)
+  return policy_device(rs, d_bytes, d_offsets, n, nullptr, st, [&](const ScanWork& w) { return launch_verdicts(rs->dev, w, verdicts, n, G.sm_count, st); });
 }
 
 // ---------------------------------------------------------------------------------- SHA / Merkle

@@ -60,6 +60,7 @@ struct ScanWork {
                                  //           [6]=flagged grams (level 1a) [7..15]=debug [17]=n_heavy [18]=verify cursor (light events) [19]=grams past the recheck map
                                  //           [24..27]=flag words queued, [28..31]=(gram, entry) pairs compared, per piece of the batch
                                  //           span resolution: [16]=status (kResolve*) [20]=resolved spans [21]=digests to compute [22]=messages to splice
+                                 //           hit list: [16]=status (kResolve*) [23]=(msg, rule) hits
   uint32_t* l1_pos;              // [l1_cap] factor occurrences scan_kernel confirms itself (head check, trigger bytes): buffer offset of the
   uint32_t* l1_fac;              //          factor's first byte, factor id
   uint2* fq;                     // [l1_cap] scan_kernel's flag words: x = the lane's chunk number after the round, y = 4 tiles x 8 (4) probe bits
@@ -75,13 +76,13 @@ struct ScanWork {
   uint32_t* spans;               // [span_cap * 6] msg, rule, start_byte, end_byte, start16, end16
   uint32_t l1_cap, msg_cap, slot_cap, event_cap, span_cap;
   uint32_t q_cap, q_slot;        // this launch's piece of fq (a step scans the batch in up to 4 pieces: q_slot 0..3) and its counter [24 + q_slot]
-  // span resolution (span-mode steps only): [res_cap + 1] per message, [span_cap] per raw span
-  uint64_t* words;               // [res_cap] result words of span-mode steps
+  // span resolution (span-mode steps) and hit lists: [res_cap + 1] per message, [span_cap] per raw span
+  uint64_t* words;               // [res_cap] result words of span-mode steps and of cg_policy_verdict_batch_device
   uint32_t* seg_cnt;             // raw spans per message (counted down again by the scatter)
   uint32_t* seg_begin;           // exclusive scan of seg_cnt: the message's segment of `sorted`
   uint32_t* kept_cnt;            // spans resolveOverlaps keeps per message
   uint32_t* kept_begin;          // exclusive scan of kept_cnt: the message's first resolved span
-  uint64_t* out_len;             // redacted bytes per message
+  uint64_t* out_len;             // redacted bytes per message (hit list: rules hit per message)
   uint64_t* out_off;             // exclusive scan of out_len
   uint4* sorted;                 // [span_cap] (start16, ~length16, rule rank, raw span index) in message order; kept keys first
   uint4* sort_tmp;               // [span_cap] merge passes of long segments
@@ -116,8 +117,16 @@ int launch_resolve(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_byt
 // CTAs per SM than at one, so the caller sizes the grid by what the previous steps sent to the VM
 int launch_verify(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off,
                   bool want_spans, int sm_count, cudaStream_t stream, int ctas_per_sm = 4);
-// one verdict word per hit message: action | matched policies << 2 | deciding rule << 12 (cg_policy_verdict_batch)
-int launch_verdicts(const DevRuleset& rs, const ScanWork& w, uint32_t* d_verdicts, int sm_count, cudaStream_t stream);
+// one verdict word per hit message: action | matched policies << 2 | deciding rule << 12 (cg_policy_verdict_batch); on an
+// incomplete step all n verdicts = 0xffffffff
+int launch_verdicts(const DevRuleset& rs, const ScanWork& w, uint32_t* d_verdicts, uint32_t n, int sm_count, cudaStream_t stream);
+// the hit list of a finished policy-mode step (w.res_cap >= n): the hit count of every result word into w.out_len and their
+// exclusive scan into w.out_off (w.out_off[n] = the total); then the (msg, rule) pairs sorted by (msg, rule), the first cap
+// of them, as two u32 each into d_out, the total into *d_count (0xffffffff: incomplete step, or 2^32 - 1 hits or more) and
+// counters[23], the status into counters[16] (kResolveCapacity past cap, kResolveTooLarge).  Grids depend on n and the SM
+// count only.
+int launch_hit_count(const ScanWork& w, const uint64_t* d_words, uint32_t n, int sm_count, cudaStream_t stream);
+int launch_hit_emit(const DevRuleset& rs, const ScanWork& w, uint32_t n, uint32_t* d_out, uint32_t cap, uint32_t* d_count, int sm_count, cudaStream_t stream);
 int launch_finalize(const DevRuleset& rs, const ScanWork& w, uint64_t* d_words, uint32_t n, int sm_count, cudaStream_t stream);
 // start of a step: counters = 0, slot_of_msg = none, candidate / hit rows of the slots the previous step used = 0
 int launch_reset(const DevRuleset& rs, const ScanWork& w, uint32_t n, int sm_count, cudaStream_t stream);

@@ -707,7 +707,13 @@ __global__ void finalize_kernel(DevRuleset rs, ScanWork w, uint64_t* __restrict_
 // policies in priority order, per policy the FIRST matching rule counts, deny beats audit beats allow, and the first
 // policy that produced the winning action is the one whose reason is reported.  Rules are stored policy by policy, so an
 // ascending walk over the hit bits meets every policy's deciding rule first.
-__global__ void verdict_kernel(DevRuleset rs, ScanWork w, uint32_t* __restrict__ verdicts) {
+// An incomplete step (a queue overflowed, the VM failed) has no verdicts: every one of the batch is 0xffffffff, which no
+// verdict can be (action 3 does not exist).
+__global__ void verdict_kernel(DevRuleset rs, ScanWork w, uint32_t* __restrict__ verdicts, uint32_t n) {
+  if (w.counters[3]) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) verdicts[i] = 0xffffffffu;
+    return;
+  }
   const uint32_t n_slots = min(w.counters[0], w.slot_cap);
   for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_slots; s += gridDim.x * blockDim.x) {
     const uint32_t msg = w.slot_msg[s];
@@ -725,6 +731,56 @@ __global__ void verdict_kernel(DevRuleset rs, ScanWork w, uint32_t* __restrict__
       }
     }
     if (matched) verdicts[msg] = best | (min(matched, 1023u) << 2) | (decide << 12);
+  }
+}
+
+// The (msg, rule) hit list of a finished policy-mode step, sorted by message, then rule (cg_scan_hits_batch_device,
+// cg_scan_batch): hit_count_kernel -> exclusive scan of the counts -> hit_emit_kernel.
+// cnt[m] = the rules message m hit, from its result word (finalize_kernel counted them in the same hit row); cnt[n] = 0, so
+// that the scan's last element is the total.
+__global__ void __launch_bounds__(256) hit_count_kernel(const uint64_t* __restrict__ words, uint32_t n, uint64_t* __restrict__ cnt) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += gridDim.x * blockDim.x) {
+    const uint64_t v = i < n ? words[i] : 0ull;
+    cnt[i] = (v >> 63) ? (v >> 32) & 0x7fffffffull : 0ull;
+  }
+}
+
+// One warp per 32 consecutive messages: a ballot finds the ones with hits (w.out_len = counts, w.out_off = their exclusive
+// scan), then all 32 lanes write each such message's hit row together -- lane k takes row words k, k + 32, ..., and a popc
+// prefix over the lanes places its rules -- so a row of 157 words (5000 rules) costs five wave steps, not one lane's walk.
+// Pairs go to out (two u32 each) below position cap only.  *count = the total (0xffffffff: incomplete step, or 2^32 - 1 hits
+// or more), also counters[23] for cg_stats.hits; counters[16] = kResolveCapacity / kResolveTooLarge past cap / 2^32 - 1.
+__global__ void __launch_bounds__(256) hit_emit_kernel(DevRuleset rs, ScanWork w, uint32_t n, uint32_t* __restrict__ out, uint32_t cap,
+                                                       uint32_t* __restrict__ count) {
+  const bool incomplete = w.counters[3] != 0;
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    const uint64_t total = w.out_off[n];
+    if (incomplete) *count = 0xffffffffu;
+    else {
+      const uint32_t t = total >= 0xffffffffull ? 0xffffffffu : (uint32_t)total;
+      *count = t; w.counters[23] = t;
+      w.counters[16] = total >= 0xffffffffull ? kResolveTooLarge : total > cap ? kResolveCapacity : kResolveOk;
+    }
+  }
+  if (incomplete) return;
+  const uint32_t lane = threadIdx.x & 31, warps = gridDim.x * (blockDim.x / 32);
+  for (uint32_t g = blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5); (uint64_t)g * 32 < n; g += warps) {
+    const uint32_t m = g * 32 + lane;
+    const uint32_t c = m < n ? (uint32_t)w.out_len[m] : 0u;
+    const uint64_t at = m < n ? w.out_off[m] : 0ull;
+    for (uint32_t todo = __ballot_sync(0xffffffffu, c != 0 && at < cap); todo; todo &= todo - 1) {
+      const uint32_t j = __ffs(todo) - 1, msg = g * 32 + j;
+      uint64_t pos = __shfl_sync(0xffffffffu, at, j);
+      const uint32_t* row = w.hit + (size_t)w.slot_of_msg[msg] * rs.rw;
+      for (uint32_t k0 = 0; k0 < rs.rw && pos < cap; k0 += 32) {          // (pos is the same on every lane)
+        uint32_t v = k0 + lane < rs.rw ? row[k0 + lane] : 0u;
+        const uint32_t pc = __popc(v);
+        uint32_t incl = pc;
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= (uint32_t)d) incl += t; }
+        for (uint64_t p = pos + (incl - pc); v && p < cap; v &= v - 1, p++) { out[2 * p] = msg; out[2 * p + 1] = (k0 + lane) * 32 + (__ffs(v) - 1); }
+        pos += __shfl_sync(0xffffffffu, incl, 31);
+      }
+    }
   }
 }
 
@@ -798,8 +854,18 @@ int launch_verify(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_byte
   return k;
 }
 
-int launch_verdicts(const DevRuleset& rs, const ScanWork& w, uint32_t* d_verdicts, int sm_count, cudaStream_t stream) {
-  verdict_kernel<<<sm_count * 2, 256, 0, stream>>>(rs, w, d_verdicts);
+int launch_verdicts(const DevRuleset& rs, const ScanWork& w, uint32_t* d_verdicts, uint32_t n, int sm_count, cudaStream_t stream) {
+  verdict_kernel<<<sm_count * 2, 256, 0, stream>>>(rs, w, d_verdicts, n);
+  return 1;
+}
+
+int launch_hit_count(const ScanWork& w, const uint64_t* d_words, uint32_t n, int sm_count, cudaStream_t stream) {
+  hit_count_kernel<<<sm_count * 4, 256, 0, stream>>>(d_words, n, w.out_len);
+  return 1 + launch_exclusive_scan(w.out_len, w.out_off, n + 1, w.scan_part, sm_count, stream);
+}
+int launch_hit_emit(const DevRuleset& rs, const ScanWork& w, uint32_t n, uint32_t* d_out, uint32_t cap, uint32_t* d_count, int sm_count, cudaStream_t stream) {
+  const uint32_t blocks = std::max<uint32_t>(1u, std::min<uint32_t>((uint32_t)(((uint64_t)n + 255) / 256), (uint32_t)sm_count * 4));   // 8 warps x 32 messages per block
+  hit_emit_kernel<<<blocks, 256, 0, stream>>>(rs, w, n, d_out, cap, d_count);
   return 1;
 }
 
