@@ -28,6 +28,12 @@ class Harness:
                     n_always=int(o[4]), image_bytes=int(o[5]), prog_words=int(o[6]), entries=int(o[7]), shapes=int(o[8]),
                     triggers=int(o[9]), bitmap_bytes=int(o[10]), tables_resident=int(o[11]))
 
+    def confirm_block_bytes(self):
+        """bytes of confirm_kernel's table block for this rule set (staged in shared memory up to kConfirmTableBudget)"""
+        self.L.harness_confirm_bytes.restype = C.c_uint32
+        self.L.harness_confirm_bytes.argtypes = [C.c_void_p]
+        return int(self.L.harness_confirm_bytes(self.h))
+
     def find_all(self, rule, msg: bytes):
         cap = 64
         while True:

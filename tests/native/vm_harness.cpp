@@ -78,6 +78,17 @@ void harness_info(void* p, uint32_t* out) {
   out[7] = (uint32_t)h->H.pf.entries.size(); out[8] = (uint32_t)h->H.pf.shapes.size(); out[9] = (uint32_t)h->H.pf.trig_bytes.size();
   out[10] = h->H.bm_bytes; out[11] = h->H.tables_resident ? 1u : 0u;
 }
+// bytes of confirm_kernel's table block, laid out as cg_ruleset_create lays it out (capi.cu): recheck map, slots, group
+// entries (+16), factor words (+64), byte sets (+32), each part rounded up to 16 bytes.  The kernel stages the block into
+// shared memory when it is at most kConfirmTableBudget bytes.
+uint32_t harness_confirm_bytes(void* p) {
+  const HostImage& H = ((Harness*)p)->H;
+  size_t n = 0;
+  auto put = [&](size_t bytes, size_t pad) { n = (n + bytes + pad + 15) & ~(size_t)15; };
+  put(H.rk_bytes, 0); put(H.slot_words.size() * 4, 0); put(H.group_entries.size() * 4, 16);
+  put(H.factor_words.size() * 4, 64); put(H.pf.bytesets.size() * 4, 32);
+  return (uint32_t)n;
+}
 const char* harness_rule_error(void* p, uint32_t rule) { return ((Harness*)p)->H.rules[rule].error.c_str(); }
 int harness_rule_nfactors(void* p, uint32_t rule) { return (int)((Harness*)p)->H.rules[rule].factors.size(); }
 int harness_rule_exact(void* p, uint32_t rule) { return ((Harness*)p)->H.rules[rule].factors_exact ? 1 : 0; }
