@@ -116,7 +116,7 @@ struct cg_ruleset {
   // verify_small_kernel's grid (CTAs per SM): one while the island matcher decides (nearly) everything, four once a step has
   // sent more than 2048 pairs to the VM (non-ASCII traffic); back to one below 256.  Part of the cached graphs' keys.
   int verify_ctas = 1;
-  void size_verify_grid() { const uint32_t ev = last_counters[1]; if (ev > 2048u) verify_ctas = 4; else if (ev < 256u) verify_ctas = 1; }
+  void size_verify_grid() { const uint32_t ev = last_counters[kCtrEvents]; if (ev > 2048u) verify_ctas = 4; else if (ev < 256u) verify_ctas = 1; }
   uint32_t last_counters[kCounterWords] = {};
   uint64_t scratch_gen = 0;       // advanced by every change to what a captured step holds (scratch buffers, DevRuleset)
   // the device-resident step replayed as one CUDA graph (keyed on its arguments, the scratch generation and the verify grid)
@@ -201,9 +201,16 @@ int ensure_work(cg_ruleset* rs, ScanWork& w, uint32_t n_msgs, uint32_t l1_cap, u
 }
 
 static uint32_t scan_pieces() { static const uint32_t k = [] { const char* e = getenv("CG_PIECES"); const int v = e ? atoi(e) : 1; return (uint32_t)(v >= 1 && v <= 4 ? v : 1); }(); return k; }
-// One step on device-resident input: scratch reset, gram scan (+ exact factors), resolve, verify, finalize.  Asynchronous.
-int run_scan_device(cg_ruleset* rs, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, uint64_t* d_words, bool spans, cudaStream_t st) {
+// What a step computes: result words only; a policy step whose per-message scratch a hit list or verdicts read afterwards;
+// or a span step (raw spans for the span resolver, result words in ScanWork::words).
+enum StepKind { kStepWords, kStepPolicy, kStepSpans };
+
+// One step on device-resident input: scratch reset, gram scan (+ exact factors), resolve, verify, finalize; over no message
+// only the zeroed counter block.  Asynchronous.
+int run_scan_device(cg_ruleset* rs, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, uint64_t* d_words, StepKind kind, cudaStream_t st) {
   const ScanWork& w = rs->work;
+  if (!n) { CU(cudaMemsetAsync(w.counters, 0, kCounterWords * sizeof(uint32_t), st)); return CG_OK; }
+  const bool spans = kind == kStepSpans;
   int k = launch_reset(rs->dev, w, n, G.sm_count, st);
   if (G.profiling) cudaEventRecord(G.pev[0], st);
   // CG_PIECES = 2..4 scans the batch in pieces, each followed by its own lookup + check, so that a flagged gram is read again
@@ -236,43 +243,48 @@ void prepare_kernels() { static bool done = false; if (!done) { prepare_scan_ker
 
 // capacities a batch of n messages starts with (confirmed occurrences are rare: about one per hundred messages on chat text;
 // a step without spans writes none)
-void default_caps(const cg_ruleset* rs, uint32_t n, bool spans, uint32_t* l1, uint32_t* slot, uint32_t* ev, uint32_t* span) {
+void default_caps(const cg_ruleset* rs, uint32_t n, StepKind kind, uint32_t* l1, uint32_t* slot, uint32_t* ev, uint32_t* span) {
   *l1 = std::max(std::max<uint32_t>(std::max<uint32_t>(2 * n, 1u << 16), rs->work.l1_cap), rs->grow_l1);
   *slot = std::max(std::max<uint32_t>(std::max<uint32_t>(n / 4, 4096), rs->work.slot_cap), rs->grow_slot);
   *ev = std::max(std::max<uint32_t>(std::max<uint32_t>(n, 4096), rs->work.event_cap), rs->grow_ev);
-  *span = spans ? std::max(std::max<uint32_t>(std::max<uint32_t>(n, 4096), rs->work.span_cap), rs->grow_span) : 1;
+  *span = kind == kStepSpans ? std::max(std::max<uint32_t>(std::max<uint32_t>(n, 4096), rs->work.span_cap), rs->grow_span) : 1;
 }
-// the verify grid and the scratch of a step over n messages; growing waits for st (nothing may still use a replaced buffer).
-// per_msg: the step is followed by a hit list or verdicts, which need the per-message scratch of span-mode steps.
-int prepare_step(cg_ruleset* rs, uint32_t n, bool spans, cudaStream_t st, bool per_msg = false) {
+// the verify grid and the scratch of a step over n messages; growing waits for st (nothing may still use a replaced buffer)
+int prepare_step(cg_ruleset* rs, uint32_t n, StepKind kind, cudaStream_t st) {
   rs->size_verify_grid();
   const ScanWork& w = rs->work;
   uint32_t l1, slot, ev, span;
-  default_caps(rs, n, spans, &l1, &slot, &ev, &span);
+  default_caps(rs, n, kind, &l1, &slot, &ev, &span);
   n = std::max<uint32_t>(n, 1);
-  const uint32_t res = spans || per_msg ? n : 0;
+  const uint32_t res = kind != kStepWords ? n : 0;
   if (n <= w.msg_cap && l1 <= w.l1_cap && slot <= w.slot_cap && ev <= w.event_cap && span <= w.span_cap && res <= w.res_cap) return CG_OK;
   CU(cudaStreamSynchronize(st));
   return ensure_work(rs, rs->work, n, l1, slot, ev, span, res);
 }
 // fq is cut into four equal pieces at most: the fullest piece decides
-static uint32_t queue_need(const uint32_t* hc) { uint32_t m = 0; for (int i = 24; i < 28; i++) m = std::max(m, hc[i]); return m > 0xffffffffu / scan_pieces() ? 0xffffffffu : scan_pieces() * m; }
+static uint32_t queue_need(const uint32_t* hc) { uint32_t m = 0; for (int i = 0; i < 4; i++) m = std::max(m, hc[kCtrFlagWords + i]); return m > 0xffffffffu / scan_pieces() ? 0xffffffffu : scan_pieces() * m; }
 // what an overflowed step teaches about the capacities the next one needs
 void learn_caps(cg_ruleset* rs, const uint32_t* hc) {
-  const uint32_t flags = hc[3];
-  if (flags & ERR_L1_OVERFLOW) { const uint32_t need = std::max(hc[4], queue_need(hc)); rs->grow_l1 = std::max<uint32_t>(rs->grow_l1, std::max<uint32_t>(2 * need, need + 65536)); }
-  if (flags & ERR_SLOT_OVERFLOW) rs->grow_slot = std::max<uint32_t>(rs->grow_slot, std::max<uint32_t>(2 * hc[0], hc[0] + 4096));
-  if (flags & ERR_EVENT_OVERFLOW) rs->grow_ev = std::max<uint32_t>(rs->grow_ev, std::max<uint32_t>(2 * hc[1], hc[1] + 4096));
-  if (flags & ERR_SPAN_OVERFLOW) rs->grow_span = std::max<uint32_t>(rs->grow_span, std::max<uint32_t>(2 * hc[2], hc[2] + 4096));
+  const uint32_t flags = hc[kCtrErrors];
+  if (flags & ERR_L1_OVERFLOW) { const uint32_t need = std::max(hc[kCtrConfirmed], queue_need(hc)); rs->grow_l1 = std::max<uint32_t>(rs->grow_l1, std::max<uint32_t>(2 * need, need + 65536)); }
+  if (flags & ERR_SLOT_OVERFLOW) rs->grow_slot = std::max<uint32_t>(rs->grow_slot, std::max<uint32_t>(2 * hc[kCtrSlots], hc[kCtrSlots] + 4096));
+  if (flags & ERR_EVENT_OVERFLOW) rs->grow_ev = std::max<uint32_t>(rs->grow_ev, std::max<uint32_t>(2 * hc[kCtrEvents], hc[kCtrEvents] + 4096));
+  if (flags & ERR_SPAN_OVERFLOW) rs->grow_span = std::max<uint32_t>(rs->grow_span, std::max<uint32_t>(2 * hc[kCtrRawSpans], hc[kCtrRawSpans] + 4096));
 }
 const char* const kVmOverflow = "matcher thread list / stack overflow on device";
 // a finished step's counter block -> CG_OK, CG_ERR_TOO_LARGE, or 1 = a queue overflowed (the capacities the step needs
 // have been learnt)
 int absorb_counters(cg_ruleset* rs, const uint32_t* hc) {
   memcpy(rs->last_counters, hc, sizeof rs->last_counters);
-  if (hc[3] & (ERR_VM_STACK | ERR_VM_LIST)) return fail(CG_ERR_TOO_LARGE, kVmOverflow);
-  if (hc[3]) learn_caps(rs, hc);
-  return hc[3] ? 1 : CG_OK;
+  if (hc[kCtrErrors] & (ERR_VM_STACK | ERR_VM_LIST)) return fail(CG_ERR_TOO_LARGE, kVmOverflow);
+  if (hc[kCtrErrors]) learn_caps(rs, hc);
+  return hc[kCtrErrors] ? 1 : CG_OK;
+}
+// the statistics of a completed host-side step over n messages of `bytes` bytes (device calls count messages at enqueue and
+// the rest in poll_mirrors)
+void count_step(uint32_t n, uint64_t bytes, const uint32_t* hc) {
+  G.stats.messages_scanned += n; G.stats.bytes_scanned += bytes;
+  G.stats.candidate_events += hc[kCtrEvents]; G.stats.verified_pairs += hc[kCtrEvents];
 }
 // the kernels enqueue() puts on st, captured as one graph; they are counted each time the graph is launched, not here
 template <typename Enqueue>
@@ -298,18 +310,17 @@ uint32_t append_hit_row(const uint32_t* row, uint32_t rw, uint32_t nh, uint32_t 
   return nh;
 }
 
-struct HostScan {
-  std::vector<uint32_t> counters;
-};
-
 int check_offsets(const uint32_t* offsets, uint32_t n) {
   for (uint32_t i = 0; i < n; i++) if (offsets[i + 1] < offsets[i]) return fail(CG_ERR_INVALID_ARG, "offsets must be non-decreasing");
   return CG_OK;
 }
 
-// full host-buffer scan with capacity retry; leaves words in G.d_words (a span-mode step: in the rule set's scratch).
-// per_msg: see prepare_step.
-int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, bool spans, HostScan* hs, bool per_msg = false) {
+// The host-buffer calls' driver: stages the batch into G.d_bytes / G.d_off32, then per attempt the step of `kind` (result
+// words to G.d_words, a span step's to the scratch), the work after(scratch) enqueues behind it (-> CG_OK or an error; it
+// may copy sizes to the host, never into the caller's buffers), the counter block to the host and one synchronise.  A
+// queue overflow grows the scratch and runs the attempt again.  last_scan_ms times the step alone.
+template <typename After>
+int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, StepKind kind, After&& after) {
   if (int rc = require_ready()) return rc;
   if (!rs || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
   int rc;
@@ -324,20 +335,20 @@ int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uin
     CU(cudaMemsetAsync(G.d_bytes + total, 0, 64, st));
     CU(cudaMemcpyAsync(G.d_off32, offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
   }
-  hs->counters.assign(kCounterWords, 0);
+  uint32_t hc[kCounterWords] = {};
   for (int attempt = 0; attempt < 10; attempt++) {
-    if ((rc = prepare_step(rs, n, spans, st, per_msg))) return rc;
+    if ((rc = prepare_step(rs, n, kind, st))) return rc;
+    const ScanWork& w = rs->work;
     CU(cudaEventRecord(G.ev0, st));
-    if (n) { if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32, n, spans ? rs->work.words : G.d_words, spans, st))) return rc; }
-    else CU(cudaMemsetAsync(rs->work.counters, 0, kCounterWords * sizeof(uint32_t), st));
+    if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32, n, kind == kStepSpans ? w.words : G.d_words, kind, st))) return rc;
     CU(cudaEventRecord(G.ev1, st));
-    CU(cudaMemcpyAsync(hs->counters.data(), rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
+    if ((rc = after(w))) return rc;
+    CU(cudaMemcpyAsync(hc, w.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     float ms = 0; cudaEventElapsedTime(&ms, G.ev0, G.ev1); G.stats.last_scan_ms = ms;
-    if ((rc = absorb_counters(rs, hs->counters.data())) == 1) continue;
+    if ((rc = absorb_counters(rs, hc)) == 1) continue;
     if (rc) return rc;
-    G.stats.messages_scanned += n; G.stats.bytes_scanned += total - first;
-    G.stats.candidate_events += hs->counters[1]; G.stats.verified_pairs += hs->counters[1];
+    count_step(n, total - first, hc);
     return CG_OK;
   }
   return fail(CG_ERR_CAPACITY, "candidate queues kept overflowing");
@@ -367,7 +378,7 @@ int scan_host_chunked(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offs
   cudaStream_t st = G.stream;
   const uint32_t per = (n + C - 1) / C;
   CU(cudaStreamSynchronize(st));                            // (whatever still read the staging buffers is done: s_h2d does not wait for st)
-  if ((rc = prepare_step(rs, per, false, st))) return rc;
+  if ((rc = prepare_step(rs, per, kStepWords, st))) return rc;
   CU(cudaMemcpyAsync(G.d_off32, offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, G.s_h2d));
   CU(cudaMemsetAsync(G.d_bytes + total, 0, 64, G.s_h2d));
   CU(cudaEventRecord(G.ev0, st));
@@ -382,7 +393,7 @@ int scan_host_chunked(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offs
     CU(cudaStreamWaitEvent(st, G.e_h2d[c], 0));
     // (a piece reads up to 16 bytes past its last message -- bytes of the next piece that may still be in flight; whatever
     // it sees there cannot produce an occurrence inside its own range)
-    if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32 + m0, m1 - m0, G.d_words + m0, false, st))) return rc;
+    if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32 + m0, m1 - m0, G.d_words + m0, kStepWords, st))) return rc;
     CU(cudaMemcpyAsync(G.h_chunk_counters + (size_t)c * kCounterWords, rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(G.e_done[c], st));
     CU(cudaStreamWaitEvent(G.s_d2h, G.e_done[c], 0));
@@ -392,16 +403,15 @@ int scan_host_chunked(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offs
   CU(cudaStreamSynchronize(st)); CU(cudaStreamSynchronize(G.s_d2h)); CU(cudaStreamSynchronize(G.s_h2d));
   float ms = 0; cudaEventElapsedTime(&ms, G.ev0, G.ev1); G.stats.last_scan_ms = ms;
   bool overflow = false;
-  uint64_t events = 0;
   for (int c = 0; c < used; c++) {
-    const uint32_t* hc = G.h_chunk_counters + (size_t)c * kCounterWords;
-    if ((rc = absorb_counters(rs, hc)) < 0) return rc;
+    if ((rc = absorb_counters(rs, G.h_chunk_counters + (size_t)c * kCounterWords)) < 0) return rc;
     overflow |= rc == 1;
-    events += hc[1];
   }
   if (overflow) return 1;
-  G.stats.messages_scanned += n; G.stats.bytes_scanned += total - offsets[0];
-  G.stats.candidate_events += events; G.stats.verified_pairs += events;
+  for (int c = 0; c < used; c++) {
+    const uint32_t m0 = c * per, m1 = std::min<uint64_t>((uint64_t)(c + 1) * per, n);
+    count_step(m1 - m0, offsets[m1] - offsets[m0], G.h_chunk_counters + (size_t)c * kCounterWords);
+  }
   return CG_OK;
 }
 
@@ -413,9 +423,9 @@ void poll_mirrors(cg_ruleset* rs, bool wait) {
     else if (cudaEventQuery(rs->e_cnt[i]) != cudaSuccess) { cudaGetLastError(); continue; }
     rs->cnt_pending[i] = false;
     const uint32_t* hc = rs->h_counters + (size_t)i * kCounterWords;
-    rs->sticky_flags |= hc[3];
-    if (!hc[3]) rs->sticky_status |= hc[16] ? 1u << hc[16] : 0u;
-    G.stats.spans += hc[20]; G.stats.sha256_items += hc[21]; G.stats.hits += hc[23];     // (zero for steps without them)
+    rs->sticky_flags |= hc[kCtrErrors];
+    if (!hc[kCtrErrors]) rs->sticky_status |= hc[kCtrResolveStatus] ? 1u << hc[kCtrResolveStatus] : 0u;
+    G.stats.spans += hc[kCtrResolved]; G.stats.sha256_items += hc[kCtrDigests]; G.stats.hits += hc[kCtrHits];     // (zero for steps without them)
     absorb_counters(rs, hc);                                // (cg_scan_join reports the flags)
   }
 }
@@ -441,7 +451,7 @@ int mirror_counters(cg_ruleset* rs, cudaStream_t st) {
 // [word][counters][hit row] out (kOneOut).  The span calls add, on their first use, the packed result (kOnePack bytes,
 // layout in kernels.h) on both sides and, on the device only, the digests and the redacted bytes before the pack step
 // moves them behind the spans (kOnePack each).
-constexpr uint32_t kOneBytes = 16384, kOneRw = 128, kOneIn = 256 + kOneBytes + 64, kOneOut = (2 + kCounterWords + kOneRw) * 4;
+constexpr uint32_t kOneBytes = 16384, kOneRw = 128, kOneIn = 256 + kOneBytes + 64, kOneOut = (kOneHitRow + kOneRw) * 4;
 constexpr uint32_t kOnePack = 512 * 1024;
 // the resolver's capacities on this path: every resolved span (and, redacting, its digest and the output) must fit the block
 constexpr uint32_t kOneSpansFind = (kOnePack - kPackHeader) / 24, kOneSpansRedact = (kOnePack - kPackHeader) / 56;
@@ -475,20 +485,61 @@ int stage_one(cg_ruleset::OnePath& o, const uint8_t* bytes, uint32_t len, cudaSt
   return CG_OK;
 }
 
-// cg_scan_hits_batch_device / cg_policy_verdict_batch_device: a policy-mode step over a batch in HBM (result words to
-// d_words, or to the rule set's scratch when it is null), the per-message work enqueue(scratch) puts on st, then the counter
-// block into the mirror ring.  Launched directly (no graph); never waits for the device except when the scratch must grow.
-template <typename Enqueue>
-int policy_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, uint64_t* d_words, cudaStream_t st, Enqueue&& enqueue) {
+// cg_scan_batch_device's step as a CUDA graph: captured once per (arguments, scratch generation, verify grid) into the
+// least recently used of two entries, then replayed -- one launch per step instead of six, so the host never becomes the
+// bottleneck
+template <typename Step>
+int replay_step(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_words, cudaStream_t st, Step&& step) {
+  cg_ruleset::CachedGraph* hit = nullptr;
+  for (auto& g : rs->graphs) if (g.exec && g.bytes == d_bytes && g.off == d_offsets && g.words == d_words && g.n == n && g.gen == rs->scratch_gen && g.ctas == rs->verify_ctas) hit = &g;
+  if (!hit) {
+    hit = rs->graphs[0].used <= rs->graphs[1].used ? &rs->graphs[0] : &rs->graphs[1];
+    if (hit->exec) { cudaGraphExecDestroy(hit->exec); hit->exec = nullptr; }
+    if (int rc = capture(st, step, &hit->exec, &hit->kernels)) return rc;
+    hit->bytes = d_bytes; hit->off = d_offsets; hit->words = d_words; hit->n = n; hit->gen = rs->scratch_gen; hit->ctas = rs->verify_ctas;
+  }
+  hit->used = ++rs->graph_clock;
+  CU(cudaGraphLaunch(hit->exec, st));
+  count_launches(hit->kernels);
+  return CG_OK;
+}
+
+// The device-resident calls' driver, asynchronous on st: grows the scratch first if an earlier batch overflowed, enqueues
+// the step of `kind` (replayed as a graph when `graph`), the work after(scratch) enqueues behind it (-> its launch count)
+// and the counter block into the mirror ring.  Result words go to d_words, or when it is null to the scratch's (looked up
+// after prepare_step, which may replace that buffer).  Never waits for the device except when the scratch must grow.
+template <typename After>
+int scan_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, uint64_t* d_words, StepKind kind, cudaStream_t st,
+                After&& after, bool graph = false) {
   int rc;
   if ((rc = ensure_mirrors(rs))) return rc;
   poll_mirrors(rs, false);                                  // (an earlier batch overflowed?  grow before this one runs)
-  if ((rc = prepare_step(rs, n, false, st, true))) return rc;
-  if ((rc = run_scan_device(rs, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, n, d_words ? d_words : rs->work.words, false, st))) return rc;
-  count_launches(enqueue(rs->work));
+  if ((rc = prepare_step(rs, n, kind, st))) return rc;
+  if (!d_words) d_words = rs->work.words;
+  const auto step = [&] { return run_scan_device(rs, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, n, d_words, kind, st); };
+  if ((rc = graph ? replay_step(rs, d_bytes, d_offsets, n, d_words, st, step) : step())) return rc;
+  count_launches(after(rs->work));
   CU(cudaGetLastError());
   G.stats.messages_scanned += n;
   return mirror_counters(rs, st);
+}
+
+// the checks every device-resident call starts with: an initialised library, a rule set and the batch in HBM (16-byte aligned)
+int device_batch_args(const cg_ruleset* rs, const void* d_bytes, const void* d_offsets) {
+  if (int rc = require_ready()) return rc;
+  if (!rs || !d_bytes || !d_offsets) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if ((uintptr_t)d_bytes & 15u) return fail(CG_ERR_INVALID_ARG, "d_bytes must be 16-byte aligned");
+  return CG_OK;
+}
+
+// the redacted output behind a span resolver: SHA-256 of every resolved span into d_digests, then the copy + placeholder
+// splice of n messages into d_out.  The resolver set how many of each run (counters[kCtrDigests] / [kCtrSplice]: none unless
+// every output fits).
+int enqueue_redact_tail(const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, const uint32_t* d_out_offsets, uint32_t* d_digests,
+                        uint8_t* d_out, uint32_t n, cudaStream_t st) {
+  const int k = launch_redact_digests(d_bytes, w.sp_start, w.sp_len, w.counters + kCtrDigests, d_digests, G.sm_count, st);
+  return k + launch_redact_splice(d_bytes, d_off, d_out_offsets, w.kept_begin, w.sp_start, w.sp_len, w.sp_cat, d_digests, d_out,
+                                  w.counters + kCtrSplice, n, G.sm_count, st);
 }
 
 }  // namespace
@@ -568,7 +619,7 @@ int cg_scan_work_counters(const cg_ruleset* rs, uint32_t out16[16]) {
   if (!rs || !out16) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (!rs->work.counters) return fail(CG_ERR_INVALID_ARG, "no scan has run");
   memcpy(out16, rs->last_counters, 64);
-  if (!(rs->dev.debug_flags & 2u)) { out16[7] = rs->last_counters[19]; out16[8] = out16[9] = 0; for (int i = 0; i < 4; i++) { out16[8] += rs->last_counters[24 + i]; out16[9] += rs->last_counters[28 + i]; } }   // grams past the recheck map, flag words, (gram, entry) pairs
+  if (!(rs->dev.debug_flags & 2u)) { out16[7] = rs->last_counters[kCtrPastRecheck]; out16[8] = out16[9] = 0; for (int i = 0; i < 4; i++) { out16[8] += rs->last_counters[kCtrFlagWords + i]; out16[9] += rs->last_counters[kCtrPairs + i]; } }   // grams past the recheck map, flag words, (gram, entry) pairs
   return CG_OK;
 }
 
@@ -695,7 +746,6 @@ int cg_ruleset_get_info(const cg_ruleset* rs, cg_ruleset_info* o) {
 int cg_scan_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint64_t* out_words,
                   cg_hit* out_hits, uint32_t hits_cap, uint32_t* out_nhits) {
   std::lock_guard<std::mutex> lk(g_mu);
-  HostScan hs;
   int rc;
   // large words-only batches: chunked, copies overlapped with the kernels (the hit list needs the per-batch slot tables)
   static const bool no_chunks = getenv("CG_NO_CHUNKS") && atoi(getenv("CG_NO_CHUNKS"));
@@ -708,29 +758,29 @@ int cg_scan_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets,
     }
     // rc == 1: a queue overflowed in some piece; capacities have been raised -- run the batch in one piece below
   }
+  // the hit list on the device (as cg_scan_hits_batch_device builds it): counts and their scan behind the step, the total to
+  // the host, then the first min(total, hits_cap) pairs into a staging buffer and back
   const bool want_hits = out_hits || out_nhits;
-  rc = scan_host(rs, bytes, offsets, n, false, &hs, want_hits);
-  if (rc) return rc;
   cudaStream_t st = G.stream;
-  if (out_words && n) CU(cudaMemcpyAsync(out_words, G.d_words, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
-  // the hit list on the device (as cg_scan_hits_batch_device builds it): counts and their scan, the total to the host, then
-  // the first min(total, hits_cap) pairs into a staging buffer and back
   uint64_t total = 0;
-  if (want_hits && n) {
-    count_launches(launch_hit_count(rs->work, G.d_words, n, G.sm_count, st));
+  rc = scan_host(rs, bytes, offsets, n, want_hits ? kStepPolicy : kStepWords, [&](const ScanWork& w) {
+    if (!want_hits || !n) return CG_OK;
+    count_launches(launch_hit_count(w, G.d_words, n, G.sm_count, st));
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(&total, rs->work.out_off + n, 8, cudaMemcpyDeviceToHost, st));
-  }
-  CU(cudaStreamSynchronize(st));
-  if (total >> 32) { if (out_nhits) *out_nhits = 0xffffffffu; return fail(CG_ERR_TOO_LARGE, "2^32 hits or more in one batch"); }
-  const uint32_t nh = (uint32_t)total, k = out_hits ? std::min(nh, hits_cap) : 0u;
+    CU(cudaMemcpyAsync(&total, w.out_off + n, 8, cudaMemcpyDeviceToHost, st));
+    return CG_OK;
+  });
+  if (rc) return rc;
+  const uint32_t nh = (uint32_t)total, k = out_hits && !(total >> 32) ? std::min(nh, hits_cap) : 0u;
+  if (out_words && n) CU(cudaMemcpyAsync(out_words, G.d_words, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
   if (k) {
     if ((rc = grow(&G.d_hits, &G.cap_hits, 2 * (size_t)k + 1))) return rc;      // [count][pairs]
     count_launches(launch_hit_emit(rs->dev, rs->work, n, G.d_hits + 1, k, G.d_hits, G.sm_count, st));
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(out_hits, G.d_hits + 1, (size_t)k * sizeof(cg_hit), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
   }
+  CU(cudaStreamSynchronize(st));
+  if (total >> 32) { if (out_nhits) *out_nhits = 0xffffffffu; return fail(CG_ERR_TOO_LARGE, "2^32 hits or more in one batch"); }
   if (out_nhits) *out_nhits = nh;
   G.stats.hits += nh;
   if (out_hits && nh > hits_cap) return fail(CG_ERR_CAPACITY, "out_hits too small");
@@ -746,25 +796,25 @@ int scan_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* 
   cudaStream_t st = G.stream;
   int rc;
   if ((rc = one_staging(o, false))) return rc;
-  if ((rc = prepare_step(rs, 1, false, st))) return rc;
+  if ((rc = prepare_step(rs, 1, kStepWords, st))) return rc;
   const uint8_t* d_bytes = o.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(o.d_buf);
   uint32_t* d_out = reinterpret_cast<uint32_t*>(o.d_buf + kOneIn); uint64_t* d_word = reinterpret_cast<uint64_t*>(o.d_buf + kOneIn + kOneOut - 8);   // (the word lands behind the hit row, then is packed to the front)
   if ((rc = one_graph(rs, kOneScan, [&] {
-        const int r = run_scan_device(rs, d_bytes, d_off, 1, d_word, false, st);
+        const int r = run_scan_device(rs, d_bytes, d_off, 1, d_word, kStepWords, st);
         if (r == CG_OK) count_launches(launch_pack_one(rs->dev, rs->work, d_word, d_out, kOneRw - 2, st));
         return r;
       }))) return rc;
   if ((rc = stage_one(o, bytes, len, st))) return rc;
   CU(cudaGraphLaunch(o.g[kOneScan].exec, st));
-  CU(cudaMemcpyAsync(o.h_pin + kOneIn, d_out, (2 + kCounterWords + rs->dev.rw) * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(o.h_pin + kOneIn, d_out, (kOneHitRow + rs->dev.rw) * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   count_launches(o.g[kOneScan].kernels);
   const uint32_t* ho = reinterpret_cast<const uint32_t*>(o.h_pin + kOneIn);
-  const uint32_t* hc = ho + 2;
+  const uint32_t* hc = ho + kOneCounters;
   if ((rc = absorb_counters(rs, hc))) return rc;                 // 1: a queue overflowed, the general path retries with larger scratch
-  G.stats.messages_scanned += 1; G.stats.bytes_scanned += len; G.stats.candidate_events += hc[1]; G.stats.verified_pairs += hc[1];
+  count_step(1, len, hc);
   if (out_word) *out_word = (uint64_t)ho[0] | ((uint64_t)ho[1] << 32);
-  const uint32_t nh = append_hit_row(ho + 2 + kCounterWords, rs->dev.rw, 0, out_rules ? rules_cap : 0, [&](uint32_t i, uint32_t r) { out_rules[i] = r; });
+  const uint32_t nh = append_hit_row(ho + kOneHitRow, rs->dev.rw, 0, out_rules ? rules_cap : 0, [&](uint32_t i, uint32_t r) { out_rules[i] = r; });
   if (out_nrules) *out_nrules = nh;
   G.stats.hits += nh;
   if (out_rules && nh > rules_cap) return fail(CG_ERR_CAPACITY, "out_rules too small");
@@ -785,41 +835,30 @@ int cg_scan_one(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* ou
 }
 
 namespace {
-// findMatches + resolveOverlaps for a host batch: scan_host (with its retries), then the span resolver on the library stream.
-// Resolved spans land in G.d_spans; redacting, G.d_redact_meta holds [sizes, 4 words][out offsets, n + 1][digests, 16-byte
-// aligned, room for every raw span] and *out_offsets the output offsets.  *ns = resolved spans, *need = redacted bytes.
-// Leaves the input in G.d_bytes / G.d_off32.
-int resolve_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, bool redact, uint32_t* out_offsets,
-                 uint32_t* ns, uint64_t* need, uint32_t** d_digests) {
-  HostScan hs;
-  int rc = scan_host(rs, bytes, offsets, n, true, &hs);
-  if (rc) return rc;
-  const ScanWork& w = rs->work;
-  cudaStream_t st = G.stream;
+// the span resolver behind a host-buffer span step, its sizes to the host (sizes[0] resolved spans, or redacting {output
+// bytes, resolved spans}).  Resolved spans land in G.d_spans; redacting, G.d_redact_meta holds [sizes, 4 words][out offsets,
+// n + 1][digests, 16-byte aligned, room for every raw span: *d_digests].
+int resolve_staged(const ScanWork& w, uint32_t n, bool redact, uint64_t sizes[2], uint32_t** d_digests) {
   const size_t dig_at = ((size_t)n + 1 + 4 + 3) & ~(size_t)3;
+  int rc;
   if ((rc = grow(&G.d_spans, &G.cap_spans, (size_t)w.span_cap))) return rc;
   if ((rc = grow(&G.d_redact_meta, &G.cap_redact_meta, dig_at + (redact ? (size_t)w.span_cap * 8 : 0)))) return rc;
-  uint32_t* d_sizes = G.d_redact_meta; uint32_t* d_out_off = G.d_redact_meta + 4;
   *d_digests = G.d_redact_meta + dig_at;
-  const SpanOutputs o{reinterpret_cast<uint32_t*>(G.d_spans), w.span_cap, d_out_off, ~0ull, d_sizes, redact};
-  count_launches(launch_span_resolve(w, G.d_off32, n, o, G.sm_count, st));
+  const SpanOutputs o{reinterpret_cast<uint32_t*>(G.d_spans), w.span_cap, G.d_redact_meta + 4, ~0ull, G.d_redact_meta, redact};
+  count_launches(launch_span_resolve(w, G.d_off32, n, o, G.sm_count, G.stream));
   CU(cudaGetLastError());
-  uint64_t sizes[2] = {0, 0};
-  CU(cudaMemcpyAsync(sizes, d_sizes, redact ? 16 : 4, cudaMemcpyDeviceToHost, st));
-  if (redact) CU(cudaMemcpyAsync(out_offsets, d_out_off, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  *ns = redact ? (uint32_t)sizes[1] : (uint32_t)sizes[0]; *need = redact ? sizes[0] : 0;
-  G.stats.spans += *ns;
+  CU(cudaMemcpyAsync(sizes, G.d_redact_meta, redact ? 16 : 4, cudaMemcpyDeviceToHost, G.stream));
   return CG_OK;
 }
 }  // namespace
 
 int cg_find_matches_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans) {
   std::lock_guard<std::mutex> lk(g_mu);
-  uint32_t outn = 0; uint64_t need = 0; uint32_t* d_dig = nullptr;
-  int rc = resolve_host(rs, bytes, offsets, n, false, nullptr, &outn, &need, &d_dig);
+  uint64_t sizes[2] = {0, 0}; uint32_t* d_dig = nullptr;
+  int rc = scan_host(rs, bytes, offsets, n, kStepSpans, [&](const ScanWork& w) { return resolve_staged(w, n, false, sizes, &d_dig); });
   if (rc) return rc;
-  const uint32_t k = std::min(outn, spans_cap);
+  const uint32_t outn = (uint32_t)sizes[0], k = std::min(outn, spans_cap);
+  G.stats.spans += outn;
   if (out_spans && k) { CU(cudaMemcpyAsync(out_spans, G.d_spans, (size_t)k * sizeof(cg_span), cudaMemcpyDeviceToHost, G.stream)); CU(cudaStreamSynchronize(G.stream)); }
   if (out_nspans) *out_nspans = outn;
   if (out_spans && outn > spans_cap) return fail(CG_ERR_CAPACITY, "out_spans too small");
@@ -848,18 +887,18 @@ int cg_policy_verdict_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t
   std::lock_guard<std::mutex> lk(g_mu);
   if (!rs || !out_verdicts) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (!rs->dev.rule_policy) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy has not been called");
-  HostScan hs;
-  int rc = scan_host(rs, bytes, offsets, n, false, &hs);
-  if (rc) return rc;
-  if (!n) return CG_OK;
-  if ((rc = grow(&G.d_verdicts, &G.cap_verdicts, (size_t)n))) return rc;
-  uint32_t* d_verdicts = G.d_verdicts;
   cudaStream_t st = G.stream;
-  CU(cudaMemsetAsync(d_verdicts, 0, (size_t)n * 4, st));
-  int k = launch_verdicts(rs->dev, rs->work, d_verdicts, n, G.sm_count, st);
-  count_launches(k);
-  CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out_verdicts, d_verdicts, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+  int rc = scan_host(rs, bytes, offsets, n, kStepWords, [&](const ScanWork& w) {
+    if (!n) return CG_OK;
+    int r;
+    if ((r = grow(&G.d_verdicts, &G.cap_verdicts, (size_t)n))) return r;
+    CU(cudaMemsetAsync(G.d_verdicts, 0, (size_t)n * 4, st));  // (verdict_kernel writes the messages that hit)
+    count_launches(launch_verdicts(rs->dev, w, G.d_verdicts, n, G.sm_count, st));
+    CU(cudaGetLastError());
+    return CG_OK;
+  });
+  if (rc || !n) return rc;
+  CU(cudaMemcpyAsync(out_verdicts, G.d_verdicts, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
 }
@@ -868,26 +907,28 @@ int cg_redact_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offset
                     uint64_t* out_need, uint32_t* out_offsets, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans, uint8_t* out_digests32) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!out_offsets || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
-  uint32_t ns = 0; uint64_t pos = 0; uint32_t* d_dig = nullptr;
-  int rc = resolve_host(rs, bytes, offsets, n, true, out_offsets, &ns, &pos, &d_dig);     // input bytes / offsets stay in G.d_bytes / G.d_off32
-  if (rc) return rc;
+  uint64_t sizes[2] = {0, 0}; uint32_t* d_dig = nullptr;
+  int rc = scan_host(rs, bytes, offsets, n, kStepSpans, [&](const ScanWork& w) { return resolve_staged(w, n, true, sizes, &d_dig); });
+  if (rc) return rc;                                        // (input bytes / offsets stay in G.d_bytes / G.d_off32)
+  const uint64_t pos = sizes[0]; const uint32_t ns = (uint32_t)sizes[1];
+  G.stats.spans += ns;
   if (out_need) *out_need = pos;
   if (out_nspans) *out_nspans = ns;
-  if (pos >> 32) return fail(CG_ERR_TOO_LARGE, "redacted batch exceeds 4 GiB");
-  if ((out_spans && ns > spans_cap) || pos > out_cap || !out_bytes) return fail(CG_ERR_CAPACITY, "output buffer too small (see *out_need / *out_nspans)");
+  const bool too_large = pos >> 32, fits = !too_large && !(out_spans && ns > spans_cap) && pos <= out_cap && out_bytes;
   cudaStream_t st = G.stream;
-  if ((rc = grow(&G.d_redact_out, &G.cap_redact_out, (size_t)pos + 64))) return rc;
-  uint8_t* d_out = G.d_redact_out;
-  // device: digests and the splice itself, over the resolver's per-span arrays; it set their counts (counters[21], [22])
-  const ScanWork& w = rs->work;
-  int kl = launch_redact_digests(G.d_bytes, w.sp_start, w.sp_len, w.counters + 21, d_dig, G.sm_count, st);
-  kl += launch_redact_splice(G.d_bytes, G.d_off32, G.d_redact_meta + 4, w.kept_begin, w.sp_start, w.sp_len, w.sp_cat, d_dig, d_out, w.counters + 22, n, G.sm_count, st);
-  count_launches(kl); G.stats.sha256_items += ns;
-  CU(cudaGetLastError());
-  if (pos) CU(cudaMemcpyAsync(out_bytes, d_out, (size_t)pos, cudaMemcpyDeviceToHost, st));
-  if (ns && out_spans) CU(cudaMemcpyAsync(out_spans, G.d_spans, (size_t)ns * sizeof(cg_span), cudaMemcpyDeviceToHost, st));
-  if (ns && out_digests32) CU(cudaMemcpyAsync(out_digests32, d_dig, (size_t)ns * 32, cudaMemcpyDeviceToHost, st));
+  if (fits && (rc = grow(&G.d_redact_out, &G.cap_redact_out, (size_t)pos + 64))) return rc;
+  CU(cudaMemcpyAsync(out_offsets, G.d_redact_meta + 4, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, st));
+  if (fits) {
+    count_launches(enqueue_redact_tail(rs->work, G.d_bytes, G.d_off32, G.d_redact_meta + 4, d_dig, G.d_redact_out, n, st));
+    G.stats.sha256_items += ns;
+    CU(cudaGetLastError());
+    if (pos) CU(cudaMemcpyAsync(out_bytes, G.d_redact_out, (size_t)pos, cudaMemcpyDeviceToHost, st));
+    if (ns && out_spans) CU(cudaMemcpyAsync(out_spans, G.d_spans, (size_t)ns * sizeof(cg_span), cudaMemcpyDeviceToHost, st));
+    if (ns && out_digests32) CU(cudaMemcpyAsync(out_digests32, d_dig, (size_t)ns * 32, cudaMemcpyDeviceToHost, st));
+  }
   CU(cudaStreamSynchronize(st));
+  if (too_large) return fail(CG_ERR_TOO_LARGE, "redacted batch exceeds 4 GiB");
+  if (!fits) return fail(CG_ERR_CAPACITY, "output buffer too small (see *out_need / *out_nspans)");
   return CG_OK;
 }
 
@@ -904,7 +945,7 @@ int span_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, bool redac
   cudaStream_t st = G.stream;
   int rc;
   if ((rc = one_staging(o, true))) return rc;
-  if ((rc = prepare_step(rs, 1, true, st))) return rc;
+  if ((rc = prepare_step(rs, 1, kStepSpans, st))) return rc;
   const ScanWork& w = rs->work;
   const uint8_t* d_bytes = o.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(o.d_buf);
   uint32_t* d_pack = reinterpret_cast<uint32_t*>(o.d_pack);
@@ -912,16 +953,12 @@ int span_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, bool redac
   uint8_t* d_out = o.d_pack + 2 * kOnePack;
   const int m = redact ? kOneRedact : kOneFind;
   if ((rc = one_graph(rs, m, [&] {
-        const int r = run_scan_device(rs, d_bytes, d_off, 1, w.words, true, st);
+        const int r = run_scan_device(rs, d_bytes, d_off, 1, w.words, kStepSpans, st);
         if (r != CG_OK) return r;
         const SpanOutputs so{d_pack + kPackHeader / 4, redact ? kOneSpansRedact : kOneSpansFind, d_pack + kPackOffsets,
                              redact ? (uint64_t)(kOnePack - kPackHeader) : 0ull, d_pack + kPackSizes, redact};
         int k = launch_span_resolve_one(w, d_off, so, st);
-        if (redact) {
-          k += launch_redact_digests(d_bytes, w.sp_start, w.sp_len, w.counters + 21, d_dig, G.sm_count, st);
-          k += launch_redact_splice(d_bytes, d_off, d_pack + kPackOffsets, w.kept_begin, w.sp_start, w.sp_len, w.sp_cat, d_dig, d_out,
-                                    w.counters + 22, 1, G.sm_count, st);
-        }
+        if (redact) k += enqueue_redact_tail(w, d_bytes, d_off, d_pack + kPackOffsets, d_dig, d_out, 1, st);
         k += launch_span_pack_one(w, d_dig, d_out, d_pack, kOnePack, redact, st);
         count_launches(k);
         CU(cudaGetLastError());
@@ -944,7 +981,7 @@ int span_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, bool redac
     CU(cudaMemcpyAsync(h_pack + window, reinterpret_cast<const uint8_t*>(d_pack) + window, packed - window, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
   }
-  G.stats.messages_scanned += 1; G.stats.bytes_scanned += len; G.stats.candidate_events += hc[1]; G.stats.verified_pairs += hc[1];
+  count_step(1, len, hc);
   const uint8_t* body = h_pack + kPackHeader;
   if (!redact) {
     const uint32_t ns = hp[kPackSizes];
@@ -987,40 +1024,12 @@ int cg_redact_one(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint8_t* o
 
 int cg_scan_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_words, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (int rc = require_ready()) return rc;
-  if (!rs || !d_bytes || !d_offsets || !d_out_words) return fail(CG_ERR_INVALID_ARG, "null argument");
-  if ((uintptr_t)d_bytes & 15u) return fail(CG_ERR_INVALID_ARG, "d_bytes must be 16-byte aligned");
+  if (int rc = device_batch_args(rs, d_bytes, d_offsets)) return rc;
+  if (!d_out_words) return fail(CG_ERR_INVALID_ARG, "null argument");
   cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
   if (!n) return CG_OK;
   static const bool use_graph = !(getenv("CG_NO_GRAPH") && atoi(getenv("CG_NO_GRAPH")));
-  int rc;
-  if ((rc = ensure_mirrors(rs))) return rc;
-  // did an earlier batch overflow a queue?  (its result words say "incomplete"; grow the scratch before this one runs)
-  poll_mirrors(rs, false);
-  if ((rc = prepare_step(rs, n, false, st))) return rc;
-  const auto enqueue = [&] { return run_scan_device(rs, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, n, (uint64_t*)d_out_words, false, st); };
-  if (!use_graph || G.profiling) {
-    rc = enqueue();
-  } else {
-    // memsets + scan + resolve + verify + finalize captured once per (arguments, scratch generation, verify grid), then
-    // replayed: one launch per step instead of six, so the host never becomes the bottleneck
-    cg_ruleset::CachedGraph* hit = nullptr;
-    for (auto& g : rs->graphs) if (g.exec && g.bytes == d_bytes && g.off == d_offsets && g.words == d_out_words && g.n == n && g.gen == rs->scratch_gen && g.ctas == rs->verify_ctas) hit = &g;
-    if (!hit) {
-      hit = rs->graphs[0].used <= rs->graphs[1].used ? &rs->graphs[0] : &rs->graphs[1];       // least recently used entry
-      if (hit->exec) { cudaGraphExecDestroy(hit->exec); hit->exec = nullptr; }
-      if ((rc = capture(st, enqueue, &hit->exec, &hit->kernels))) return rc;
-      hit->bytes = d_bytes; hit->off = d_offsets; hit->words = d_out_words; hit->n = n; hit->gen = rs->scratch_gen; hit->ctas = rs->verify_ctas;
-    }
-    hit->used = ++rs->graph_clock;
-    CU(cudaGraphLaunch(hit->exec, st));
-    count_launches(hit->kernels);
-  }
-  if (rc == CG_OK) {
-    G.stats.messages_scanned += n;
-    rc = mirror_counters(rs, st);
-  }
-  return rc;
+  return scan_device(rs, d_bytes, d_offsets, n, (uint64_t*)d_out_words, kStepWords, st, [](const ScanWork&) { return 0; }, use_graph && !G.profiling);
 }
 
 int cg_scan_join(cg_ruleset* rs, void* stream) {
@@ -1037,86 +1046,63 @@ int cg_scan_join(cg_ruleset* rs, void* stream) {
   return CG_OK;
 }
 
-namespace {
-// findMatches (+ redaction) of a batch in HBM, enqueued on st: the span-mode step, the resolver, digests and splice (redact),
-// then the counter block into the mirror ring.  Never waits for the device except when the scratch must grow.
-int spans_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, const SpanOutputs& o, void* d_out_bytes,
-                 void* d_digests, void* stream) {
-  if (!rs || !d_bytes || !d_offsets || !o.sizes) return fail(CG_ERR_INVALID_ARG, "null argument");
-  if ((uintptr_t)d_bytes & 15u) return fail(CG_ERR_INVALID_ARG, "d_bytes must be 16-byte aligned");
-  cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
-  const uint8_t* bytes = (const uint8_t*)d_bytes; const uint32_t* off = (const uint32_t*)d_offsets;
-  int rc;
-  if ((rc = ensure_mirrors(rs))) return rc;
-  poll_mirrors(rs, false);                                  // (an earlier batch overflowed?  grow before this one runs)
-  if ((rc = prepare_step(rs, n, true, st))) return rc;
-  const ScanWork& w = rs->work;
-  if (n) { if ((rc = run_scan_device(rs, bytes, off, n, w.words, true, st))) return rc; }
-  else CU(cudaMemsetAsync(w.counters, 0, kCounterWords * sizeof(uint32_t), st));
-  int k = launch_span_resolve(w, off, n, o, G.sm_count, st);
-  if (o.redact) {
-    k += launch_redact_digests(bytes, w.sp_start, w.sp_len, w.counters + 21, (uint32_t*)d_digests, G.sm_count, st);
-    k += launch_redact_splice(bytes, off, o.out_offsets, w.kept_begin, w.sp_start, w.sp_len, w.sp_cat, (const uint32_t*)d_digests,
-                              (uint8_t*)d_out_bytes, w.counters + 22, n, G.sm_count, st);
-  }
-  count_launches(k);
-  CU(cudaGetLastError());
-  G.stats.messages_scanned += n;
-  return mirror_counters(rs, st);
-}
-}  // namespace
-
 int cg_find_matches_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_spans, uint32_t spans_cap,
                                  void* d_out_nspans, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (int rc = require_ready()) return rc;
-  if (spans_cap && !d_out_spans) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (int rc = device_batch_args(rs, d_bytes, d_offsets)) return rc;
+  if ((spans_cap && !d_out_spans) || !d_out_nspans) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (((uintptr_t)d_offsets | (uintptr_t)d_out_spans | (uintptr_t)d_out_nspans) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets, d_out_spans and d_out_nspans must be 4-byte aligned");
+  cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
   const SpanOutputs o{(uint32_t*)d_out_spans, d_out_spans ? spans_cap : 0u, nullptr, 0, d_out_nspans, false};
-  return spans_device(rs, d_bytes, d_offsets, n, o, nullptr, nullptr, stream);
+  return scan_device(rs, d_bytes, d_offsets, n, nullptr, kStepSpans, st, [&](const ScanWork& w) {
+    return launch_span_resolve(w, (const uint32_t*)d_offsets, n, o, G.sm_count, st);
+  });
 }
 
 int cg_redact_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_bytes, uint64_t out_cap,
                            void* d_out_offsets, void* d_out_spans, uint32_t spans_cap, void* d_out_digests32, void* d_out_sizes, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (int rc = require_ready()) return rc;
-  if (!d_out_offsets || (out_cap && !d_out_bytes) || (spans_cap && (!d_out_spans || !d_out_digests32))) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (int rc = device_batch_args(rs, d_bytes, d_offsets)) return rc;
+  if (!d_out_offsets || !d_out_sizes || (out_cap && !d_out_bytes) || (spans_cap && (!d_out_spans || !d_out_digests32))) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (((uintptr_t)d_offsets | (uintptr_t)d_out_offsets | (uintptr_t)d_out_spans) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets, d_out_offsets and d_out_spans must be 4-byte aligned");
   if ((uintptr_t)d_out_sizes & 7u) return fail(CG_ERR_INVALID_ARG, "d_out_sizes must be 8-byte aligned");
   if ((uintptr_t)d_out_digests32 & 15u) return fail(CG_ERR_INVALID_ARG, "d_out_digests32 must be 16-byte aligned");
+  cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
   const SpanOutputs o{(uint32_t*)d_out_spans, spans_cap, (uint32_t*)d_out_offsets, d_out_bytes ? out_cap : 0ull, d_out_sizes, true};
-  return spans_device(rs, d_bytes, d_offsets, n, o, d_out_bytes, d_out_digests32, stream);
+  return scan_device(rs, d_bytes, d_offsets, n, nullptr, kStepSpans, st, [&](const ScanWork& w) {
+    const int k = launch_span_resolve(w, (const uint32_t*)d_offsets, n, o, G.sm_count, st);
+    return k + enqueue_redact_tail(w, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, o.out_offsets, (uint32_t*)d_out_digests32,
+                                   (uint8_t*)d_out_bytes, n, st);
+  });
 }
 
 int cg_scan_hits_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_words, void* d_out_hits,
                               uint32_t hits_cap, void* d_out_nhits, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (int rc = require_ready()) return rc;
-  if (!rs || !d_bytes || !d_offsets || !d_out_words || !d_out_nhits || (hits_cap && !d_out_hits)) return fail(CG_ERR_INVALID_ARG, "null argument");
-  if ((uintptr_t)d_bytes & 15u) return fail(CG_ERR_INVALID_ARG, "d_bytes must be 16-byte aligned");
+  if (int rc = device_batch_args(rs, d_bytes, d_offsets)) return rc;
+  if (!d_out_words || !d_out_nhits || (hits_cap && !d_out_hits)) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (((uintptr_t)d_offsets | (uintptr_t)d_out_hits | (uintptr_t)d_out_nhits) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets, d_out_hits and d_out_nhits must be 4-byte aligned");
   if ((uintptr_t)d_out_words & 7u) return fail(CG_ERR_INVALID_ARG, "d_out_words must be 8-byte aligned");
   cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
   if (!n) { CU(cudaMemsetAsync(d_out_nhits, 0, 4, st)); return CG_OK; }
   uint64_t* words = (uint64_t*)d_out_words;
-  return policy_device(rs, d_bytes, d_offsets, n, words, st, [&](const ScanWork& w) {
-    return launch_hit_count(w, words, n, G.sm_count, st) +
-           launch_hit_emit(rs->dev, w, n, (uint32_t*)d_out_hits, d_out_hits ? hits_cap : 0u, (uint32_t*)d_out_nhits, G.sm_count, st);
+  return scan_device(rs, d_bytes, d_offsets, n, words, kStepPolicy, st, [&](const ScanWork& w) {
+    const int k = launch_hit_count(w, words, n, G.sm_count, st);
+    return k + launch_hit_emit(rs->dev, w, n, (uint32_t*)d_out_hits, d_out_hits ? hits_cap : 0u, (uint32_t*)d_out_nhits, G.sm_count, st);
   });
 }
 
 int cg_policy_verdict_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_verdicts, void* stream) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (int rc = require_ready()) return rc;
-  if (!rs || !d_bytes || !d_offsets || !d_out_verdicts) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (int rc = device_batch_args(rs, d_bytes, d_offsets)) return rc;
+  if (!d_out_verdicts) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (!rs->dev.rule_policy) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy has not been called");
-  if ((uintptr_t)d_bytes & 15u) return fail(CG_ERR_INVALID_ARG, "d_bytes must be 16-byte aligned");
   if (((uintptr_t)d_offsets | (uintptr_t)d_out_verdicts) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets and d_out_verdicts must be 4-byte aligned");
   cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
   if (!n) return CG_OK;
   uint32_t* verdicts = (uint32_t*)d_out_verdicts;
   CU(cudaMemsetAsync(verdicts, 0, (size_t)n * 4, st));       // (verdict_kernel writes the messages that hit)
-  return policy_device(rs, d_bytes, d_offsets, n, nullptr, st, [&](const ScanWork& w) { return launch_verdicts(rs->dev, w, verdicts, n, G.sm_count, st); });
+  return scan_device(rs, d_bytes, d_offsets, n, nullptr, kStepPolicy, st, [&](const ScanWork& w) { return launch_verdicts(rs->dev, w, verdicts, n, G.sm_count, st); });
 }
 
 // ---------------------------------------------------------------------------------- SHA / Merkle

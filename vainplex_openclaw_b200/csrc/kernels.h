@@ -34,7 +34,7 @@ struct DevRuleset {
   uint32_t n_factors;
   uint32_t max_prog_len;         // longest Pike program of the set (picks the VM capacity)
   uint32_t debug_flags;          // CG_SCAN_DEBUG (experiments only): bit 0 = drop flagged grams (results wrong),
-                                 //   bit 1 = histogram of VM cycles per event in counters[7..15]
+                                 //   bit 1 = histogram of VM cycles per event in the kCtrDebug words
   const uint32_t* factors;       // 12 words per full factor: rule, len | exact<<24, 16 x u16 set ids, max prefix units, prefix-alphabet set id
   const uint32_t* bytesets;      // 8 words per 256-bit byte set
   const uint32_t* always_rules;  // candidates for every message
@@ -56,11 +56,7 @@ struct DevRuleset {
 
 // Per-call scratch in HBM.  A "slot" is one message with at least one confirmed candidate.
 struct ScanWork {
-  uint32_t* counters;            // 32 words: [0]=n_slots [1]=n_events [2]=n_spans [3]=error flags [4]=n_l1 (confirmed factor occurrences) [5]=verify cursor
-                                 //           [6]=flagged grams (level 1a) [7..15]=debug [17]=n_heavy [18]=verify cursor (light events) [19]=grams past the recheck map
-                                 //           [24..27]=flag words queued, [28..31]=(gram, entry) pairs compared, per piece of the batch
-                                 //           span resolution: [16]=status (kResolve*) [20]=resolved spans [21]=digests to compute [22]=messages to splice
-                                 //           hit list: [16]=status (kResolve*) [23]=(msg, rule) hits
+  uint32_t* counters;            // kCounterWords words, indexed by kCtr* (below)
   uint32_t* l1_pos;              // [l1_cap] factor occurrences scan_kernel confirms itself (head check, trigger bytes): buffer offset of the
   uint32_t* l1_fac;              //          factor's first byte, factor id
   uint2* fq;                     // [l1_cap] scan_kernel's flag words: x = the lane's chunk number after the round, y = 4 tiles x 8 (4) probe bits
@@ -70,12 +66,12 @@ struct ScanWork {
   uint32_t* cand;                // [slot_cap * rw]  candidate (msg,rule) pairs already queued
   uint32_t* hit;                 // [slot_cap * rw]  verified pairs
   uint2* events;                 // [event_cap]  (slot, rule | heavy << 31) for the Pike VM
-  uint32_t* heavy_idx;           // [event_cap]  indices of the events expected to run long (counters[17] of them): verified first
+  uint32_t* heavy_idx;           // [event_cap]  indices of the events expected to run long (counters[kCtrHeavy] of them): verified first
   uint32_t* event_pos;           // [event_cap]  policy mode: message offset of the confirmed factor's first byte
   uint32_t* event_pre;           // [event_cap]  policy mode: max units of a match before that factor (0xffff = unbounded)
   uint32_t* spans;               // [span_cap * 6] msg, rule, start_byte, end_byte, start16, end16
   uint32_t l1_cap, msg_cap, slot_cap, event_cap, span_cap;
-  uint32_t q_cap, q_slot;        // this launch's piece of fq (a step scans the batch in up to 4 pieces: q_slot 0..3) and its counter [24 + q_slot]
+  uint32_t q_cap, q_slot;        // this launch's piece of fq (a step scans the batch in up to 4 pieces: q_slot 0..3) and its counter [kCtrFlagWords + q_slot]
   // span resolution (span-mode steps) and hit lists: [res_cap + 1] per message, [span_cap] per raw span
   uint64_t* words;               // [res_cap] result words of span-mode steps and of cg_policy_verdict_batch_device
   uint32_t* seg_cnt;             // raw spans per message (counted down again by the scatter)
@@ -97,9 +93,30 @@ struct ScanWork {
 };
 
 enum : uint32_t { ERR_EVENT_OVERFLOW = 1, ERR_SPAN_OVERFLOW = 2, ERR_VM_STACK = 4, ERR_VM_LIST = 8, ERR_SLOT_OVERFLOW = 16, ERR_L1_OVERFLOW = 32 };
-// span resolution status (counters[16]); kept out of the error flags, which mean "a queue overflowed"
+// span resolution / hit list status (counters[kCtrResolveStatus]); kept out of the error flags, which mean "a queue overflowed"
 enum : uint32_t { kResolveOk = 0, kResolveCapacity = 1, kResolveTooLarge = 2 };
 constexpr uint32_t kCounterWords = 32;
+// The words of a step's counter block (ScanWork::counters), zeroed by reset_kernel.
+enum : uint32_t {
+  kCtrSlots = 0,                 // slots taken: messages with at least one confirmed candidate
+  kCtrEvents = 1,                // (message, rule) pairs queued for the VM
+  kCtrRawSpans = 2,              // raw spans the VM found (span-mode steps)
+  kCtrErrors = 3,                // error flags (ERR_*)
+  kCtrConfirmed = 4,             // factor occurrences scan_kernel / confirm_kernel confirmed (l1_pos / l1_fac)
+  kCtrVerifyHeavy = 5,           // verify cursor over the heavy events
+  kCtrFlagged = 6,               // flagged grams (level 1a)
+  kCtrDebug = 7,                 // [7..15] CG_SCAN_DEBUG bit 1: most VM cycles of an event, then their histogram
+  kCtrResolveStatus = 16,        // span resolver / hit list status (kResolve*)
+  kCtrHeavy = 17,                // events expected to run long (heavy_idx)
+  kCtrVerifyLight = 18,          // verify cursor over the light events
+  kCtrPastRecheck = 19,          // grams past the recheck map
+  kCtrResolved = 20,             // resolved spans
+  kCtrDigests = 21,              // spans to digest (redaction; 0 unless every output fits)
+  kCtrSplice = 22,               // messages to splice (likewise)
+  kCtrHits = 23,                 // (msg, rule) hits of the hit list
+  kCtrFlagWords = 24,            // [24..27] flag words queued, per piece of the batch (q_slot)
+  kCtrPairs = 28,                // [28..31] (gram, entry) pairs compared, per piece
+};
 constexpr uint32_t kScanPartials = 1024;         // blocks an exclusive scan uses at most
 constexpr uint32_t kConfirmTableBudget = 176u * 1024u;     // shared memory confirm_kernel may spend on its tables (beside 32 KB of rings)
 constexpr uint64_t kWordIncomplete = ~0ull;      // result word of every message of a batch whose queues overflowed / whose VM failed
@@ -123,7 +140,7 @@ int launch_verdicts(const DevRuleset& rs, const ScanWork& w, uint32_t* d_verdict
 // the hit list of a finished policy-mode step (w.res_cap >= n): the hit count of every result word into w.out_len and their
 // exclusive scan into w.out_off (w.out_off[n] = the total); then the (msg, rule) pairs sorted by (msg, rule), the first cap
 // of them, as two u32 each into d_out, the total into *d_count (0xffffffff: incomplete step, or 2^32 - 1 hits or more) and
-// counters[23], the status into counters[16] (kResolveCapacity past cap, kResolveTooLarge).  Grids depend on n and the SM
+// counters[kCtrHits], the status into counters[kCtrResolveStatus] (kResolveCapacity past cap, kResolveTooLarge).  Grids depend on n and the SM
 // count only.
 int launch_hit_count(const ScanWork& w, const uint64_t* d_words, uint32_t n, int sm_count, cudaStream_t stream);
 int launch_hit_emit(const DevRuleset& rs, const ScanWork& w, uint32_t n, uint32_t* d_out, uint32_t cap, uint32_t* d_count, int sm_count, cudaStream_t stream);
@@ -131,7 +148,9 @@ int launch_finalize(const DevRuleset& rs, const ScanWork& w, uint64_t* d_words, 
 // start of a step: counters = 0, slot_of_msg = none, candidate / hit rows of the slots the previous step used = 0
 int launch_reset(const DevRuleset& rs, const ScanWork& w, uint32_t n, int sm_count, cudaStream_t stream);
 
-// single-message path: result word, counters and the message's hit row packed into one block (one D2H copy)
+// single-message path: result word, counters and the message's hit row packed into one block (one D2H copy) as u32 words:
+//   [0..1] result word  [kOneCounters..] counter block  [kOneHitRow..] hit row (rw_cap words at most)
+constexpr uint32_t kOneCounters = 2, kOneHitRow = kOneCounters + kCounterWords;
 int launch_pack_one(const DevRuleset& rs, const ScanWork& w, const uint64_t* d_word, uint32_t* d_out, uint32_t rw_cap, cudaStream_t stream);
 
 // raises the dynamic shared-memory limits of every kernel once (not legal inside stream capture)
@@ -142,7 +161,7 @@ int launch_exclusive_scan(const uint32_t* d_in, uint32_t* d_out, uint32_t count,
 int launch_exclusive_scan(const uint64_t* d_in, uint64_t* d_out, uint32_t count, uint64_t* d_part, int sm_count, cudaStream_t stream);
 // where resolved spans go (device pointers).  spans: 6 words per span, the first spans_cap written; redact: out_offsets[n+1],
 // and sizes = u64[2] {output bytes needed, resolved spans}, else sizes = u32[1] resolved spans; sizes are ~0 when the step
-// is incomplete (a queue overflowed or the VM failed).  The status goes to counters[16]: kResolveTooLarge (redact, 4 GiB or
+// is incomplete (a queue overflowed or the VM failed).  The status goes to counters[kCtrResolveStatus]: kResolveTooLarge (redact, 4 GiB or
 // more), kResolveCapacity (more spans than spans_cap, or more bytes than out_cap).
 struct SpanOutputs {
   uint32_t* spans; uint32_t spans_cap;
@@ -151,7 +170,7 @@ struct SpanOutputs {
   bool redact;
 };
 // resolveOverlaps of a span-mode step over n messages (d_off as scanned): a fixed number of kernels for given n and mode,
-// whatever the span count.  Redact also leaves the splice's input in w.sp_* / w.kept_begin and sets counters[21] / [22] to the
+// whatever the span count.  Redact also leaves the splice's input in w.sp_* / w.kept_begin and sets counters[kCtrDigests] / [kCtrSplice] to the
 // spans to digest / messages to splice (0 unless every output fits).
 int launch_span_resolve(const ScanWork& w, const uint32_t* d_off, uint32_t n, const SpanOutputs& o, int sm_count, cudaStream_t stream);
 // the same for a batch of one message in one block (one launch, any raw span count up to w.span_cap)

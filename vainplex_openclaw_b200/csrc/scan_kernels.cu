@@ -82,8 +82,8 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t saddr) { uint32_t v; asm vo
 struct QueueEmit {
   const ScanWork& w;
   __device__ __forceinline__ void operator()(uint32_t t0, uint32_t f) {
-    const uint32_t k = atomicAdd(&w.counters[4], 1u);
-    if (k < w.l1_cap) { w.l1_pos[k] = t0; w.l1_fac[k] = f; } else atomicOr(&w.counters[3], ERR_L1_OVERFLOW);
+    const uint32_t k = atomicAdd(&w.counters[kCtrConfirmed], 1u);
+    if (k < w.l1_cap) { w.l1_pos[k] = t0; w.l1_fac[k] = f; } else atomicOr(&w.counters[kCtrErrors], ERR_L1_OVERFLOW);
   }
 };
 
@@ -257,12 +257,12 @@ scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanW
   uint32_t h1 = 0, t1 = 0;       // the ring holds [h1, t1)
   auto append32 = [&](uint32_t k) {                         // k <= 32 entries from the ring -> the queue
     uint32_t base = 0;
-    if (lane == 0) base = atomicAdd(&w.counters[24 + w.q_slot], k);
+    if (lane == 0) base = atomicAdd(&w.counters[kCtrFlagWords + w.q_slot], k);
     base = __shfl_sync(FULL, base, 0);
     if (lane < k) {
       uint32_t cw, aw;
       asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(cw), "=r"(aw) : "r"(ring1 + (((h1 + lane) & (kRing - 1)) << 3)));
-      if (base + lane < w.q_cap) w.fq[base + lane] = make_uint2(cw, aw); else atomicOr(&w.counters[3], ERR_L1_OVERFLOW);
+      if (base + lane < w.q_cap) w.fq[base + lane] = make_uint2(cw, aw); else atomicOr(&w.counters[kCtrErrors], ERR_L1_OVERFLOW);
     }
     h1 += k;
   };
@@ -297,8 +297,8 @@ struct SlotSink {
     if (slot != 0xffffffffu) return slot < w.slot_cap;
     uint32_t s = *reinterpret_cast<volatile uint32_t*>(&w.slot_of_msg[msg]);
     if (s == 0xffffffffu) {
-      uint32_t mine = atomicAdd(&w.counters[0], 1u);
-      if (mine >= w.slot_cap) { atomicOr(&w.counters[3], ERR_SLOT_OVERFLOW); slot = mine; return false; }
+      uint32_t mine = atomicAdd(&w.counters[kCtrSlots], 1u);
+      if (mine >= w.slot_cap) { atomicOr(&w.counters[kCtrErrors], ERR_SLOT_OVERFLOW); slot = mine; return false; }
       w.slot_msg[mine] = msg;                            // (the slot's candidate / hit rows are zero already: reset_kernel; no fence on this path)
       uint32_t old = atomicCAS(&w.slot_of_msg[msg], 0xffffffffu, mine);
       if (old == 0xffffffffu) s = mine; else { s = old; w.slot_msg[mine] = 0xffffffffu; }   // lost the race: slot stays unused
@@ -325,14 +325,14 @@ struct SlotSink {
     uint32_t bit = 1u << (r & 31);
     uint32_t old = atomicOr(&w.cand[(size_t)slot * rs.rw + (r >> 5)], bit);
     if (want_spans && (old & bit)) return;
-    uint32_t e = atomicAdd(&w.counters[1], 1u);
+    uint32_t e = atomicAdd(&w.counters[kCtrEvents], 1u);
     if (e < w.event_cap) {
       // a long stretch of pattern before the factor (or an unbounded one) means many start positions for the VM: such
       // runs are an order of magnitude longer than the rest and are handed out first, so that none of them starts last
       const bool heavy = !want_spans && (pre & 0xffffu) >= 24u;
       w.events[e] = make_uint2(slot, r | (heavy ? 0x80000000u : 0u)); w.event_pos[e] = t0; w.event_pre[e] = pre;
-      if (heavy) w.heavy_idx[atomicAdd(&w.counters[17], 1u)] = e;
-    } else atomicOr(&w.counters[3], ERR_EVENT_OVERFLOW);
+      if (heavy) w.heavy_idx[atomicAdd(&w.counters[kCtrHeavy], 1u)] = e;
+    } else atomicOr(&w.counters[kCtrErrors], ERR_EVENT_OVERFLOW);
   }
   // rules without factors: one whole-message run (event_pos = 0xffffffff)
   __device__ void candidate_always(uint32_t r) {
@@ -340,8 +340,8 @@ struct SlotSink {
     uint32_t bit = 1u << (r & 31);
     uint32_t old = atomicOr(&w.cand[(size_t)slot * rs.rw + (r >> 5)], bit);
     if (old & bit) return;
-    uint32_t e = atomicAdd(&w.counters[1], 1u);
-    if (e < w.event_cap) { w.events[e] = make_uint2(slot, r); w.event_pos[e] = 0xffffffffu; } else atomicOr(&w.counters[3], ERR_EVENT_OVERFLOW);
+    uint32_t e = atomicAdd(&w.counters[kCtrEvents], 1u);
+    if (e < w.event_cap) { w.events[e] = make_uint2(slot, r); w.event_pos[e] = 0xffffffffu; } else atomicOr(&w.counters[kCtrErrors], ERR_EVENT_OVERFLOW);
   }
   // a confirmed exact factor already proves RegExp.test(message) for this rule
   __device__ void direct(uint32_t r) {
@@ -431,8 +431,8 @@ __device__ __forceinline__ void confirm_pairs(ConfirmCtx& c, uint2 pr, bool acti
     ok = bits != 0;
   }
   if (ok) {
-    const uint32_t k = atomicAdd(&c.w.counters[4], 1u);
-    if (k < c.w.l1_cap) { c.w.l1_pos[k] = (uint32_t)t0; c.w.l1_fac[k] = f; } else atomicOr(&c.w.counters[3], ERR_L1_OVERFLOW);
+    const uint32_t k = atomicAdd(&c.w.counters[kCtrConfirmed], 1u);
+    if (k < c.w.l1_cap) { c.w.l1_pos[k] = (uint32_t)t0; c.w.l1_fac[k] = f; } else atomicOr(&c.w.counters[kCtrErrors], ERR_L1_OVERFLOW);
   }
 }
 
@@ -487,7 +487,7 @@ __global__ void __launch_bounds__(kCfThreads, 1)
 confirm_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, uint32_t cstep) {
   extern __shared__ __align__(16) uint8_t cf_smem[];          // [pair rings][gram rings][tables, when resident]
   const uint32_t kbits = rs.stride == 2 ? 8u : 4u, kshift = rs.stride == 2 ? 1u : 2u;
-  const uint32_t nq = (rs.debug_flags & 1u) ? 0u : min(w.counters[24 + w.q_slot], w.q_cap);
+  const uint32_t nq = (rs.debug_flags & 1u) ? 0u : min(w.counters[kCtrFlagWords + w.q_slot], w.q_cap);
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5, FULL = 0xffffffffu, lt = (1u << lane) - 1u;
   uint2* pring = reinterpret_cast<uint2*>(cf_smem) + warp * kCfRing;
   uint32_t* ring = reinterpret_cast<uint32_t*>(cf_smem + (size_t)wpb * kCfRing * 8) + warp * kCfRing;
@@ -524,12 +524,12 @@ confirm_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ Sc
   if (tail != head) { const bool a = lane < tail - head; const uint32_t pos = a ? ring[(head + lane) & (kCfRing - 1)] : 0u; __syncwarp(); confirm_gram(c, pos, a); }
   if (c.ptail != c.phead) { const bool a = lane < c.ptail - c.phead; const uint2 pr = a ? c.pring[(c.phead + lane) & (kCfRing - 1)] : make_uint2(0u, 0u); confirm_pairs(c, pr, a); }
   const uint32_t passed = __reduce_add_sync(FULL, c.passed);
-  if (lane == 0) { if (flagged) atomicAdd(&w.counters[6], flagged); if (passed) atomicAdd(&w.counters[19], passed); if (c.ptail) atomicAdd(&w.counters[28 + w.q_slot], c.ptail); }
+  if (lane == 0) { if (flagged) atomicAdd(&w.counters[kCtrFlagged], flagged); if (passed) atomicAdd(&w.counters[kCtrPastRecheck], passed); if (c.ptail) atomicAdd(&w.counters[kCtrPairs + w.q_slot], c.ptail); }
 }
 
 __global__ void __launch_bounds__(256, 4)
 resolve_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, int want_spans, uint32_t spread) {
-  const uint32_t n1 = min(w.counters[4], w.l1_cap);
+  const uint32_t n1 = min(w.counters[kCtrConfirmed], w.l1_cap);
   const uint32_t stride = gridDim.x * blockDim.x, tid = blockIdx.x * blockDim.x + threadIdx.x;
   // Occurrences take different paths of very different lengths (direct hit, island matcher of 5 .. 96 steps, slot allocation),
   // and a warp executes the union of its lanes' paths one dependent instruction after the other: with 32 occurrences per warp
@@ -562,9 +562,9 @@ struct GlobalSpanSink {
   const ScanWork& w; uint32_t msg, rule; bool lane0_only;
   __device__ void span(uint32_t sb, uint32_t eb, uint32_t s16, uint32_t e16) {
     if (lane0_only && (threadIdx.x & 31u)) return;         // warp-redundant runs (verify_small_kernel): one lane reports
-    uint32_t k = atomicAdd(&w.counters[2], 1u);
+    uint32_t k = atomicAdd(&w.counters[kCtrRawSpans], 1u);
     if (k < w.span_cap) { uint32_t* o = w.spans + (size_t)k * 6; o[0] = msg; o[1] = rule; o[2] = sb; o[3] = eb; o[4] = s16; o[5] = e16; }
-    else atomicOr(&w.counters[3], ERR_SPAN_OVERFLOW);
+    else atomicOr(&w.counters[kCtrErrors], ERR_SPAN_OVERFLOW);
   }
 };
 
@@ -589,7 +589,7 @@ template <bool SPANS>
 __global__ void __launch_bounds__(kVerifyBlock, kVerifyCtasPerSm)
 verify_small_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off) {
   extern __shared__ __align__(16) uint8_t vsm[];
-  const uint32_t n_events = min(w.counters[1], w.event_cap);
+  const uint32_t n_events = min(w.counters[kCtrEvents], w.event_cap);
   if (n_events == 0) return;                    // (the island matcher decided everything: the common case)
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   // One run per warp.  All 32 lanes execute it redundantly -- identical registers, uniform control flow, the VM
@@ -605,11 +605,11 @@ verify_small_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes
   VMS<SmemStore> vm(rs, st);
   // events are handed out one at a time (their cost varies by two orders of magnitude): a static split leaves most
   // warps idle while a few finish their second or third long run
-  const uint32_t n_heavy = min(w.counters[17], n_events);
+  const uint32_t n_heavy = min(w.counters[kCtrHeavy], n_events);
   bool heavy_phase = true;
   for (;;) {
     uint32_t e = 0;
-    if (lane == 0) e = atomicAdd(&w.counters[heavy_phase ? 5 : 18], 1u);
+    if (lane == 0) e = atomicAdd(&w.counters[heavy_phase ? kCtrVerifyHeavy : kCtrVerifyLight], 1u);
     e = __shfl_sync(0xffffffffu, e, 0);
     if (heavy_phase) {
       if (e >= n_heavy) { heavy_phase = false; continue; }
@@ -636,21 +636,21 @@ verify_small_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes
     else any = test_at_factor(vm, rs, rule, m, len, t0, w.event_pre[e]);
     __syncwarp();
     if (any && lane == 0) atomicOr(&w.hit[(size_t)slot * rs.rw + (rule >> 5)], 1u << (rule & 31));
-    if ((rs.debug_flags & 2u) && lane == 0) {       // CG_SCAN_DEBUG=2: histogram of VM cycles per event in counters[8..15] (<2^11, <2^12, ... >=2^17), max in [7]
+    if ((rs.debug_flags & 2u) && lane == 0) {       // CG_SCAN_DEBUG=2: histogram of VM cycles per event behind counters[kCtrDebug] (<2^11, <2^12, ... >=2^17), the max in it
       const uint32_t cyc = (uint32_t)(clock64() - tc0);
       int bkt = 31 - __clz(cyc | 1u) - 10; bkt = bkt < 0 ? 0 : bkt > 7 ? 7 : bkt;
-      atomicAdd(&w.counters[8 + bkt], 1u); atomicMax(&w.counters[7], cyc);
+      atomicAdd(&w.counters[kCtrDebug + 1 + bkt], 1u); atomicMax(&w.counters[kCtrDebug], cyc);
     }
     __syncwarp();                                          // lane 0 reported; everyone together again before the next run touches shared memory
   }
-  if (vm.err && lane == 0) atomicOr(&w.counters[3], vm.err);
+  if (vm.err && lane == 0) atomicOr(&w.counters[kCtrErrors], vm.err);
 }
 
 // programs longer than kSmallProg: per-thread local arrays
 template <bool SPANS>
 __global__ void __launch_bounds__(kVerifyThreads)
 verify_large_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off) {
-  const uint32_t n_events = min(w.counters[1], w.event_cap);
+  const uint32_t n_events = min(w.counters[kCtrEvents], w.event_cap);
   VMT<kMaxProgLen> vm(rs);
   for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < n_events; e += gridDim.x * blockDim.x) {
     uint2 ev = w.events[e];
@@ -668,7 +668,7 @@ verify_large_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes
     }
     if (any) atomicOr(&w.hit[(size_t)slot * rs.rw + (rule >> 5)], 1u << (rule & 31));
   }
-  if (vm.err) atomicOr(&w.counters[3], vm.err);
+  if (vm.err) atomicOr(&w.counters[kCtrErrors], vm.err);
 }
 
 // Start of a step.  The candidate / hit rows of a slot must be zero when a message takes it; clearing them there cost every
@@ -683,14 +683,14 @@ __global__ void reset_kernel(DevRuleset rs, ScanWork w, uint32_t n) {
 }
 
 __global__ void finalize_kernel(DevRuleset rs, ScanWork w, uint64_t* __restrict__ words, uint32_t n) {
-  if (blockIdx.x == 0 && threadIdx.x == 0) w.persist[0] = min(w.counters[0], w.slot_cap);
+  if (blockIdx.x == 0 && threadIdx.x == 0) w.persist[0] = min(w.counters[kCtrSlots], w.slot_cap);
   // A step whose queues overflowed or whose VM ran out of space has incomplete results: every word of the batch says so
   // (in-band, so that a caller of the asynchronous device path cannot mistake them for "no hit").
-  if (w.counters[3]) {
+  if (w.counters[kCtrErrors]) {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) words[i] = kWordIncomplete;
     return;
   }
-  const uint32_t n_slots = min(w.counters[0], w.slot_cap);
+  const uint32_t n_slots = min(w.counters[kCtrSlots], w.slot_cap);
   for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_slots; s += gridDim.x * blockDim.x) {
     const uint32_t msg = w.slot_msg[s];
     if (msg == 0xffffffffu) continue;                    // slot lost an allocation race: unused
@@ -710,11 +710,11 @@ __global__ void finalize_kernel(DevRuleset rs, ScanWork w, uint64_t* __restrict_
 // An incomplete step (a queue overflowed, the VM failed) has no verdicts: every one of the batch is 0xffffffff, which no
 // verdict can be (action 3 does not exist).
 __global__ void verdict_kernel(DevRuleset rs, ScanWork w, uint32_t* __restrict__ verdicts, uint32_t n) {
-  if (w.counters[3]) {
+  if (w.counters[kCtrErrors]) {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) verdicts[i] = 0xffffffffu;
     return;
   }
-  const uint32_t n_slots = min(w.counters[0], w.slot_cap);
+  const uint32_t n_slots = min(w.counters[kCtrSlots], w.slot_cap);
   for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_slots; s += gridDim.x * blockDim.x) {
     const uint32_t msg = w.slot_msg[s];
     if (msg == 0xffffffffu) continue;
@@ -749,17 +749,17 @@ __global__ void __launch_bounds__(256) hit_count_kernel(const uint64_t* __restri
 // scan), then all 32 lanes write each such message's hit row together -- lane k takes row words k, k + 32, ..., and a popc
 // prefix over the lanes places its rules -- so a row of 157 words (5000 rules) costs five wave steps, not one lane's walk.
 // Pairs go to out (two u32 each) below position cap only.  *count = the total (0xffffffff: incomplete step, or 2^32 - 1 hits
-// or more), also counters[23] for cg_stats.hits; counters[16] = kResolveCapacity / kResolveTooLarge past cap / 2^32 - 1.
+// or more), also counters[kCtrHits] for cg_stats.hits; counters[kCtrResolveStatus] = kResolveCapacity / kResolveTooLarge past cap / 2^32 - 1.
 __global__ void __launch_bounds__(256) hit_emit_kernel(DevRuleset rs, ScanWork w, uint32_t n, uint32_t* __restrict__ out, uint32_t cap,
                                                        uint32_t* __restrict__ count) {
-  const bool incomplete = w.counters[3] != 0;
+  const bool incomplete = w.counters[kCtrErrors] != 0;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     const uint64_t total = w.out_off[n];
     if (incomplete) *count = 0xffffffffu;
     else {
       const uint32_t t = total >= 0xffffffffull ? 0xffffffffu : (uint32_t)total;
-      *count = t; w.counters[23] = t;
-      w.counters[16] = total >= 0xffffffffull ? kResolveTooLarge : total > cap ? kResolveCapacity : kResolveOk;
+      *count = t; w.counters[kCtrHits] = t;
+      w.counters[kCtrResolveStatus] = total >= 0xffffffffull ? kResolveTooLarge : total > cap ? kResolveCapacity : kResolveOk;
     }
   }
   if (incomplete) return;
@@ -869,13 +869,13 @@ int launch_hit_emit(const DevRuleset& rs, const ScanWork& w, uint32_t n, uint32_
   return 1;
 }
 
-// cg_scan_one: out = [word lo, word hi][counters x 32][hit row of the message, rw words]
+// cg_scan_one: out = [word lo, word hi][counter block][hit row of the message, rw words] (kernels.h: kOneCounters, kOneHitRow)
 __global__ void pack_one_kernel(DevRuleset rs, ScanWork w, const uint64_t* __restrict__ word, uint32_t* __restrict__ out, uint32_t rw_cap) {
   const uint32_t t = threadIdx.x;
   if (t == 0) { out[0] = (uint32_t)word[0]; out[1] = (uint32_t)(word[0] >> 32); }
-  if (t < kCounterWords) out[2 + t] = w.counters[t];
+  if (t < kCounterWords) out[kOneCounters + t] = w.counters[t];
   const uint32_t s = w.slot_of_msg[0];
-  for (uint32_t k = t; k < rs.rw && k < rw_cap; k += blockDim.x) out[2 + kCounterWords + k] = (s != 0xffffffffu && s < w.slot_cap) ? w.hit[(size_t)s * rs.rw + k] : 0u;
+  for (uint32_t k = t; k < rs.rw && k < rw_cap; k += blockDim.x) out[kOneHitRow + k] = (s != 0xffffffffu && s < w.slot_cap) ? w.hit[(size_t)s * rs.rw + k] : 0u;
 }
 int launch_pack_one(const DevRuleset& rs, const ScanWork& w, const uint64_t* d_word, uint32_t* d_out, uint32_t rw_cap, cudaStream_t stream) {
   pack_one_kernel<<<1, 64, 0, stream>>>(rs, w, d_word, d_out, rw_cap);

@@ -195,13 +195,13 @@ __device__ uint32_t sort_keep_segment(const ScanWork& w, const uint32_t* __restr
 
 // ---------------------------------------------------------------------------------------------- kernels
 __global__ void __launch_bounds__(256) span_count_kernel(ScanWork w) {
-  const uint32_t ns = min(w.counters[2], w.span_cap);
+  const uint32_t ns = min(w.counters[kCtrRawSpans], w.span_cap);
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < ns; i += gridDim.x * blockDim.x) atomicAdd(&w.seg_cnt[w.spans[(size_t)i * 6]], 1u);
 }
 
 // raw span -> its message's segment (positions inside a segment in arbitrary order: the sort fixes them)
 __global__ void __launch_bounds__(256) span_scatter_kernel(ScanWork w, const uint32_t* __restrict__ rank) {
-  const uint32_t ns = min(w.counters[2], w.span_cap);
+  const uint32_t ns = min(w.counters[kCtrRawSpans], w.span_cap);
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < ns; i += gridDim.x * blockDim.x) {
     const uint32_t* s = w.spans + (size_t)i * 6;
     const uint32_t msg = s[0], s16 = s[4], e16 = s[5];
@@ -264,8 +264,8 @@ __global__ void __launch_bounds__(kSortBlock) span_sort_keep_kernel(ScanWork w, 
 __global__ void __launch_bounds__(kSortBlock) span_resolve_one_kernel(ScanWork w, const uint32_t* __restrict__ category,
                                                                       const uint32_t* __restrict__ rank, const uint32_t* __restrict__ off,
                                                                       SpanOutputs o) {
-  const bool incomplete = w.counters[3] != 0;
-  const uint32_t c = incomplete ? 0u : min(w.counters[2], w.span_cap);
+  const bool incomplete = w.counters[kCtrErrors] != 0;
+  const uint32_t c = incomplete ? 0u : min(w.counters[kCtrRawSpans], w.span_cap);
   for (uint32_t i = threadIdx.x; i < c; i += blockDim.x) {
     const uint32_t* s = w.spans + (size_t)i * 6;
     w.sorted[i] = make_uint4(s[4], ~(s[5] - s[4]), rank[s[1]], i);
@@ -297,10 +297,10 @@ __global__ void __launch_bounds__(kSortBlock) span_resolve_one_kernel(ScanWork w
       o.out_offsets[0] = 0; o.out_offsets[1] = (uint32_t)need;
       uint64_t* z = reinterpret_cast<uint64_t*>(o.sizes); z[0] = incomplete ? ~0ull : need; z[1] = incomplete ? ~0ull : total;
     } else *reinterpret_cast<uint32_t*>(o.sizes) = incomplete ? ~0u : total;
-    w.counters[16] = status;
-    w.counters[20] = incomplete ? 0u : total;
-    w.counters[21] = go && o.redact ? total : 0u;
-    w.counters[22] = go && o.redact ? 1u : 0u;
+    w.counters[kCtrResolveStatus] = status;
+    w.counters[kCtrResolved] = incomplete ? 0u : total;
+    w.counters[kCtrDigests] = go && o.redact ? total : 0u;
+    w.counters[kCtrSplice] = go && o.redact ? 1u : 0u;
   }
 }
 
@@ -309,7 +309,7 @@ __global__ void __launch_bounds__(kSortBlock) span_resolve_one_kernel(ScanWork w
 // redacting, the digests and the output bytes behind the spans -- when all of it fits in pack_cap bytes.
 __global__ void __launch_bounds__(512) span_pack_one_kernel(ScanWork w, const uint32_t* __restrict__ digests, const uint8_t* __restrict__ out,
                                                             uint32_t* __restrict__ packed, uint32_t pack_cap, int redact) {
-  const uint32_t flags = w.counters[3], status = w.counters[16];
+  const uint32_t flags = w.counters[kCtrErrors], status = w.counters[kCtrResolveStatus];
   uint32_t ns = 0; uint64_t need = 0;
   if (redact) { const uint64_t* z = reinterpret_cast<const uint64_t*>(packed + kPackSizes); need = z[0]; ns = (uint32_t)z[1]; }
   else ns = packed[kPackSizes];
@@ -328,7 +328,7 @@ __global__ void __launch_bounds__(512) span_pack_one_kernel(ScanWork w, const ui
 // Resolved span r = the (r - kept_begin[m])-th kept key of message m; sizes, status and the output offsets.
 __global__ void __launch_bounds__(256) span_emit_kernel(ScanWork w, const uint32_t* __restrict__ category, const uint32_t* __restrict__ off,
                                                         uint32_t n, SpanOutputs o) {
-  const bool incomplete = w.counters[3] != 0;
+  const bool incomplete = w.counters[kCtrErrors] != 0;
   const uint32_t total = w.kept_begin[n];
   const uint64_t need = o.redact ? w.out_off[n] : 0;
   uint32_t status = kResolveOk;
@@ -354,10 +354,10 @@ __global__ void __launch_bounds__(256) span_emit_kernel(ScanWork w, const uint32
   if (tid == 0) {
     if (o.redact) { uint64_t* z = reinterpret_cast<uint64_t*>(o.sizes); z[0] = incomplete ? ~0ull : need; z[1] = incomplete ? ~0ull : total; }
     else *reinterpret_cast<uint32_t*>(o.sizes) = incomplete ? ~0u : total;
-    w.counters[16] = status;
-    w.counters[20] = incomplete ? 0u : total;
-    w.counters[21] = go && o.redact ? total : 0u;
-    w.counters[22] = go && o.redact ? n : 0u;
+    w.counters[kCtrResolveStatus] = status;
+    w.counters[kCtrResolved] = incomplete ? 0u : total;
+    w.counters[kCtrDigests] = go && o.redact ? total : 0u;
+    w.counters[kCtrSplice] = go && o.redact ? n : 0u;
   }
 }
 
