@@ -219,6 +219,48 @@ CG_API int cg_policy_verdict_batch_device(cg_ruleset *rs, const void *d_bytes, c
  * all ones as well; a redacted batch of 4 GiB or more; a hit list of 2^32 - 1 hits or more). */
 CG_API int cg_scan_join(cg_ruleset *rs, void *stream);
 
+/* ---- per-message views of one rule set.  Which rules a text is tested against depends on where it comes from: the output
+ * of an exempt tool goes through the credential built-ins only (credentialOnlyEngine, src/redaction/hooks.ts:79-81,176-178,
+ * 218-222), and a policy's scope.channels / scope.excludeAgents decide whether it applies to a context
+ * (src/policy-evaluator.ts:18-26).  A view is a subset of the rules of a rule set; each message of a batch carries one view
+ * id.  The result for message m under view v equals what the call without views returns for m on a rule set compiled from
+ * the rules of v alone (same relative order, flags, categories and policy assignment), with rule indices still those of the
+ * whole set: result words count in-view rules only, hit lists hold in-view pairs, resolveOverlaps (registry.ts:288-316) runs
+ * among in-view rules only (an out-of-view rule's longer match displaces nothing), redaction follows from those spans, and a
+ * policy without an in-view rule never matches.  An empty view gives word 0, no hit, no span, the input bytes unchanged and
+ * verdict 0.  cg_stats counts what the filtered step did.
+ *
+ * cg_ruleset_set_views: rows holds n_views x ceil(n_rules / 32) words, bit r of row v set = rule r is in view v.
+ * 1 <= n_views <= 256; a bit at or past n_rules is CG_ERR_INVALID_ARG.  Like cg_ruleset_set_policy it waits for the library's
+ * stream and replaces the rows: device-resident calls already enqueued on the caller's own streams must be joined first. */
+CG_API int cg_ruleset_set_views(cg_ruleset *rs, const uint32_t *rows, uint32_t n_views);
+/* Host-buffer twins: views = one id per message (host memory); otherwise the signature, outputs and statuses of the call
+ * without views.  An id >= n_views, or a call before cg_ruleset_set_views, is CG_ERR_INVALID_ARG before anything is copied
+ * or written.  cg_scan_batch_views runs a large words-only batch as one piece (cg_scan_batch overlaps its copies in chunks). */
+CG_API int cg_scan_batch_views(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, const uint8_t *views, uint32_t n,
+                               uint64_t *out_words, cg_hit *out_hits, uint32_t hits_cap, uint32_t *out_nhits);
+CG_API int cg_find_matches_batch_views(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, const uint8_t *views, uint32_t n,
+                                       cg_span *out_spans, uint32_t spans_cap, uint32_t *out_nspans);
+CG_API int cg_redact_batch_views(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, const uint8_t *views, uint32_t n,
+                                 uint8_t *out_bytes, uint64_t out_cap, uint64_t *out_need, uint32_t *out_offsets,
+                                 cg_span *out_spans, uint32_t spans_cap, uint32_t *out_nspans, uint8_t *out_digests32);
+CG_API int cg_policy_verdict_batch_views(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, const uint8_t *views, uint32_t n,
+                                         uint32_t *out_verdicts);
+/* Device-resident twins: d_views = one uint8 id per message in HBM (advance it with d_offsets for a sub-range); otherwise the
+ * asynchrony, alignment rules, capacities, overflow protocol and cg_scan_join reporting of the call without views.  The host
+ * cannot read the ids: an id >= n_views selects the empty view.  A call before cg_ruleset_set_views, or d_views = NULL, is
+ * CG_ERR_INVALID_ARG before anything is enqueued.  cg_scan_hits_batch_device_views with d_out_hits = NULL, hits_cap = 0 and
+ * d_out_nhits = NULL writes the result words alone (cg_scan_batch_device's output, launched directly, not from a graph). */
+CG_API int cg_scan_hits_batch_device_views(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, const void *d_views, uint32_t n,
+                                           void *d_out_words, void *d_out_hits, uint32_t hits_cap, void *d_out_nhits, void *stream);
+CG_API int cg_find_matches_batch_device_views(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, const void *d_views, uint32_t n,
+                                              void *d_out_spans, uint32_t spans_cap, void *d_out_nspans, void *stream);
+CG_API int cg_redact_batch_device_views(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, const void *d_views, uint32_t n,
+                                        void *d_out_bytes, uint64_t out_cap, void *d_out_offsets,
+                                        void *d_out_spans, uint32_t spans_cap, void *d_out_digests32, void *d_out_sizes, void *stream);
+CG_API int cg_policy_verdict_batch_device_views(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, const void *d_views, uint32_t n,
+                                                void *d_out_verdicts, void *stream);
+
 /* ---- SHA-256.  Replaces createHash("sha256").update(s).digest() at src/util.ts:77-79,
  * src/redaction/vault.ts:26-28 (and nats/src/hooks.ts:90-94) for a batch of n byte strings. */
 CG_API int cg_sha256_batch(const uint8_t *bytes, const uint64_t *offsets, uint32_t n, uint8_t *out_digests32);

@@ -31,6 +31,13 @@ type Addon = {
   redactOne(handle: unknown, bytes: Uint8Array): { bytes: Uint8Array; spans: Uint32Array; digests: Uint8Array };
   setPolicy(handle: unknown, rulePolicy: Uint32Array, ruleAction: Uint8Array): void;
   verdictBatch(handle: unknown, bytes: Uint8Array, offsets: Uint32Array): Uint32Array;
+  // per-message views of one rule set: rows = nViews x ceil(nRules / 32) words (bit r = rule r in the view); views = one id
+  // per message -- an exempt tool's output on the credential view, a context on the view of its in-scope policies
+  setViews(handle: unknown, rows: Uint32Array, nViews: number): void;
+  scanBatchViews(handle: unknown, bytes: Uint8Array, offsets: Uint32Array, views: Uint8Array): { words: BigUint64Array; hits: Uint32Array };
+  findMatchesBatchViews(handle: unknown, bytes: Uint8Array, offsets: Uint32Array, views: Uint8Array): Uint32Array;
+  redactBatchViews(handle: unknown, bytes: Uint8Array, offsets: Uint32Array, views: Uint8Array): { bytes: Uint8Array; offsets: Uint32Array; spans: Uint32Array; digests: Uint8Array };
+  verdictBatchViews(handle: unknown, bytes: Uint8Array, offsets: Uint32Array, views: Uint8Array): Uint32Array;
   sha256Batch(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array;
   merkleRoot(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array;
   logCreate(keepLeafDigests: boolean): unknown;

@@ -22,6 +22,9 @@
  *   findMatchesOne(handle, bytes: Uint8Array): Uint32Array  // one message, blocking: findMatchesBatch's spans for a batch of one
  *   redactOne(handle, bytes: Uint8Array): {bytes, spans, digests}  // one message, blocking: scanString spliced on the device
  *   setPolicy(handle, rulePolicy: Uint32Array, ruleAction: Uint8Array): void ; verdictBatch(handle, bytes, offsets): Uint32Array
+ *   setViews(handle, rows: Uint32Array, nViews: number): void  // nViews rows of ceil(nRules / 32) words, bit r = rule r in the view
+ *   scanBatchViews / findMatchesBatchViews / redactBatchViews / verdictBatchViews(handle, bytes, offsets, views: Uint8Array)
+ *     // the batch calls above with one view id per message: each message decided on its view's rules alone
  *   sha256Batch(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array  // 32 bytes per item
  *   merkleRoot(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array   // 32 bytes
  *   logCreate(keepLeafDigests: boolean): External ; logRestore(size: bigint, frontier: Uint8Array): External
@@ -75,6 +78,16 @@ static int64_t get_batch(napi_env env, napi_value vb, napi_value vo, int wide, u
   }
   return (int64_t)n;
 }
+/* the *Views calls' last argument: one view id per message (Uint8Array of n elements).  0 = thrown. */
+static int get_views(napi_env env, napi_value v, int64_t n, uint8_t **ids) {
+  size_t nv;
+  if (!get_ta(env, v, ids, &nv, napi_uint8_array) || (int64_t)nv != n) { napi_throw_type_error(env, NULL, "views: a Uint8Array with one view id per message"); return 0; }
+  if (!nv) *ids = NULL;
+  return 1;
+}
+/* arguments (handle, bytes, offsets[, views]) of a batch call: 3 + views of them */
+#define BATCH_ARGS(env, info, views) size_t argc = 4; napi_value argv[4]; NAPI_CALL(env, napi_get_cb_info(env, info, &argc, argv, NULL, NULL)); \
+  if (argc < 3u + (size_t)(views)) { napi_throw_type_error(env, NULL, "too few arguments"); return NULL; }
 static napi_value make_u8(napi_env env, const void *src, size_t len) {
   napi_value ab, arr; void *data;
   if (napi_create_arraybuffer(env, len, &data, &ab) != napi_ok) return NULL;
@@ -160,18 +173,22 @@ static napi_value js_create_ruleset(napi_env env, napi_callback_info info) {
   return out;
 }
 
-static napi_value js_scan_batch(napi_env env, napi_callback_info info) {
-  ARGS(env, info, 3)
-  cg_ruleset *rs; uint8_t *bytes, *offp;
+static napi_value scan_batch(napi_env env, napi_callback_info info, int views) {
+  BATCH_ARGS(env, info, views)
+  cg_ruleset *rs; uint8_t *bytes, *offp, *ids = NULL;
   NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
   const int64_t nn = get_batch(env, argv[1], argv[2], 0, &bytes, &offp); if (nn < 0) return NULL;
+  if (views && !get_views(env, argv[3], nn, &ids)) return NULL;
   const uint32_t n = (uint32_t)nn;
+#define SCAN(cap) (views ? cg_scan_batch_views(rs, bytes, (const uint32_t *)offp, ids, n, (uint64_t *)wdata, tmp, (cap), &nh) \
+                         : cg_scan_batch(rs, bytes, (const uint32_t *)offp, n, (uint64_t *)wdata, tmp, (cap), &nh))
   napi_value words_ab, words, hits_ab, hits, out; void *wdata, *hdata;
   NAPI_CALL(env, napi_create_arraybuffer(env, (size_t)n * 8, &wdata, &words_ab));
   NAPI_CALL(env, napi_create_typedarray(env, napi_biguint64_array, n, words_ab, 0, &words));
   uint32_t nh = 0, cap = 1024; cg_hit *tmp = (cg_hit *)malloc(sizeof(cg_hit) * cap);
-  int rc = tmp ? cg_scan_batch(rs, bytes, (const uint32_t *)offp, n, (uint64_t *)wdata, tmp, cap, &nh) : CG_ERR_CUDA;
-  if (rc == CG_ERR_CAPACITY) { cap = nh; cg_hit *t2 = (cg_hit *)realloc(tmp, sizeof(cg_hit) * cap); if (t2) { tmp = t2; rc = cg_scan_batch(rs, bytes, (const uint32_t *)offp, n, (uint64_t *)wdata, tmp, cap, &nh); } }
+  int rc = tmp ? SCAN(cap) : CG_ERR_CUDA;
+  if (rc == CG_ERR_CAPACITY) { cap = nh; cg_hit *t2 = (cg_hit *)realloc(tmp, sizeof(cg_hit) * cap); if (t2) { tmp = t2; rc = SCAN(cap); } }
+#undef SCAN
   if (rc != CG_OK) { free(tmp); napi_throw_error(env, NULL, cg_last_error()); return NULL; }
   if (napi_create_arraybuffer(env, (size_t)nh * 8, &hdata, &hits_ab) != napi_ok) { free(tmp); napi_throw_error(env, NULL, "N-API call failed"); return NULL; }
   memcpy(hdata, tmp, (size_t)nh * 8); free(tmp);
@@ -181,6 +198,8 @@ static napi_value js_scan_batch(napi_env env, napi_callback_info info) {
   NAPI_CALL(env, napi_set_named_property(env, out, "hits", hits));
   return out;
 }
+static napi_value js_scan_batch(napi_env env, napi_callback_info info) { return scan_batch(env, info, 0); }
+static napi_value js_scan_batch_views(napi_env env, napi_callback_info info) { return scan_batch(env, info, 1); }
 
 static napi_value js_scan_one(napi_env env, napi_callback_info info) {
   ARGS(env, info, 2)
@@ -200,20 +219,40 @@ static napi_value js_scan_one(napi_env env, napi_callback_info info) {
   return out;
 }
 
-static napi_value js_find_matches_batch(napi_env env, napi_callback_info info) {
-  ARGS(env, info, 3)
-  cg_ruleset *rs; uint8_t *bytes, *offp;
+static napi_value find_matches_batch(napi_env env, napi_callback_info info, int views) {
+  BATCH_ARGS(env, info, views)
+  cg_ruleset *rs; uint8_t *bytes, *offp, *ids = NULL;
   NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
   const int64_t nn = get_batch(env, argv[1], argv[2], 0, &bytes, &offp); if (nn < 0) return NULL;
+  if (views && !get_views(env, argv[3], nn, &ids)) return NULL;
   uint32_t n = (uint32_t)nn, ns = 0, cap = 256; cg_span *tmp = (cg_span *)malloc(sizeof(cg_span) * cap);
-  int rc = tmp ? cg_find_matches_batch(rs, bytes, (const uint32_t *)offp, n, tmp, cap, &ns) : CG_ERR_CUDA;
-  if (rc == CG_ERR_CAPACITY) { cap = ns; cg_span *t2 = (cg_span *)realloc(tmp, sizeof(cg_span) * cap); if (t2) { tmp = t2; rc = cg_find_matches_batch(rs, bytes, (const uint32_t *)offp, n, tmp, cap, &ns); } }
+#define FIND(cap) (views ? cg_find_matches_batch_views(rs, bytes, (const uint32_t *)offp, ids, n, tmp, (cap), &ns) \
+                         : cg_find_matches_batch(rs, bytes, (const uint32_t *)offp, n, tmp, (cap), &ns))
+  int rc = tmp ? FIND(cap) : CG_ERR_CUDA;
+  if (rc == CG_ERR_CAPACITY) { cap = ns; cg_span *t2 = (cg_span *)realloc(tmp, sizeof(cg_span) * cap); if (t2) { tmp = t2; rc = FIND(cap); } }
+#undef FIND
   if (rc != CG_OK) { free(tmp); napi_throw_error(env, NULL, cg_last_error()); return NULL; }
   napi_value ab, arr; void *data;
   if (napi_create_arraybuffer(env, (size_t)ns * sizeof(cg_span), &data, &ab) != napi_ok) { free(tmp); napi_throw_error(env, NULL, "N-API call failed"); return NULL; }
   memcpy(data, tmp, (size_t)ns * sizeof(cg_span)); free(tmp);
   NAPI_CALL(env, napi_create_typedarray(env, napi_uint32_array, (size_t)ns * 6, ab, 0, &arr));
   return arr;
+}
+static napi_value js_find_matches_batch(napi_env env, napi_callback_info info) { return find_matches_batch(env, info, 0); }
+static napi_value js_find_matches_batch_views(napi_env env, napi_callback_info info) { return find_matches_batch(env, info, 1); }
+
+static napi_value js_set_views(napi_env env, napi_callback_info info) {
+  ARGS(env, info, 3)
+  cg_ruleset *rs; uint8_t *rows; size_t nb; uint32_t nv = 0; cg_ruleset_info ri;
+  NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
+  CG_CALL(env, cg_ruleset_get_info(rs, &ri));
+  /* the library reads nViews rows of exactly ceil(nRules / 32) words (one word for a set without rules) */
+  const size_t row_words = ri.n_rules ? ((size_t)ri.n_rules + 31) / 32 : 1;
+  if (!get_ta(env, argv[1], &rows, &nb, napi_uint32_array) || napi_get_value_uint32(env, argv[2], &nv) != napi_ok || !nv || nb != (size_t)nv * row_words * 4) {
+    napi_throw_type_error(env, NULL, "setViews(handle, rows: Uint32Array of nViews x ceil(nRules / 32) words, nViews)"); return NULL;
+  }
+  CG_CALL(env, cg_ruleset_set_views(rs, (const uint32_t *)rows, nv));
+  return NULL;
 }
 
 static napi_value js_set_policy(napi_env env, napi_callback_info info) {
@@ -224,16 +263,20 @@ static napi_value js_set_policy(napi_env env, napi_callback_info info) {
   CG_CALL(env, cg_ruleset_set_policy(rs, (const uint32_t *)pol, act, (uint32_t)na));
   return NULL;
 }
-static napi_value js_verdict_batch(napi_env env, napi_callback_info info) {
-  ARGS(env, info, 3)
-  cg_ruleset *rs; uint8_t *bytes, *offp; napi_value ab, arr; void *data;
+static napi_value verdict_batch(napi_env env, napi_callback_info info, int views) {
+  BATCH_ARGS(env, info, views)
+  cg_ruleset *rs; uint8_t *bytes, *offp, *ids = NULL; napi_value ab, arr; void *data;
   NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
   const int64_t nn = get_batch(env, argv[1], argv[2], 0, &bytes, &offp); if (nn < 0) return NULL;
+  if (views && !get_views(env, argv[3], nn, &ids)) return NULL;
   NAPI_CALL(env, napi_create_arraybuffer(env, (size_t)nn * 4, &data, &ab));
-  CG_CALL(env, cg_policy_verdict_batch(rs, bytes, (const uint32_t *)offp, (uint32_t)nn, (uint32_t *)data));
+  CG_CALL(env, views ? cg_policy_verdict_batch_views(rs, bytes, (const uint32_t *)offp, ids, (uint32_t)nn, (uint32_t *)data)
+                     : cg_policy_verdict_batch(rs, bytes, (const uint32_t *)offp, (uint32_t)nn, (uint32_t *)data));
   NAPI_CALL(env, napi_create_typedarray(env, napi_uint32_array, (size_t)nn, ab, 0, &arr));
   return arr;
 }
+static napi_value js_verdict_batch(napi_env env, napi_callback_info info) { return verdict_batch(env, info, 0); }
+static napi_value js_verdict_batch_views(napi_env env, napi_callback_info info) { return verdict_batch(env, info, 1); }
 
 static napi_value js_sha256_batch(napi_env env, napi_callback_info info) {
   ARGS(env, info, 2)
@@ -402,11 +445,12 @@ static napi_value js_verify_consistency(napi_env env, napi_callback_info info) {
   return out;
 }
 
-static napi_value js_redact_batch(napi_env env, napi_callback_info info) {
-  ARGS(env, info, 3)
-  cg_ruleset *rs; uint8_t *bytes, *offp;
+static napi_value redact_batch(napi_env env, napi_callback_info info, int views) {
+  BATCH_ARGS(env, info, views)
+  cg_ruleset *rs; uint8_t *bytes, *offp, *ids = NULL;
   NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
   const int64_t nn = get_batch(env, argv[1], argv[2], 0, &bytes, &offp); if (nn < 0) return NULL;
+  if (views && !get_views(env, argv[3], nn, &ids)) return NULL;
   uint32_t n = (uint32_t)nn, ns = 0, cap_spans = 256; uint64_t need = 0, cap_bytes = (uint64_t)((const uint32_t *)offp)[n] + 4096;
   napi_value off_ab, off_arr; void *off_data;
   NAPI_CALL(env, napi_create_arraybuffer(env, (size_t)(n + 1) * 4, &off_data, &off_ab));
@@ -417,7 +461,8 @@ static napi_value js_redact_batch(napi_env env, napi_callback_info info) {
     if (s2) spans = s2;
     if (d2) dig = d2;
     if (!o2 || !s2 || !d2) break;
-    rc = cg_redact_batch(rs, bytes, (const uint32_t *)offp, n, out, cap_bytes, &need, (uint32_t *)off_data, spans, cap_spans, &ns, dig);
+    rc = views ? cg_redact_batch_views(rs, bytes, (const uint32_t *)offp, ids, n, out, cap_bytes, &need, (uint32_t *)off_data, spans, cap_spans, &ns, dig)
+               : cg_redact_batch(rs, bytes, (const uint32_t *)offp, n, out, cap_bytes, &need, (uint32_t *)off_data, spans, cap_spans, &ns, dig);
     if (rc == CG_ERR_CAPACITY && (need > cap_bytes || ns > cap_spans)) { if (need > cap_bytes) cap_bytes = need; if (ns > cap_spans) cap_spans = ns; continue; }
     break;
   }
@@ -431,6 +476,8 @@ static napi_value js_redact_batch(napi_env env, napi_callback_info info) {
   NAPI_CALL(env, napi_set_named_property(env, res, "spans", s_arr)); NAPI_CALL(env, napi_set_named_property(env, res, "digests", d_arr));
   return res;
 }
+static napi_value js_redact_batch(napi_env env, napi_callback_info info) { return redact_batch(env, info, 0); }
+static napi_value js_redact_batch_views(napi_env env, napi_callback_info info) { return redact_batch(env, info, 1); }
 
 /* ---- one message, blocking: the synchronous hooks' findMatches / scanString (cg_find_matches_one / cg_redact_one) */
 static uint8_t one_empty[1];                          /* the message of an empty Uint8Array */
@@ -488,6 +535,8 @@ static napi_value module_init(napi_env env, napi_value exports) {
     FN("findMatchesBatch", js_find_matches_batch), FN("redactBatch", js_redact_batch),
     FN("findMatchesOne", js_find_matches_one), FN("redactOne", js_redact_one),
     FN("setPolicy", js_set_policy), FN("verdictBatch", js_verdict_batch),
+    FN("setViews", js_set_views), FN("scanBatchViews", js_scan_batch_views), FN("findMatchesBatchViews", js_find_matches_batch_views),
+    FN("redactBatchViews", js_redact_batch_views), FN("verdictBatchViews", js_verdict_batch_views),
     FN("sha256Batch", js_sha256_batch), FN("merkleRoot", js_merkle_root),
     FN("logCreate", js_log_create), FN("logRestore", js_log_restore), FN("logAppend", js_log_append), FN("logAppendJsonl", js_log_append_jsonl),
     FN("logReserve", js_log_reserve), FN("logSize", js_log_size), FN("logRoot", js_log_root), FN("logFrontier", js_log_frontier),

@@ -57,7 +57,10 @@ EXPORTS = ["cg_init", "cg_shutdown", "cg_last_error", "cg_version", "cg_device_c
            "cg_scan_one", "cg_find_matches_batch", "cg_find_matches_one", "cg_redact_one", "cg_scan_batch_device", "cg_find_matches_batch_device", "cg_redact_batch_device",
            "cg_scan_hits_batch_device", "cg_policy_verdict_batch_device", "cg_sha256_batch", "cg_merkle_root",
            "cg_merkle_root_fixed", "cg_merkle_block_roots_device", "cg_merkle_fold", "cg_merkle_fold_device",
-           "cg_merkle_log_create_tree", "cg_merkle_log_proofs", "cg_merkle_log_consistency_between", "cg_merkle_verify_proofs"]
+           "cg_merkle_log_create_tree", "cg_merkle_log_proofs", "cg_merkle_log_consistency_between", "cg_merkle_verify_proofs",
+           "cg_ruleset_set_views", "cg_scan_batch_views", "cg_find_matches_batch_views", "cg_redact_batch_views",
+           "cg_policy_verdict_batch_views", "cg_scan_hits_batch_device_views", "cg_find_matches_batch_device_views",
+           "cg_redact_batch_device_views", "cg_policy_verdict_batch_device_views"]
 
 _lib = None
 
@@ -135,6 +138,15 @@ def load():
     L.cg_merkle_log_proofs.argtypes = [vp, vp, u32, u64, vp, u32, vp]; L.cg_merkle_log_proofs.restype = i32
     L.cg_merkle_log_consistency_between.argtypes = [vp, u64, u64, vp, u32, vp]; L.cg_merkle_log_consistency_between.restype = i32
     L.cg_merkle_verify_proofs.argtypes = [vp, vp, vp, u32, u64, vp, u32, vp, vp, vp]; L.cg_merkle_verify_proofs.restype = i32
+    L.cg_ruleset_set_views.argtypes = [vp, vp, u32]; L.cg_ruleset_set_views.restype = i32
+    L.cg_scan_batch_views.argtypes = [vp, vp, vp, vp, u32, vp, vp, u32, C.POINTER(u32)]; L.cg_scan_batch_views.restype = i32
+    L.cg_find_matches_batch_views.argtypes = [vp, vp, vp, vp, u32, vp, u32, C.POINTER(u32)]; L.cg_find_matches_batch_views.restype = i32
+    L.cg_redact_batch_views.argtypes = [vp, vp, vp, vp, u32, vp, u64, vp, vp, vp, u32, vp, vp]; L.cg_redact_batch_views.restype = i32
+    L.cg_policy_verdict_batch_views.argtypes = [vp, vp, vp, vp, u32, vp]; L.cg_policy_verdict_batch_views.restype = i32
+    L.cg_scan_hits_batch_device_views.argtypes = [vp, vp, vp, vp, u32, vp, vp, u32, vp, vp]; L.cg_scan_hits_batch_device_views.restype = i32
+    L.cg_find_matches_batch_device_views.argtypes = [vp, vp, vp, vp, u32, vp, u32, vp, vp]; L.cg_find_matches_batch_device_views.restype = i32
+    L.cg_redact_batch_device_views.argtypes = [vp, vp, vp, vp, u32, vp, u64, vp, vp, u32, vp, vp, vp]; L.cg_redact_batch_device_views.restype = i32
+    L.cg_policy_verdict_batch_device_views.argtypes = [vp, vp, vp, vp, u32, vp, vp]; L.cg_policy_verdict_batch_device_views.restype = i32
     _lib = L
     return L
 
@@ -177,6 +189,26 @@ def pack(messages) -> tuple[np.ndarray, np.ndarray]:
     return data, off
 
 
+def view_rows(views, n_rules: int) -> np.ndarray:
+    """rows for cg_ruleset_set_views from one iterable of rule indices per view: uint32[n_views, ceil(n_rules / 32)], bit r of
+    row v set = rule r is in view v."""
+    views = [np.asarray(sorted(set(int(r) for r in v)), dtype=np.int64) for v in views]
+    rows = np.zeros((len(views), max(1, (n_rules + 31) // 32)), dtype=np.uint32)
+    for v, idx in enumerate(views):
+        if len(idx) and (idx.min() < 0 or idx.max() >= n_rules):
+            raise ValueError("view %d names a rule outside 0 .. %d" % (v, n_rules - 1))
+        np.bitwise_or.at(rows[v], idx >> 5, (np.uint32(1) << (idx & 31).astype(np.uint32)))
+    return rows
+
+
+def _ids(views, n: int) -> np.ndarray:
+    """one uint8 view id per message of a batch of n"""
+    ids = np.ascontiguousarray(views, dtype=np.uint8).reshape(-1)
+    if len(ids) != n:
+        raise ValueError("views: %d ids for a batch of %d messages" % (len(ids), n))
+    return ids
+
+
 class Ruleset:
     """cg_ruleset handle.  rules: iterable of (source:str|bytes, flags:int, category:int)."""
 
@@ -209,16 +241,34 @@ class Ruleset:
         check(load().cg_ruleset_get_info(self.handle, C.byref(o)))
         return o
 
-    def scan_batch(self, data: np.ndarray, off: np.ndarray, want_hits: bool = True):
-        """-> (words[n] uint64, hits structured array sorted by (msg, rule))."""
+    def set_views(self, views):
+        """cg_ruleset_set_views: views = uint32 rows [n_views, ceil(n_rules / 32)] (bit r of row v = rule r in view v), or one
+        iterable of rule indices per view (view_rows)."""
+        if isinstance(views, np.ndarray) and views.dtype == np.uint32 and views.ndim == 2:
+            rows = np.ascontiguousarray(views)
+            rw = max(1, (self.n_rules + 31) // 32)
+            if rows.shape[1] != rw:
+                raise ValueError("view rows must be %d words wide (ceil(n_rules / 32)), not %d" % (rw, rows.shape[1]))
+        else:
+            rows = view_rows(views, self.n_rules)
+        check(load().cg_ruleset_set_views(self.handle, rows.ctypes.data, rows.shape[0]))
+
+    def scan_batch(self, data: np.ndarray, off: np.ndarray, want_hits: bool = True, views=None):
+        """-> (words[n] uint64, hits structured array sorted by (msg, rule)).  views: one view id per message
+        (cg_scan_batch_views)."""
         n = len(off) - 1
         words = np.zeros(max(n, 1), dtype=np.uint64)
         nh = C.c_uint32(0)
         cap = 1024
+        ids = None if views is None else _ids(views, n)
         while True:
             hits = np.zeros(cap, dtype=HIT_DTYPE)
-            rc = load().cg_scan_batch(self.handle, data.ctypes.data, off.ctypes.data, n, words.ctypes.data,
-                                      hits.ctypes.data if want_hits else None, cap, C.byref(nh))
+            if ids is None:
+                rc = load().cg_scan_batch(self.handle, data.ctypes.data, off.ctypes.data, n, words.ctypes.data,
+                                          hits.ctypes.data if want_hits else None, cap, C.byref(nh))
+            else:
+                rc = load().cg_scan_batch_views(self.handle, data.ctypes.data, off.ctypes.data, ids.ctypes.data, n, words.ctypes.data,
+                                                hits.ctypes.data if want_hits else None, cap, C.byref(nh))
             if rc == CG_ERR_CAPACITY and nh.value > cap:
                 cap = nh.value
                 continue
@@ -234,14 +284,20 @@ class Ruleset:
         check(load().cg_scan_one(self.handle, buf.ctypes.data, len(msg), C.byref(word), rules.ctypes.data, len(rules), C.byref(nr)))
         return word.value, [int(x) for x in rules[:nr.value]]
 
-    def find_matches_batch(self, data: np.ndarray, off: np.ndarray):
-        """-> spans structured array, resolved per registry.ts:288-316, sorted by (msg, start)."""
+    def find_matches_batch(self, data: np.ndarray, off: np.ndarray, views=None):
+        """-> spans structured array, resolved per registry.ts:288-316, sorted by (msg, start).  views: one view id per
+        message (cg_find_matches_batch_views)."""
         n = len(off) - 1
         ns = C.c_uint32(0)
         cap = 1024
+        ids = None if views is None else _ids(views, n)
         while True:
             spans = np.zeros(cap, dtype=SPAN_DTYPE)
-            rc = load().cg_find_matches_batch(self.handle, data.ctypes.data, off.ctypes.data, n, spans.ctypes.data, cap, C.byref(ns))
+            if ids is None:
+                rc = load().cg_find_matches_batch(self.handle, data.ctypes.data, off.ctypes.data, n, spans.ctypes.data, cap, C.byref(ns))
+            else:
+                rc = load().cg_find_matches_batch_views(self.handle, data.ctypes.data, off.ctypes.data, ids.ctypes.data, n, spans.ctypes.data,
+                                                        cap, C.byref(ns))
             if rc == CG_ERR_CAPACITY and ns.value > cap:
                 cap = ns.value
                 continue
@@ -284,17 +340,23 @@ class Ruleset:
         pol = np.ascontiguousarray(rule_policy, dtype=np.uint32); act = np.ascontiguousarray(rule_action, dtype=np.uint8)
         check(load().cg_ruleset_set_policy(self.handle, pol.ctypes.data, act.ctypes.data, len(pol)))
 
-    def verdict_batch(self, data: np.ndarray, off: np.ndarray) -> np.ndarray:
-        """-> uint32 verdict per message: action | matched policies << 2 | deciding rule << 12 (openclaw_gov.h)."""
+    def verdict_batch(self, data: np.ndarray, off: np.ndarray, views=None) -> np.ndarray:
+        """-> uint32 verdict per message: action | matched policies << 2 | deciding rule << 12 (openclaw_gov.h).  views: one
+        view id per message (cg_policy_verdict_batch_views)."""
         n = len(off) - 1
         out = np.zeros(max(n, 1), dtype=np.uint32)
-        check(load().cg_policy_verdict_batch(self.handle, data.ctypes.data, off.ctypes.data, n, out.ctypes.data))
+        if views is None:
+            check(load().cg_policy_verdict_batch(self.handle, data.ctypes.data, off.ctypes.data, n, out.ctypes.data))
+        else:
+            ids = _ids(views, n)
+            check(load().cg_policy_verdict_batch_views(self.handle, data.ctypes.data, off.ctypes.data, ids.ctypes.data, n, out.ctypes.data))
         return out[:n]
 
-    def redact_batch(self, data: np.ndarray, off: np.ndarray):
-        """RedactionEngine.scanString for a batch, spliced on the device.
-        -> (out_bytes uint8[..], out_offsets uint32[n+1], resolved spans, digests uint8[ns, 32])"""
+    def redact_batch(self, data: np.ndarray, off: np.ndarray, views=None):
+        """RedactionEngine.scanString for a batch, spliced on the device.  views: one view id per message
+        (cg_redact_batch_views).  -> (out_bytes uint8[..], out_offsets uint32[n+1], resolved spans, digests uint8[ns, 32])"""
         n = len(off) - 1
+        ids = None if views is None else _ids(views, n)
         total = int(off[n]) if n else 0
         out_off = np.zeros(n + 1, dtype=np.uint32)
         need, ns = C.c_uint64(0), C.c_uint32(0)
@@ -303,8 +365,12 @@ class Ruleset:
             out = np.zeros(cap_bytes + 64, dtype=np.uint8)
             spans = np.zeros(cap_spans, dtype=SPAN_DTYPE)
             dig = np.zeros((cap_spans, 32), dtype=np.uint8)
-            rc = load().cg_redact_batch(self.handle, data.ctypes.data, off.ctypes.data, n, out.ctypes.data, cap_bytes, C.byref(need),
-                                        out_off.ctypes.data, spans.ctypes.data, cap_spans, C.byref(ns), dig.ctypes.data)
+            if ids is None:
+                rc = load().cg_redact_batch(self.handle, data.ctypes.data, off.ctypes.data, n, out.ctypes.data, cap_bytes, C.byref(need),
+                                            out_off.ctypes.data, spans.ctypes.data, cap_spans, C.byref(ns), dig.ctypes.data)
+            else:
+                rc = load().cg_redact_batch_views(self.handle, data.ctypes.data, off.ctypes.data, ids.ctypes.data, n, out.ctypes.data, cap_bytes,
+                                                  C.byref(need), out_off.ctypes.data, spans.ctypes.data, cap_spans, C.byref(ns), dig.ctypes.data)
             if rc == CG_ERR_CAPACITY and (need.value > cap_bytes or ns.value > cap_spans):
                 cap_bytes, cap_spans = max(cap_bytes, need.value), max(cap_spans, ns.value)
                 continue
@@ -326,28 +392,49 @@ class Ruleset:
     def scan_batch_device(self, d_bytes: int, d_off: int, n: int, d_words: int, stream: int = 0):
         check(load().cg_scan_batch_device(self.handle, d_bytes, d_off, n, d_words, stream))
 
-    def find_matches_batch_device(self, d_bytes: int, d_off: int, n: int, d_spans: int, spans_cap: int, d_nspans: int, stream: int = 0):
+    def find_matches_batch_device(self, d_bytes: int, d_off: int, n: int, d_spans: int, spans_cap: int, d_nspans: int, stream: int = 0,
+                                  views=None):
         """cg_find_matches_batch_device on raw device pointers (asynchronous; status from scan_join): resolved spans
-        (SPAN_DTYPE, at most spans_cap) into d_spans, their number (uint32) into d_nspans."""
-        check(load().cg_find_matches_batch_device(self.handle, d_bytes, d_off, n, d_spans or None, spans_cap, d_nspans, stream))
+        (SPAN_DTYPE, at most spans_cap) into d_spans, their number (uint32) into d_nspans.  views: device pointer to one uint8
+        view id per message (cg_find_matches_batch_device_views)."""
+        if views is None:
+            check(load().cg_find_matches_batch_device(self.handle, d_bytes, d_off, n, d_spans or None, spans_cap, d_nspans, stream))
+        else:
+            check(load().cg_find_matches_batch_device_views(self.handle, d_bytes, d_off, views or None, n, d_spans or None, spans_cap, d_nspans, stream))
 
     def redact_batch_device(self, d_bytes: int, d_off: int, n: int, d_out: int, out_cap: int, d_out_off: int, d_spans: int,
-                            spans_cap: int, d_digests: int, d_sizes: int, stream: int = 0):
+                            spans_cap: int, d_digests: int, d_sizes: int, stream: int = 0, views=None):
         """cg_redact_batch_device on raw device pointers (asynchronous; status from scan_join): redacted bytes into d_out,
         offsets (uint32[n+1]) into d_out_off, spans and their SHA-256 (32 bytes each) into d_spans / d_digests, and
-        uint64[2] = (bytes needed, resolved spans) into d_sizes."""
-        check(load().cg_redact_batch_device(self.handle, d_bytes, d_off, n, d_out or None, out_cap, d_out_off, d_spans or None,
-                                            spans_cap, d_digests or None, d_sizes, stream))
+        uint64[2] = (bytes needed, resolved spans) into d_sizes.  views: device pointer to one uint8 view id per message
+        (cg_redact_batch_device_views)."""
+        if views is None:
+            check(load().cg_redact_batch_device(self.handle, d_bytes, d_off, n, d_out or None, out_cap, d_out_off, d_spans or None,
+                                                spans_cap, d_digests or None, d_sizes, stream))
+        else:
+            check(load().cg_redact_batch_device_views(self.handle, d_bytes, d_off, views or None, n, d_out or None, out_cap, d_out_off,
+                                                      d_spans or None, spans_cap, d_digests or None, d_sizes, stream))
 
-    def scan_hits_batch_device(self, d_bytes: int, d_off: int, n: int, d_words: int, d_hits: int, hits_cap: int, d_nhits: int, stream: int = 0):
+    def scan_hits_batch_device(self, d_bytes: int, d_off: int, n: int, d_words: int, d_hits: int, hits_cap: int, d_nhits: int, stream: int = 0,
+                               views=None):
         """cg_scan_hits_batch_device on raw device pointers (asynchronous; status from scan_join): result words (uint64[n])
-        into d_words, the (msg, rule) hits (HIT_DTYPE, sorted, at most hits_cap) into d_hits, their number (uint32) into d_nhits."""
-        check(load().cg_scan_hits_batch_device(self.handle, d_bytes, d_off, n, d_words, d_hits or None, hits_cap, d_nhits, stream))
+        into d_words, the (msg, rule) hits (HIT_DTYPE, sorted, at most hits_cap) into d_hits, their number (uint32) into d_nhits.
+        views: device pointer to one uint8 view id per message (cg_scan_hits_batch_device_views; there d_hits = d_nhits = 0
+        with hits_cap 0 writes the words alone)."""
+        if views is None:
+            check(load().cg_scan_hits_batch_device(self.handle, d_bytes, d_off, n, d_words, d_hits or None, hits_cap, d_nhits, stream))
+        else:
+            check(load().cg_scan_hits_batch_device_views(self.handle, d_bytes, d_off, views or None, n, d_words, d_hits or None, hits_cap,
+                                                         d_nhits or None, stream))
 
-    def verdict_batch_device(self, d_bytes: int, d_off: int, n: int, d_verdicts: int, stream: int = 0):
+    def verdict_batch_device(self, d_bytes: int, d_off: int, n: int, d_verdicts: int, stream: int = 0, views=None):
         """cg_policy_verdict_batch_device on raw device pointers (asynchronous; status from scan_join): one uint32 verdict per
-        message into d_verdicts, as verdict_batch returns them (0xffffffff each after an internal queue overflow)."""
-        check(load().cg_policy_verdict_batch_device(self.handle, d_bytes, d_off, n, d_verdicts, stream))
+        message into d_verdicts, as verdict_batch returns them (0xffffffff each after an internal queue overflow).  views:
+        device pointer to one uint8 view id per message (cg_policy_verdict_batch_device_views)."""
+        if views is None:
+            check(load().cg_policy_verdict_batch_device(self.handle, d_bytes, d_off, n, d_verdicts, stream))
+        else:
+            check(load().cg_policy_verdict_batch_device_views(self.handle, d_bytes, d_off, views or None, n, d_verdicts, stream))
 
 
 def sha256_batch(data: np.ndarray, off64: np.ndarray) -> np.ndarray:

@@ -48,6 +48,7 @@ struct Ctx {
   uint8_t* d_redact_out = nullptr; size_t cap_redact_out = 0; uint32_t* d_redact_meta = nullptr; size_t cap_redact_meta = 0;
   uint32_t* d_verdicts = nullptr; size_t cap_verdicts = 0;
   uint32_t* d_hits = nullptr; size_t cap_hits = 0;          // cg_scan_batch's hit list: [count][(msg, rule) pairs]
+  uint8_t* d_views = nullptr; size_t cap_views = 0;         // the host-buffer *_views calls' view ids, staged beside the offsets
 } G;
 
 int fail(int code, const std::string& msg) { g_err = msg; return code; }
@@ -129,7 +130,10 @@ struct cg_ruleset {
   struct OnePath { OneGraph g[3]; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint8_t* h_pack = nullptr; uint8_t* d_pack = nullptr; } one;
   CachedGraph graphs[2];          // two entries: callers that alternate between two input/output buffer sets replay, never re-capture
   uint64_t graph_clock = 0;
+  // cg_ruleset_set_views: n_views rows of dev.rw words in HBM (bit r of row v = rule r is in view v); none before the first call
+  uint32_t* view_rows = nullptr; uint32_t n_views = 0;
   ~cg_ruleset() {
+    cudaFree(view_rows);
     for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     for (auto& g : one.g) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (one.h_pin) cudaFreeHost(one.h_pin);
@@ -206,8 +210,10 @@ static uint32_t scan_pieces() { static const uint32_t k = [] { const char* e = g
 enum StepKind { kStepWords, kStepPolicy, kStepSpans };
 
 // One step on device-resident input: scratch reset, gram scan (+ exact factors), resolve, verify, finalize; over no message
-// only the zeroed counter block.  Asynchronous.
-int run_scan_device(cg_ruleset* rs, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, uint64_t* d_words, StepKind kind, cudaStream_t st) {
+// only the zeroed counter block.  With views, resolve admits only the (message, rule) pairs of each message's view.
+// Asynchronous.
+int run_scan_device(cg_ruleset* rs, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, uint64_t* d_words, StepKind kind, cudaStream_t st,
+                    const ViewTable* views = nullptr) {
   const ScanWork& w = rs->work;
   if (!n) { CU(cudaMemsetAsync(w.counters, 0, kCounterWords * sizeof(uint32_t), st)); return CG_OK; }
   const bool spans = kind == kStepSpans;
@@ -228,7 +234,7 @@ int run_scan_device(cg_ruleset* rs, const uint8_t* d_bytes, const uint32_t* d_of
     k += launch_confirm(rs->dev, wk, d_bytes, d_off + m0, m1 - m0, G.sm_count, st);
   }
   if (G.profiling) cudaEventRecord(G.pev[1], st);
-  k += launch_resolve(rs->dev, w, d_bytes, d_off, n, spans, G.sm_count, st);
+  k += launch_resolve(rs->dev, w, d_bytes, d_off, n, spans, G.sm_count, st, views);
   if (G.profiling) cudaEventRecord(G.pev[2], st);
   k += launch_verify(rs->dev, w, d_bytes, d_off, spans, G.sm_count, st, spans ? 4 : rs->verify_ctas);
   if (G.profiling) cudaEventRecord(G.pev[3], st);
@@ -318,9 +324,10 @@ int check_offsets(const uint32_t* offsets, uint32_t n) {
 // The host-buffer calls' driver: stages the batch into G.d_bytes / G.d_off32, then per attempt the step of `kind` (result
 // words to G.d_words, a span step's to the scratch), the work after(scratch) enqueues behind it (-> CG_OK or an error; it
 // may copy sizes to the host, never into the caller's buffers), the counter block to the host and one synchronise.  A
-// queue overflow grows the scratch and runs the attempt again.  last_scan_ms times the step alone.
+// queue overflow grows the scratch and runs the attempt again.  last_scan_ms times the step alone.  views (one id per message,
+// checked by the caller): staged beside the offsets, the step filtered by them.
 template <typename After>
-int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, StepKind kind, After&& after) {
+int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, StepKind kind, After&& after, const uint8_t* views = nullptr) {
   if (int rc = require_ready()) return rc;
   if (!rs || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
   int rc;
@@ -329,18 +336,21 @@ int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uin
   if ((rc = grow_bytes(total + 64))) return rc;
   if ((rc = grow(&G.d_off32, &G.cap_off32, (size_t)n + 1))) return rc;
   if ((rc = grow(&G.d_words, &G.cap_words, (size_t)n + 1))) return rc;
+  if (views && (rc = grow(&G.d_views, &G.cap_views, (size_t)n + 1))) return rc;
   cudaStream_t st = G.stream;
   if (n) {
     if (total > first) CU(cudaMemcpyAsync(G.d_bytes + first, bytes + first, total - first, cudaMemcpyHostToDevice, st));
     CU(cudaMemsetAsync(G.d_bytes + total, 0, 64, st));
     CU(cudaMemcpyAsync(G.d_off32, offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (views) CU(cudaMemcpyAsync(G.d_views, views, n, cudaMemcpyHostToDevice, st));
   }
+  const ViewTable vt{rs->view_rows, G.d_views, rs->n_views};
   uint32_t hc[kCounterWords] = {};
   for (int attempt = 0; attempt < 10; attempt++) {
     if ((rc = prepare_step(rs, n, kind, st))) return rc;
     const ScanWork& w = rs->work;
     CU(cudaEventRecord(G.ev0, st));
-    if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32, n, kind == kStepSpans ? w.words : G.d_words, kind, st))) return rc;
+    if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32, n, kind == kStepSpans ? w.words : G.d_words, kind, st, views ? &vt : nullptr))) return rc;
     CU(cudaEventRecord(G.ev1, st));
     if ((rc = after(w))) return rc;
     CU(cudaMemcpyAsync(hc, w.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
@@ -507,16 +517,17 @@ int replay_step(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint
 // The device-resident calls' driver, asynchronous on st: grows the scratch first if an earlier batch overflowed, enqueues
 // the step of `kind` (replayed as a graph when `graph`), the work after(scratch) enqueues behind it (-> its launch count)
 // and the counter block into the mirror ring.  Result words go to d_words, or when it is null to the scratch's (looked up
-// after prepare_step, which may replace that buffer).  Never waits for the device except when the scratch must grow.
+// after prepare_step, which may replace that buffer).  Never waits for the device except when the scratch must grow.  views:
+// the step filtered by them (never replayed as a graph).
 template <typename After>
 int scan_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, uint64_t* d_words, StepKind kind, cudaStream_t st,
-                After&& after, bool graph = false) {
+                After&& after, bool graph = false, const ViewTable* views = nullptr) {
   int rc;
   if ((rc = ensure_mirrors(rs))) return rc;
   poll_mirrors(rs, false);                                  // (an earlier batch overflowed?  grow before this one runs)
   if ((rc = prepare_step(rs, n, kind, st))) return rc;
   if (!d_words) d_words = rs->work.words;
-  const auto step = [&] { return run_scan_device(rs, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, n, d_words, kind, st); };
+  const auto step = [&] { return run_scan_device(rs, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, n, d_words, kind, st, views); };
   if ((rc = graph ? replay_step(rs, d_bytes, d_offsets, n, d_words, st, step) : step())) return rc;
   count_launches(after(rs->work));
   CU(cudaGetLastError());
@@ -579,7 +590,7 @@ void cg_shutdown(void) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!G.ready) return;
   cudaDeviceSynchronize();
-  cudaFree(G.d_spans); cudaFree(G.d_redact_out); cudaFree(G.d_redact_meta); cudaFree(G.d_verdicts); cudaFree(G.d_hits);
+  cudaFree(G.d_spans); cudaFree(G.d_redact_out); cudaFree(G.d_redact_meta); cudaFree(G.d_verdicts); cudaFree(G.d_hits); cudaFree(G.d_views);
   if (G.h_chunk_counters) cudaFreeHost(G.h_chunk_counters);
   if (G.s_h2d) { cudaStreamDestroy(G.s_h2d); cudaStreamDestroy(G.s_d2h); for (int c = 0; c < Ctx::kChunks; c++) { cudaEventDestroy(G.e_h2d[c]); cudaEventDestroy(G.e_done[c]); } }
   cudaFree(G.d_bytes_raw); cudaFree(G.d_off32); cudaFree(G.d_off64); cudaFree(G.d_words); cudaFree(G.d_dig[0]); cudaFree(G.d_dig[1]);
@@ -743,6 +754,11 @@ int cg_ruleset_get_info(const cg_ruleset* rs, cg_ruleset_info* o) {
   return CG_OK;
 }
 
+namespace {
+int scan_batch_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint64_t* out_words,
+                    cg_hit* out_hits, uint32_t hits_cap, uint32_t* out_nhits, const uint8_t* views);
+}  // namespace
+
 int cg_scan_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint64_t* out_words,
                   cg_hit* out_hits, uint32_t hits_cap, uint32_t* out_nhits) {
   std::lock_guard<std::mutex> lk(g_mu);
@@ -758,18 +774,25 @@ int cg_scan_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets,
     }
     // rc == 1: a queue overflowed in some piece; capacities have been raised -- run the batch in one piece below
   }
-  // the hit list on the device (as cg_scan_hits_batch_device builds it): counts and their scan behind the step, the total to
-  // the host, then the first min(total, hits_cap) pairs into a staging buffer and back
+  return scan_batch_host(rs, bytes, offsets, n, out_words, out_hits, hits_cap, out_nhits, nullptr);
+}
+
+namespace {
+// the one-piece path of cg_scan_batch, and cg_scan_batch_views.  The hit list on the device (as cg_scan_hits_batch_device
+// builds it): counts and their scan behind the step, the total to the host, then the first min(total, hits_cap) pairs into a
+// staging buffer and back
+int scan_batch_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint64_t* out_words,
+                    cg_hit* out_hits, uint32_t hits_cap, uint32_t* out_nhits, const uint8_t* views) {
   const bool want_hits = out_hits || out_nhits;
   cudaStream_t st = G.stream;
   uint64_t total = 0;
-  rc = scan_host(rs, bytes, offsets, n, want_hits ? kStepPolicy : kStepWords, [&](const ScanWork& w) {
+  int rc = scan_host(rs, bytes, offsets, n, want_hits ? kStepPolicy : kStepWords, [&](const ScanWork& w) {
     if (!want_hits || !n) return CG_OK;
     count_launches(launch_hit_count(w, G.d_words, n, G.sm_count, st));
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(&total, w.out_off + n, 8, cudaMemcpyDeviceToHost, st));
     return CG_OK;
-  });
+  }, views);
   if (rc) return rc;
   const uint32_t nh = (uint32_t)total, k = out_hits && !(total >> 32) ? std::min(nh, hits_cap) : 0u;
   if (out_words && n) CU(cudaMemcpyAsync(out_words, G.d_words, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
@@ -785,6 +808,23 @@ int cg_scan_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets,
   G.stats.hits += nh;
   if (out_hits && nh > hits_cap) return fail(CG_ERR_CAPACITY, "out_hits too small");
   return CG_OK;
+}
+
+// the host-buffer *_views calls' ids, checked before anything is staged or written
+int check_views(const cg_ruleset* rs, const uint8_t* views, uint32_t n) {
+  if (int rc = require_ready()) return rc;
+  if (!rs || (n && !views)) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (!rs->n_views) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_views has not been called");
+  for (uint32_t i = 0; i < n; i++) if (views[i] >= rs->n_views) return fail(CG_ERR_INVALID_ARG, "view id " + std::to_string(views[i]) + " of message " + std::to_string(i) + " >= n_views");
+  return CG_OK;
+}
+}  // namespace
+
+int cg_scan_batch_views(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, const uint8_t* views, uint32_t n, uint64_t* out_words,
+                        cg_hit* out_hits, uint32_t hits_cap, uint32_t* out_nhits) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = check_views(rs, views, n)) return rc;
+  return scan_batch_host(rs, bytes, offsets, n, out_words, out_hits, hits_cap, out_nhits, views);
 }
 
 namespace {
@@ -850,12 +890,11 @@ int resolve_staged(const ScanWork& w, uint32_t n, bool redact, uint64_t sizes[2]
   CU(cudaMemcpyAsync(sizes, G.d_redact_meta, redact ? 16 : 4, cudaMemcpyDeviceToHost, G.stream));
   return CG_OK;
 }
-}  // namespace
 
-int cg_find_matches_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans) {
-  std::lock_guard<std::mutex> lk(g_mu);
+int find_matches_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans,
+                      const uint8_t* views) {
   uint64_t sizes[2] = {0, 0}; uint32_t* d_dig = nullptr;
-  int rc = scan_host(rs, bytes, offsets, n, kStepSpans, [&](const ScanWork& w) { return resolve_staged(w, n, false, sizes, &d_dig); });
+  int rc = scan_host(rs, bytes, offsets, n, kStepSpans, [&](const ScanWork& w) { return resolve_staged(w, n, false, sizes, &d_dig); }, views);
   if (rc) return rc;
   const uint32_t outn = (uint32_t)sizes[0], k = std::min(outn, spans_cap);
   G.stats.spans += outn;
@@ -863,6 +902,19 @@ int cg_find_matches_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* 
   if (out_nspans) *out_nspans = outn;
   if (out_spans && outn > spans_cap) return fail(CG_ERR_CAPACITY, "out_spans too small");
   return CG_OK;
+}
+}  // namespace
+
+int cg_find_matches_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return find_matches_host(rs, bytes, offsets, n, out_spans, spans_cap, out_nspans, nullptr);
+}
+
+int cg_find_matches_batch_views(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, const uint8_t* views, uint32_t n, cg_span* out_spans,
+                                uint32_t spans_cap, uint32_t* out_nspans) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = check_views(rs, views, n)) return rc;
+  return find_matches_host(rs, bytes, offsets, n, out_spans, spans_cap, out_nspans, views);
 }
 
 int cg_ruleset_set_policy(cg_ruleset* rs, const uint32_t* rule_policy, const uint8_t* rule_action, uint32_t n_rules) {
@@ -883,10 +935,28 @@ int cg_ruleset_set_policy(cg_ruleset* rs, const uint32_t* rule_policy, const uin
   return CG_OK;
 }
 
-int cg_policy_verdict_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint32_t* out_verdicts) {
+int cg_ruleset_set_views(cg_ruleset* rs, const uint32_t* rows, uint32_t n_views) {
   std::lock_guard<std::mutex> lk(g_mu);
-  if (!rs || !out_verdicts) return fail(CG_ERR_INVALID_ARG, "null argument");
-  if (!rs->dev.rule_policy) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy has not been called");
+  if (int rc = require_ready()) return rc;
+  if (!rs || !rows) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (n_views < 1 || n_views > 256) return fail(CG_ERR_INVALID_ARG, "n_views must be 1 .. 256");
+  const uint32_t n_rules = rs->dev.n_rules, rw = rs->dev.rw;
+  for (uint32_t v = 0; v < n_views; v++)
+    for (uint32_t k = 0; k < rw; k++) {
+      const uint32_t valid = n_rules >= 32 * (k + 1) ? ~0u : n_rules > 32 * k ? (1u << (n_rules - 32 * k)) - 1u : 0u;     // bits of rules < n_rules
+      if (rows[(size_t)v * rw + k] & ~valid) return fail(CG_ERR_INVALID_ARG, "view " + std::to_string(v) + " has a bit at or past n_rules");
+    }
+  CU(cudaStreamSynchronize(G.stream));
+  cudaFree(rs->view_rows); rs->view_rows = nullptr; rs->n_views = 0;
+  CU(cudaMalloc((void**)&rs->view_rows, (size_t)n_views * rw * 4));
+  CU(cudaMemcpy(rs->view_rows, rows, (size_t)n_views * rw * 4, cudaMemcpyHostToDevice));
+  rs->n_views = n_views;
+  rs->scratch_gen++;
+  return CG_OK;
+}
+
+namespace {
+int verdict_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint32_t* out_verdicts, const uint8_t* views) {
   cudaStream_t st = G.stream;
   int rc = scan_host(rs, bytes, offsets, n, kStepWords, [&](const ScanWork& w) {
     if (!n) return CG_OK;
@@ -896,19 +966,36 @@ int cg_policy_verdict_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t
     count_launches(launch_verdicts(rs->dev, w, G.d_verdicts, n, G.sm_count, st));
     CU(cudaGetLastError());
     return CG_OK;
-  });
+  }, views);
   if (rc || !n) return rc;
   CU(cudaMemcpyAsync(out_verdicts, G.d_verdicts, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
 }
+}  // namespace
 
-int cg_redact_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint8_t* out_bytes, uint64_t out_cap,
-                    uint64_t* out_need, uint32_t* out_offsets, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans, uint8_t* out_digests32) {
+int cg_policy_verdict_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint32_t* out_verdicts) {
   std::lock_guard<std::mutex> lk(g_mu);
+  if (!rs || !out_verdicts) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (!rs->dev.rule_policy) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy has not been called");
+  return verdict_host(rs, bytes, offsets, n, out_verdicts, nullptr);
+}
+
+int cg_policy_verdict_batch_views(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, const uint8_t* views, uint32_t n, uint32_t* out_verdicts) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = check_views(rs, views, n)) return rc;
+  if (!out_verdicts) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (!rs->dev.rule_policy) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy has not been called");
+  return verdict_host(rs, bytes, offsets, n, out_verdicts, views);
+}
+
+namespace {
+int redact_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint8_t* out_bytes, uint64_t out_cap,
+                uint64_t* out_need, uint32_t* out_offsets, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans, uint8_t* out_digests32,
+                const uint8_t* views) {
   if (!out_offsets || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
   uint64_t sizes[2] = {0, 0}; uint32_t* d_dig = nullptr;
-  int rc = scan_host(rs, bytes, offsets, n, kStepSpans, [&](const ScanWork& w) { return resolve_staged(w, n, true, sizes, &d_dig); });
+  int rc = scan_host(rs, bytes, offsets, n, kStepSpans, [&](const ScanWork& w) { return resolve_staged(w, n, true, sizes, &d_dig); }, views);
   if (rc) return rc;                                        // (input bytes / offsets stay in G.d_bytes / G.d_off32)
   const uint64_t pos = sizes[0]; const uint32_t ns = (uint32_t)sizes[1];
   G.stats.spans += ns;
@@ -930,6 +1017,21 @@ int cg_redact_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offset
   if (too_large) return fail(CG_ERR_TOO_LARGE, "redacted batch exceeds 4 GiB");
   if (!fits) return fail(CG_ERR_CAPACITY, "output buffer too small (see *out_need / *out_nspans)");
   return CG_OK;
+}
+}  // namespace
+
+int cg_redact_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint8_t* out_bytes, uint64_t out_cap,
+                    uint64_t* out_need, uint32_t* out_offsets, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans, uint8_t* out_digests32) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return redact_host(rs, bytes, offsets, n, out_bytes, out_cap, out_need, out_offsets, out_spans, spans_cap, out_nspans, out_digests32, nullptr);
+}
+
+int cg_redact_batch_views(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, const uint8_t* views, uint32_t n, uint8_t* out_bytes,
+                          uint64_t out_cap, uint64_t* out_need, uint32_t* out_offsets, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans,
+                          uint8_t* out_digests32) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = check_views(rs, views, n)) return rc;
+  return redact_host(rs, bytes, offsets, n, out_bytes, out_cap, out_need, out_offsets, out_spans, spans_cap, out_nspans, out_digests32, views);
 }
 
 namespace {
@@ -1046,9 +1148,18 @@ int cg_scan_join(cg_ruleset* rs, void* stream) {
   return CG_OK;
 }
 
-int cg_find_matches_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_spans, uint32_t spans_cap,
-                                 void* d_out_nspans, void* stream) {
-  std::lock_guard<std::mutex> lk(g_mu);
+namespace {
+// the device-resident *_views calls' table: the rule set's rows and the caller's ids in HBM (which the host cannot check: an id
+// >= n_views selects the empty view)
+int device_views(const cg_ruleset* rs, const void* d_views, ViewTable* vt) {
+  if (!rs->n_views) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_views has not been called");
+  if (!d_views) return fail(CG_ERR_INVALID_ARG, "null argument");
+  *vt = ViewTable{rs->view_rows, (const uint8_t*)d_views, rs->n_views};
+  return CG_OK;
+}
+
+int find_matches_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_spans, uint32_t spans_cap,
+                        void* d_out_nspans, void* stream, const ViewTable* views) {
   if (int rc = device_batch_args(rs, d_bytes, d_offsets)) return rc;
   if ((spans_cap && !d_out_spans) || !d_out_nspans) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (((uintptr_t)d_offsets | (uintptr_t)d_out_spans | (uintptr_t)d_out_nspans) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets, d_out_spans and d_out_nspans must be 4-byte aligned");
@@ -1056,12 +1167,11 @@ int cg_find_matches_batch_device(cg_ruleset* rs, const void* d_bytes, const void
   const SpanOutputs o{(uint32_t*)d_out_spans, d_out_spans ? spans_cap : 0u, nullptr, 0, d_out_nspans, false};
   return scan_device(rs, d_bytes, d_offsets, n, nullptr, kStepSpans, st, [&](const ScanWork& w) {
     return launch_span_resolve(w, (const uint32_t*)d_offsets, n, o, G.sm_count, st);
-  });
+  }, false, views);
 }
 
-int cg_redact_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_bytes, uint64_t out_cap,
-                           void* d_out_offsets, void* d_out_spans, uint32_t spans_cap, void* d_out_digests32, void* d_out_sizes, void* stream) {
-  std::lock_guard<std::mutex> lk(g_mu);
+int redact_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_bytes, uint64_t out_cap,
+                  void* d_out_offsets, void* d_out_spans, uint32_t spans_cap, void* d_out_digests32, void* d_out_sizes, void* stream, const ViewTable* views) {
   if (int rc = device_batch_args(rs, d_bytes, d_offsets)) return rc;
   if (!d_out_offsets || !d_out_sizes || (out_cap && !d_out_bytes) || (spans_cap && (!d_out_spans || !d_out_digests32))) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (((uintptr_t)d_offsets | (uintptr_t)d_out_offsets | (uintptr_t)d_out_spans) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets, d_out_offsets and d_out_spans must be 4-byte aligned");
@@ -1073,27 +1183,28 @@ int cg_redact_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_of
     const int k = launch_span_resolve(w, (const uint32_t*)d_offsets, n, o, G.sm_count, st);
     return k + enqueue_redact_tail(w, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, o.out_offsets, (uint32_t*)d_out_digests32,
                                    (uint8_t*)d_out_bytes, n, st);
-  });
+  }, false, views);
 }
 
-int cg_scan_hits_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_words, void* d_out_hits,
-                              uint32_t hits_cap, void* d_out_nhits, void* stream) {
-  std::lock_guard<std::mutex> lk(g_mu);
+// (with views, d_out_nhits = NULL, d_out_hits = NULL and hits_cap = 0: the result words alone, as cg_scan_batch_device)
+int scan_hits_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_words, void* d_out_hits,
+                     uint32_t hits_cap, void* d_out_nhits, void* stream, const ViewTable* views) {
   if (int rc = device_batch_args(rs, d_bytes, d_offsets)) return rc;
-  if (!d_out_words || !d_out_nhits || (hits_cap && !d_out_hits)) return fail(CG_ERR_INVALID_ARG, "null argument");
+  const bool words_only = views && !d_out_nhits && !d_out_hits && !hits_cap;
+  if (!d_out_words || (!d_out_nhits && !words_only) || (hits_cap && !d_out_hits)) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (((uintptr_t)d_offsets | (uintptr_t)d_out_hits | (uintptr_t)d_out_nhits) & 3u) return fail(CG_ERR_INVALID_ARG, "d_offsets, d_out_hits and d_out_nhits must be 4-byte aligned");
   if ((uintptr_t)d_out_words & 7u) return fail(CG_ERR_INVALID_ARG, "d_out_words must be 8-byte aligned");
   cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
-  if (!n) { CU(cudaMemsetAsync(d_out_nhits, 0, 4, st)); return CG_OK; }
   uint64_t* words = (uint64_t*)d_out_words;
+  if (words_only) return n ? scan_device(rs, d_bytes, d_offsets, n, words, kStepWords, st, [](const ScanWork&) { return 0; }, false, views) : CG_OK;
+  if (!n) { CU(cudaMemsetAsync(d_out_nhits, 0, 4, st)); return CG_OK; }
   return scan_device(rs, d_bytes, d_offsets, n, words, kStepPolicy, st, [&](const ScanWork& w) {
     const int k = launch_hit_count(w, words, n, G.sm_count, st);
     return k + launch_hit_emit(rs->dev, w, n, (uint32_t*)d_out_hits, d_out_hits ? hits_cap : 0u, (uint32_t*)d_out_nhits, G.sm_count, st);
-  });
+  }, false, views);
 }
 
-int cg_policy_verdict_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_verdicts, void* stream) {
-  std::lock_guard<std::mutex> lk(g_mu);
+int verdict_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_verdicts, void* stream, const ViewTable* views) {
   if (int rc = device_batch_args(rs, d_bytes, d_offsets)) return rc;
   if (!d_out_verdicts) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (!rs->dev.rule_policy) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy has not been called");
@@ -1102,7 +1213,67 @@ int cg_policy_verdict_batch_device(cg_ruleset* rs, const void* d_bytes, const vo
   if (!n) return CG_OK;
   uint32_t* verdicts = (uint32_t*)d_out_verdicts;
   CU(cudaMemsetAsync(verdicts, 0, (size_t)n * 4, st));       // (verdict_kernel writes the messages that hit)
-  return scan_device(rs, d_bytes, d_offsets, n, nullptr, kStepPolicy, st, [&](const ScanWork& w) { return launch_verdicts(rs->dev, w, verdicts, n, G.sm_count, st); });
+  return scan_device(rs, d_bytes, d_offsets, n, nullptr, kStepPolicy, st, [&](const ScanWork& w) { return launch_verdicts(rs->dev, w, verdicts, n, G.sm_count, st); },
+                     false, views);
+}
+
+// the checks of a device-resident *_views call, then its table
+int device_views_args(const cg_ruleset* rs, const void* d_bytes, const void* d_offsets, const void* d_views, ViewTable* vt) {
+  if (int rc = device_batch_args(rs, d_bytes, d_offsets)) return rc;
+  return device_views(rs, d_views, vt);
+}
+}  // namespace
+
+int cg_find_matches_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_spans, uint32_t spans_cap,
+                                 void* d_out_nspans, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return find_matches_device(rs, d_bytes, d_offsets, n, d_out_spans, spans_cap, d_out_nspans, stream, nullptr);
+}
+int cg_find_matches_batch_device_views(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, const void* d_views, uint32_t n, void* d_out_spans,
+                                       uint32_t spans_cap, void* d_out_nspans, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  ViewTable vt;
+  if (int rc = device_views_args(rs, d_bytes, d_offsets, d_views, &vt)) return rc;
+  return find_matches_device(rs, d_bytes, d_offsets, n, d_out_spans, spans_cap, d_out_nspans, stream, &vt);
+}
+
+int cg_redact_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_bytes, uint64_t out_cap,
+                           void* d_out_offsets, void* d_out_spans, uint32_t spans_cap, void* d_out_digests32, void* d_out_sizes, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return redact_device(rs, d_bytes, d_offsets, n, d_out_bytes, out_cap, d_out_offsets, d_out_spans, spans_cap, d_out_digests32, d_out_sizes, stream, nullptr);
+}
+int cg_redact_batch_device_views(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, const void* d_views, uint32_t n, void* d_out_bytes,
+                                 uint64_t out_cap, void* d_out_offsets, void* d_out_spans, uint32_t spans_cap, void* d_out_digests32, void* d_out_sizes,
+                                 void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  ViewTable vt;
+  if (int rc = device_views_args(rs, d_bytes, d_offsets, d_views, &vt)) return rc;
+  return redact_device(rs, d_bytes, d_offsets, n, d_out_bytes, out_cap, d_out_offsets, d_out_spans, spans_cap, d_out_digests32, d_out_sizes, stream, &vt);
+}
+
+int cg_scan_hits_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_words, void* d_out_hits,
+                              uint32_t hits_cap, void* d_out_nhits, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return scan_hits_device(rs, d_bytes, d_offsets, n, d_out_words, d_out_hits, hits_cap, d_out_nhits, stream, nullptr);
+}
+int cg_scan_hits_batch_device_views(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, const void* d_views, uint32_t n, void* d_out_words,
+                                    void* d_out_hits, uint32_t hits_cap, void* d_out_nhits, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  ViewTable vt;
+  if (int rc = device_views_args(rs, d_bytes, d_offsets, d_views, &vt)) return rc;
+  return scan_hits_device(rs, d_bytes, d_offsets, n, d_out_words, d_out_hits, hits_cap, d_out_nhits, stream, &vt);
+}
+
+int cg_policy_verdict_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_verdicts, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return verdict_device(rs, d_bytes, d_offsets, n, d_out_verdicts, stream, nullptr);
+}
+int cg_policy_verdict_batch_device_views(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, const void* d_views, uint32_t n, void* d_out_verdicts,
+                                         void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  ViewTable vt;
+  if (int rc = device_views_args(rs, d_bytes, d_offsets, d_views, &vt)) return rc;
+  return verdict_device(rs, d_bytes, d_offsets, n, d_out_verdicts, stream, &vt);
 }
 
 // ---------------------------------------------------------------------------------- SHA / Merkle

@@ -128,8 +128,13 @@ int launch_scan(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes,
                 uint64_t* d_words, int sm_count, cudaStream_t stream);
 // per piece of the batch: flag words -> grams -> recheck map -> table probes -> exact factors (confirm_kernel)
 int launch_confirm(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, int sm_count, cudaStream_t stream);
-// once per step: message, slot, candidates for the VM / direct hits / island matcher
-int launch_resolve(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, bool want_spans, int sm_count, cudaStream_t stream);
+// Per-message rule subsets (cg_ruleset_set_views): row v is rw words, bit r set = rule r is in view v; ids[m] = the view of
+// message m of the launch (an id >= n_views is the empty view).  Passed by value to resolve_views_kernel only.
+struct ViewTable { const uint32_t* rows; const uint8_t* ids; uint32_t n_views; };
+// once per step: message, slot, candidates for the VM / direct hits / island matcher; with views, only the pairs whose rule
+// is in the message's view
+int launch_resolve(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, bool want_spans, int sm_count, cudaStream_t stream,
+                   const ViewTable* views = nullptr);
 // ctas_per_sm (1 .. 4): events are handed out by an atomic cursor, so any grid is correct; an empty launch costs more at four
 // CTAs per SM than at one, so the caller sizes the grid by what the previous steps sent to the VM
 int launch_verify(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off,

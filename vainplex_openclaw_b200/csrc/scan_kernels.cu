@@ -8,6 +8,7 @@
 //                   work handed from stage to stage in ballot-compacted waves.
 //   resolve_kernel  level 2: message of every confirmed factor occurrence; RegExp.test around it by the bit-parallel
 //                   island matcher (bitprog.h), or a direct hit, or a (message, rule) pair for the VM.
+//                   (resolve_views_kernel: the same for the rules of each message's view only.)
 //   verify_kernel   exact ECMAScript semantics for the queued pairs: a Pike VM over UTF-16 units
 //                   decoded on the fly from the UTF-8 bytes (leftmost-first, global-exec
 //                   iteration of registry.ts:225-236, RegExp.test of context.ts:9-25).
@@ -527,8 +528,21 @@ confirm_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ Sc
   if (lane == 0) { if (flagged) atomicAdd(&w.counters[kCtrFlagged], flagged); if (passed) atomicAdd(&w.counters[kCtrPastRecheck], passed); if (c.ptail) atomicAdd(&w.counters[kCtrPairs + w.q_slot], c.ptail); }
 }
 
-__global__ void __launch_bounds__(256, 4)
-resolve_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, int want_spans, uint32_t spread) {
+// Which (message, rule) pairs may enter a slot: every pair (the calls without views), or only the rules of the message's
+// view (ViewTable, kernels.h).  The test sits in front of SlotSink, so an out-of-view occurrence takes no slot, walks no
+// island and queues no VM event; everything downstream reads the slot's rows only and so sees the view's rules alone.
+struct AllRules { __device__ __forceinline__ bool admits(uint32_t, uint32_t) const { return true; } };
+struct InView {
+  ViewTable vt; uint32_t rw;
+  __device__ __forceinline__ bool admits(uint32_t msg, uint32_t r) const {
+    const uint32_t v = vt.ids[msg];
+    return v < vt.n_views && ((vt.rows[(size_t)v * rw + (r >> 5)] >> (r & 31)) & 1u);
+  }
+};
+
+template <class Filter>
+__device__ __forceinline__ void resolve_occurrences(const DevRuleset& rs, const ScanWork& w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off,
+                                                    uint32_t n, int want_spans, uint32_t spread, const Filter& filter) {
   const uint32_t n1 = min(w.counters[kCtrConfirmed], w.l1_cap);
   const uint32_t stride = gridDim.x * blockDim.x, tid = blockIdx.x * blockDim.x + threadIdx.x;
   // Occurrences take different paths of very different lengths (direct hit, island matcher of 5 .. 96 steps, slot allocation),
@@ -539,14 +553,28 @@ resolve_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, con
     const uint32_t pos = w.l1_pos[i], f = w.l1_fac[i];
     const uint32_t msg = message_of(off, n, pos);
     if (pos + (rs.factors[(size_t)f * 12 + 1] & 0xffu) > off[msg + 1]) continue;     // straddles two messages: not an occurrence
+    if (!filter.admits(msg, rs.factors[(size_t)f * 12])) continue;                      // (the factor's rule: factor_confirmed's)
     SlotSink sink(rs, w, msg, want_spans != 0);
     sink.text = bytes + off[msg]; sink.text_len = off[msg + 1] - off[msg];
     factor_confirmed(rs, f, pos - off[msg], want_spans != 0, sink);
   }
   if (rs.n_always) for (uint32_t msg = tid; msg < n; msg += stride) {
     SlotSink sink(rs, w, msg, want_spans != 0);
-    for (uint32_t k = 0; k < rs.n_always; k++) sink.candidate_always(rs.always_rules[k]);
+    for (uint32_t k = 0; k < rs.n_always; k++) if (filter.admits(msg, rs.always_rules[k])) sink.candidate_always(rs.always_rules[k]);
   }
+}
+
+__global__ void __launch_bounds__(256, 4)
+resolve_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, int want_spans, uint32_t spread) {
+  resolve_occurrences(rs, w, bytes, off, n, want_spans, spread, AllRules{});
+}
+// the same with the views of cg_*_views: the table is an argument of its own (DevRuleset / ScanWork keep their layout).  Two
+// CTAs per SM, not four: under resolve_kernel's 64-register cap this instantiation spills; at this bound it takes 90
+// registers and spills nothing
+__global__ void __launch_bounds__(256, 2)
+resolve_views_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, int want_spans, uint32_t spread,
+                     ViewTable views) {
+  resolve_occurrences(rs, w, bytes, off, n, want_spans, spread, InView{views, rs.rw});
 }
 
 // ------------------------------------------------------------------------------------------
@@ -829,10 +857,12 @@ int launch_confirm(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_byt
   confirm_kernel<<<scan_grid(n, sm_count), kCfThreads, (size_t)kCfRingBytes + (rs.cf_resident ? rs.cf_bytes : 0u), stream>>>(rs, w, d_bytes, d_off, n, cstep);
   return 1;
 }
-int launch_resolve(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, bool want_spans, int sm_count, cudaStream_t stream) {
+int launch_resolve(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, bool want_spans, int sm_count, cudaStream_t stream,
+                   const ViewTable* views) {
   if (n == 0) return 0;
   static const uint32_t spread = [] { const char* e = getenv("CG_RESOLVE_SPREAD"); const int v = e ? atoi(e) : 4; return (uint32_t)(v == 1 || v == 2 || v == 4 || v == 8 || v == 16 || v == 32 ? v : 4); }();
-  resolve_kernel<<<sm_count * 8, 256, 0, stream>>>(rs, w, d_bytes, d_off, n, want_spans ? 1 : 0, spread);
+  if (views) resolve_views_kernel<<<sm_count * 8, 256, 0, stream>>>(rs, w, d_bytes, d_off, n, want_spans ? 1 : 0, spread, *views);
+  else resolve_kernel<<<sm_count * 8, 256, 0, stream>>>(rs, w, d_bytes, d_off, n, want_spans ? 1 : 0, spread);
   return 1;
 }
 

@@ -253,11 +253,25 @@ class RedactionVault:
 
 # ------------------------------------------------------------------------------------- engine
 
+def credential_views(patterns: Sequence[dict]) -> Tuple[List[dict], List[int], List[int]]:
+    """One rule set for both engines of the redaction hooks: the registry's patterns, then every credential built-in the
+    configured categories left out.  -> (patterns of that set, the view of the registry's patterns, the view of the
+    credential built-ins in BUILTIN_RULES order -- credentialOnlyEngine's rules, src/redaction/hooks.ts:79-81)."""
+    ext = list(patterns)
+    have = {p["id"] for p in patterns if p["builtin"]}
+    for pid, cat, src, fl in BUILTIN_RULES:
+        if CATEGORY_ORDER[cat] == "credential" and pid not in have:
+            ext.append({"id": pid, "category": "credential", "source": src, "flags": fl, "builtin": True})
+    cred = {pid for pid, cat, _s, _f in BUILTIN_RULES if CATEGORY_ORDER[cat] == "credential"}
+    return ext, list(range(len(patterns))), [i for i, p in enumerate(ext) if p["builtin"] and p["id"] in cred]
+
+
 class RedactionEngine:
     """engine.ts:38-191."""
 
     def __init__(self, registry: PatternRegistry, vault: RedactionVault):
         self.registry, self.vault = registry, vault
+        self._views = None            # (rule set with the credential view, its patterns): scan_strings(credential_only=...)
 
     def scan_string(self, input: str):
         cats, count = set(), [0]
@@ -295,19 +309,34 @@ class RedactionEngine:
                 pass
         return self._redact_string(value, cats, count)
 
-    def scan_strings(self, inputs: Sequence[str]) -> List[dict]:
+    def scan_strings(self, inputs: Sequence[str], credential_only: Optional[Sequence[bool]] = None) -> List[dict]:
         """scanString (engine.ts:74-85) for many strings with the splice done on the device (cg_redact_batch): matches,
         SHA-256 of every match and the redacted text come back from one call; the vault learns the originals here, in the
         same loop as scan_string (_store_and_splice), so both give scanString's result.  A string is spliced on the host,
         with the placeholders the vault returned (vault.store runs once per match), when the vault issues its 12-digit form
         (another live value shares hash8, vault.ts:85-104), when the string has a lone surrogate or a match splits a
-        surrogate pair, or when several empty matches share a position (applyReplacements puts the last one first)."""
-        rs = self.registry._rs()
+        surrogate pair, or when several empty matches share a position (applyReplacements puts the last one first).
+
+        credential_only: one flag per string; a flagged string is scanned as credentialOnlyEngine scans an exempt tool's
+        output (the credential built-ins only, src/redaction/hooks.ts:79-81,176-178,218-222), the others as this engine
+        scans them -- in one call (cg_redact_batch_views), on one rule set with a view for each."""
+        patterns = self.registry.patterns
+        if credential_only is not None:
+            if self._views is None:
+                ext, full, cred = credential_views(self.registry.patterns)
+                rs = N.Ruleset([(p["source"], p["flags"], _CAT_ID[p["category"]]) for p in ext], strict=True)
+                rs.set_views([full, cred])
+                self._views = (rs, ext)
+            rs, patterns = self._views
+            views = np.array([1 if f else 0 for f in credential_only], dtype=np.uint8)
+            assert len(views) == len(inputs), "one credential_only flag per string"
+        else:
+            rs, views = self.registry._rs(), None
         if rs is None or not inputs:
             return [{"output": s, "redactionCount": 0, "categories": set()} for s in inputs]
         enc = [N.js_utf8(s) for s in inputs]
         data, off = N.pack(enc)
-        out, out_off, spans, digests = rs.redact_batch(data, off)
+        out, out_off, spans, digests = rs.redact_batch(data, off, views=views)
         res = [{"output": s, "redactionCount": 0, "categories": set()} for s in inputs]
         first = np.searchsorted(spans["msg"], np.arange(len(inputs) + 1)) if len(spans) else None
         for m in (np.unique(spans["msg"]) if len(spans) else ()):
@@ -315,7 +344,7 @@ class RedactionEngine:
             a, b = int(first[m]), int(first[m + 1])
             r = res[m]
             r["output"] = self._store_and_splice(inputs[m], enc[m], bytes(out[int(out_off[m]):int(out_off[m + 1])]), spans[a:b], digests[a:b],
-                                                 r["categories"], r)
+                                                 r["categories"], r, patterns)
         return res
 
     def _redact_string(self, input: str, cats, count) -> str:
@@ -330,7 +359,7 @@ class RedactionEngine:
         count[0] += counter["redactionCount"]
         return result
 
-    def _store_and_splice(self, s: str, enc: bytes, out: bytes, spans, digests, cats, counter: dict) -> str:
+    def _store_and_splice(self, s: str, enc: bytes, out: bytes, spans, digests, cats, counter: dict, patterns=None) -> str:
         """applyReplacements (engine.ts:165-181) for the resolved spans of one string s (enc = its UTF-8 bytes, out = the
         device's redacted bytes): vault.store for every match, last match first, with the device's SHA-256 of the match.
         The device text is the answer unless the vault issued a placeholder other than the default 8-digit one (another live
@@ -354,7 +383,7 @@ class RedactionEngine:
             else:                                                            # the device hashed other bytes than createHash() would
                 h = sha256_hex([match])[0]
                 device_text = False
-            cat = self.registry.patterns[int(sp["rule"])]["category"]
+            cat = (patterns or self.registry.patterns)[int(sp["rule"])]["category"]
             ph = self.vault.store(match, cat, h)
             device_text = device_text and ph == "[REDACTED:%s:%s]" % (cat, h[:8])
             reps.append((a, b, ph))
@@ -468,6 +497,7 @@ class MessagePolicy:
                 rules.append(r["messageContains"])
                 self.index.append((pi, ri))
         self.scanner = RuleScanner(rules, logger)
+        self._views_set = None        # the views last given to the rule set (verdict_batch with contexts)
 
     def evaluate_batch(self, texts: Sequence[str]) -> List[dict]:
         res = []
@@ -494,9 +524,13 @@ class MessagePolicy:
 
     ACTIONS = ("allow", "audit", "deny")
 
-    def verdict_batch(self, texts: Sequence[str]) -> List[dict]:
+    def verdict_batch(self, texts: Sequence[str], contexts: Optional[Sequence[dict]] = None) -> List[dict]:
         """Same action / reason as evaluate_batch, aggregated on the device (cg_policy_verdict_batch): one verdict word
-        per message comes back instead of the hit list (the `matches` list is not materialised)."""
+        per message comes back instead of the hit list (the `matches` list is not materialised).
+
+        contexts: one per text; then only the policies whose scope (excludeAgents, channels: matchesScope,
+        policy-evaluator.ts:18-26) admits the text's context take part -- one view per distinct in-scope policy set of the
+        batch (cg_policy_verdict_batch_views)."""
         rs = self.scanner.ruleset
         if rs is None or not texts:
             return [{"action": "allow", "reason": "No matching policies", "matchedPolicies": 0} for _ in texts]
@@ -508,9 +542,24 @@ class MessagePolicy:
                 pol.append(pi); act.append(self.ACTIONS.index(eff["action"]))
             rs.set_policy(pol, act)
             self._policy_set = True
-        data, off = N.pack([N.js_utf8(t) for t in texts])
+        if contexts is None:
+            data, off = N.pack([N.js_utf8(t) for t in texts])
+            words = rs.verdict_batch(data, off).tolist()
+        else:
+            assert len(contexts) == len(texts), "one context per text"
+            pattern_policy = [self.index[r][0] for r in self.scanner.rule_of_pattern]
+            views, ids = scope_views(self.policies, pattern_policy, contexts)
+            words = [0] * len(texts)
+            for v0 in range(0, len(views), 256):                # (at most 256 views per call)
+                sel = [i for i in range(len(texts)) if v0 <= ids[i] < v0 + 256]
+                if views[v0:v0 + 256] != self._views_set:        # (set_views waits for the stream and replaces the rows)
+                    rs.set_views(views[v0:v0 + 256])
+                    self._views_set = views[v0:v0 + 256]
+                data, off = N.pack([N.js_utf8(texts[i]) for i in sel])
+                for i, w in zip(sel, rs.verdict_batch(data, off, views=[ids[i] - v0 for i in sel]).tolist()):
+                    words[i] = w
         out = []
-        for v in rs.verdict_batch(data, off).tolist():
+        for v in words:
             action, matched, decide = self.ACTIONS[v & 3], (v >> 2) & 1023, v >> 12
             reason = "No matching policies" if action == "allow" else ""
             if decide != 0xfffff and action != "allow":
@@ -519,6 +568,23 @@ class MessagePolicy:
                 reason = eff.get("reason", "Denied by policy %s" % self.policies[pi]["id"]) if action == "deny" else eff.get("reason", "")
             out.append({"action": action, "reason": reason, "matchedPolicies": matched})
         return out
+
+
+def scope_views(policies: Sequence[dict], pattern_policy: Sequence[int], contexts: Sequence[dict]) -> Tuple[List[List[int]], List[int]]:
+    """The views of MessagePolicy.verdict_batch(texts, contexts): per context the policies its scope admits
+    (PolicyEvaluator._matches_scope), one view per distinct set in order of first appearance, holding the patterns
+    (pattern_policy[k] = policy of pattern k) of those policies.  -> (views, view id per context)"""
+    seen: Dict[Tuple[int, ...], int] = {}
+    views: List[List[int]] = []
+    ids: List[int] = []
+    for ctx in contexts:
+        key = tuple(pi for pi, p in enumerate(policies) if PolicyEvaluator._matches_scope(p, ctx))
+        if key not in seen:
+            seen[key] = len(views)
+            keep = set(key)
+            views.append([k for k, pi in enumerate(pattern_policy) if pi in keep])
+        ids.append(seen[key])
+    return views, ids
 
 
 # ------------------------------------------------------------------------------------- full policy slice
