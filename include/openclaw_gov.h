@@ -173,6 +173,12 @@ CG_API int cg_redact_one(cg_ruleset *rs, const uint8_t *bytes, uint32_t len, uin
 /* ---- device-resident variant (inputs/outputs already in HBM; used by bench.py `value` and by callers that pipeline
  * their own copies).  Pointers are CUDA device pointers; `stream` is a cudaStream_t (NULL = the library's own stream);
  * asynchronous w.r.t. the host, strictly in order on `stream`.
+ * Calls that share a rule set (every scan, hit-list, find-matches, redaction and verdict call on it: host-buffer,
+ * single-message or device-resident) run in the order they were issued, whatever stream each one is on: a call on another
+ * stream than the rule set's previous call waits for that call on the device, never on the host, and a blocking call returns
+ * after it.  So do the calls that share the library's digest scratch: cg_sha256_batch, cg_merkle_root[_fixed],
+ * cg_merkle_fold[_device], cg_merkle_block_roots_device, cg_merkle_root_sharded_device, the tree log's proof calls and the
+ * proof verifiers.  Other calls may overlap.
  * d_bytes must be 16-byte aligned and readable for 16 bytes past offsets[n] (padding; any content).
  * Queue capacities: a batch that overflows an internal queue (far more candidates than usual) cannot be re-run by the
  * library (the call has long returned).  Instead EVERY result word of that batch is set to 0xffffffffffffffff

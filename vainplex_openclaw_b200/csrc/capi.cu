@@ -24,6 +24,10 @@ namespace {
 thread_local std::string g_err;
 std::mutex g_mu;
 
+// Calls that share device scratch run in the order they were issued, whatever streams they are issued on.  A scratch keeps
+// the stream of the call that used it last and an event recorded there behind that use.
+struct IssueOrder { cudaEvent_t ev = nullptr; cudaStream_t last = nullptr; };
+
 struct Ctx {
   bool ready = false;
   int device = 0, sm_count = 132;
@@ -40,6 +44,7 @@ struct Ctx {
   uint64_t* d_off64 = nullptr; size_t cap_off64 = 0;
   uint64_t* d_words = nullptr; size_t cap_words = 0;
   uint32_t* d_dig[2] = {nullptr, nullptr}; size_t cap_dig[2] = {0, 0};
+  IssueOrder dig_order;           // the calls that use d_dig, on the library's stream or the caller's
   // chunked host-buffer scans: H2D of chunk c+1 and D2H of chunk c-1 overlap the kernels of chunk c
   static constexpr int kChunks = 8;
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr; cudaEvent_t e_h2d[kChunks] = {}, e_done[kChunks] = {}; uint32_t* h_chunk_counters = nullptr;
@@ -59,6 +64,23 @@ int cuda_fail(cudaError_t e, const char* what) {
 #define CU(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) return cuda_fail(_e, #x); } while (0)
 int require_ready() { return G.ready ? CG_OK : fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)"); }
 void count_launches(int k) { G.stats.kernel_launches += k; }
+
+// One call's use of a scratch on st, from before its first use (before anything is grown, captured, copied or launched) to
+// after its last: st first waits for the previous call's event when that call ran on another stream (rc: CG_OK or the
+// error), and the event is recorded on st when the scope ends.  A null order orders nothing (the call fails its argument
+// checks before it touches any scratch).
+class InOrder {
+ public:
+  InOrder(IssueOrder* o, cudaStream_t st) : o_(o), st_(st) {
+    if (o && o->last && o->last != st) { const cudaError_t e = cudaStreamWaitEvent(st, o->ev, 0); if (e != cudaSuccess) rc = cuda_fail(e, "cudaStreamWaitEvent"); }
+  }
+  ~InOrder() { if (o_) { cudaEventRecord(o_->ev, st_); o_->last = st_; } }
+  InOrder(const InOrder&) = delete;
+  InOrder& operator=(const InOrder&) = delete;
+  int rc = CG_OK;
+ private:
+  IssueOrder* o_; cudaStream_t st_;
+};
 
 // NCCL, bound at run time (nccl_load), and the communicator of cg_comm_init
 struct NcclApi {
@@ -106,6 +128,7 @@ struct cg_ruleset {
   std::vector<void*> allocs;
   uint32_t n_sets = 0, program_words = 0;
   ScanWork work{};
+  IssueOrder order;               // the calls that use work and one, on the library's stream or the caller's
   uint64_t seq = 0;               // device-path batches issued so far
   // device path: every batch's counters are mirrored into a ring of pinned slots, so that a queue overflow (results of
   // that batch marked incomplete by finalize_kernel) is seen by the next call / by cg_scan_join and the scratch grows
@@ -141,6 +164,7 @@ struct cg_ruleset {
     cudaFree(one.d_buf); cudaFree(one.d_pack);
     if (h_counters) cudaFreeHost(h_counters);
     for (auto& e : e_cnt) if (e) cudaEventDestroy(e);
+    if (order.ev) cudaEventDestroy(order.ev);
     for (void* p : allocs) cudaFree(p);
     cudaFree(work.heavy_idx); cudaFree(work.l1_pos); cudaFree(work.l1_fac); cudaFree(work.fq); cudaFree(work.slot_of_msg);
     cudaFree(work.counters); cudaFree(work.persist); cudaFree(work.slot_msg); cudaFree(work.cand); cudaFree(work.hit); cudaFree(work.events); cudaFree(work.event_pos); cudaFree(work.event_pre); cudaFree(work.spans);
@@ -386,6 +410,8 @@ int scan_host_chunked(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offs
   if ((rc = grow(&G.d_words, &G.cap_words, (size_t)n + 1))) return rc;
   if ((rc = ensure_copy_streams())) return rc;
   cudaStream_t st = G.stream;
+  InOrder turn(&rs->order, st);
+  if (turn.rc) return turn.rc;
   const uint32_t per = (n + C - 1) / C;
   CU(cudaStreamSynchronize(st));                            // (whatever still read the staging buffers is done: s_h2d does not wait for st)
   if ((rc = prepare_step(rs, per, kStepWords, st))) return rc;
@@ -522,7 +548,9 @@ int replay_step(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint
 template <typename After>
 int scan_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, uint64_t* d_words, StepKind kind, cudaStream_t st,
                 After&& after, bool graph = false, const ViewTable* views = nullptr) {
+  InOrder turn(&rs->order, st);
   int rc;
+  if ((rc = turn.rc)) return rc;
   if ((rc = ensure_mirrors(rs))) return rc;
   poll_mirrors(rs, false);                                  // (an earlier batch overflowed?  grow before this one runs)
   if ((rc = prepare_step(rs, n, kind, st))) return rc;
@@ -581,6 +609,7 @@ int cg_init(int device) {
   CU(cudaEventCreate(&G.ev0)); CU(cudaEventCreate(&G.ev1));
   for (int i = 0; i < 5; i++) CU(cudaEventCreate(&G.pev[i]));
   for (int i = 0; i < 8; i++) CU(cudaEventCreate(&G.pev_scan[i]));
+  CU(cudaEventCreateWithFlags(&G.dig_order.ev, cudaEventDisableTiming));
 
   G.ready = true;
   return CG_OK;
@@ -595,6 +624,7 @@ void cg_shutdown(void) {
   if (G.s_h2d) { cudaStreamDestroy(G.s_h2d); cudaStreamDestroy(G.s_d2h); for (int c = 0; c < Ctx::kChunks; c++) { cudaEventDestroy(G.e_h2d[c]); cudaEventDestroy(G.e_done[c]); } }
   cudaFree(G.d_bytes_raw); cudaFree(G.d_off32); cudaFree(G.d_off64); cudaFree(G.d_words); cudaFree(G.d_dig[0]); cudaFree(G.d_dig[1]);
   free_shard_roots();
+  cudaEventDestroy(G.dig_order.ev);
   cudaEventDestroy(G.ev0); cudaEventDestroy(G.ev1); for (int i = 0; i < 5; i++) cudaEventDestroy(G.pev[i]); for (int i = 0; i < 8; i++) cudaEventDestroy(G.pev_scan[i]); cudaStreamDestroy(G.stream);
   G = Ctx();
 }
@@ -650,6 +680,7 @@ int cg_ruleset_create(const cg_rule* rules, uint32_t n_rules, uint32_t options, 
   if (!out || (n_rules && !rules)) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (int rc = require_ready()) return rc;
   std::unique_ptr<cg_ruleset> rs(new cg_ruleset());
+  CU(cudaEventCreateWithFlags(&rs->order.ev, cudaEventDisableTiming));
   std::vector<RuleSrc> src(n_rules);
   rs->category.resize(n_rules);
   for (uint32_t i = 0; i < n_rules; i++) { src[i] = RuleSrc{rules[i].source, rules[i].source_len, rules[i].flags}; rs->category[i] = rules[i].category; }
@@ -785,6 +816,8 @@ int scan_batch_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offset
                     cg_hit* out_hits, uint32_t hits_cap, uint32_t* out_nhits, const uint8_t* views) {
   const bool want_hits = out_hits || out_nhits;
   cudaStream_t st = G.stream;
+  InOrder turn(rs ? &rs->order : nullptr, st);
+  if (turn.rc) return turn.rc;
   uint64_t total = 0;
   int rc = scan_host(rs, bytes, offsets, n, want_hits ? kStepPolicy : kStepWords, [&](const ScanWork& w) {
     if (!want_hits || !n) return CG_OK;
@@ -834,7 +867,9 @@ int scan_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* 
   if (off_ || !G.ready || !rs || (len && !bytes) || len > kOneBytes || rs->dev.rw > kOneRw - 2 || G.profiling) return 1;
   cg_ruleset::OnePath& o = rs->one;
   cudaStream_t st = G.stream;
+  InOrder turn(&rs->order, st);
   int rc;
+  if ((rc = turn.rc)) return rc;
   if ((rc = one_staging(o, false))) return rc;
   if ((rc = prepare_step(rs, 1, kStepWords, st))) return rc;
   const uint8_t* d_bytes = o.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(o.d_buf);
@@ -893,6 +928,8 @@ int resolve_staged(const ScanWork& w, uint32_t n, bool redact, uint64_t sizes[2]
 
 int find_matches_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans,
                       const uint8_t* views) {
+  InOrder turn(rs ? &rs->order : nullptr, G.stream);
+  if (turn.rc) return turn.rc;
   uint64_t sizes[2] = {0, 0}; uint32_t* d_dig = nullptr;
   int rc = scan_host(rs, bytes, offsets, n, kStepSpans, [&](const ScanWork& w) { return resolve_staged(w, n, false, sizes, &d_dig); }, views);
   if (rc) return rc;
@@ -958,6 +995,8 @@ int cg_ruleset_set_views(cg_ruleset* rs, const uint32_t* rows, uint32_t n_views)
 namespace {
 int verdict_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint32_t* out_verdicts, const uint8_t* views) {
   cudaStream_t st = G.stream;
+  InOrder turn(&rs->order, st);
+  if (turn.rc) return turn.rc;
   int rc = scan_host(rs, bytes, offsets, n, kStepWords, [&](const ScanWork& w) {
     if (!n) return CG_OK;
     int r;
@@ -994,6 +1033,8 @@ int redact_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, u
                 uint64_t* out_need, uint32_t* out_offsets, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans, uint8_t* out_digests32,
                 const uint8_t* views) {
   if (!out_offsets || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
+  InOrder turn(rs ? &rs->order : nullptr, G.stream);
+  if (turn.rc) return turn.rc;
   uint64_t sizes[2] = {0, 0}; uint32_t* d_dig = nullptr;
   int rc = scan_host(rs, bytes, offsets, n, kStepSpans, [&](const ScanWork& w) { return resolve_staged(w, n, true, sizes, &d_dig); }, views);
   if (rc) return rc;                                        // (input bytes / offsets stay in G.d_bytes / G.d_off32)
@@ -1045,7 +1086,9 @@ int span_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, bool redac
   if (!G.ready || !rs || !bytes || len > kOneBytes || G.profiling) return 1;
   cg_ruleset::OnePath& o = rs->one;
   cudaStream_t st = G.stream;
+  InOrder turn(&rs->order, st);
   int rc;
+  if ((rc = turn.rc)) return rc;
   if ((rc = one_staging(o, true))) return rc;
   if ((rc = prepare_step(rs, 1, kStepSpans, st))) return rc;
   const ScanWork& w = rs->work;
@@ -1283,11 +1326,13 @@ int cg_sha256_batch(const uint8_t* bytes, const uint64_t* offsets, uint32_t n, u
   if (int rc = require_ready()) return rc;
   if (!n) return CG_OK;
   if (!offsets || !out) return fail(CG_ERR_INVALID_ARG, "null argument");
+  cudaStream_t st = G.stream;
+  InOrder turn(&G.dig_order, st);
   size_t total = offsets[n]; int rc;
+  if ((rc = turn.rc)) return rc;
   if ((rc = grow_bytes(total + 64))) return rc;
   if ((rc = grow(&G.d_off64, &G.cap_off64, (size_t)n + 1))) return rc;
   if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)n * 8))) return rc;
-  cudaStream_t st = G.stream;
   if (total) CU(cudaMemcpyAsync(G.d_bytes, bytes, total, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(G.d_off64, offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
   int k = launch_sha256_batch(G.d_bytes, G.d_off64, n, (uint8_t*)G.d_dig[0], st);
@@ -1301,7 +1346,9 @@ int cg_sha256_batch(const uint8_t* bytes, const uint64_t* offsets, uint32_t n, u
 namespace {
 int empty_root(uint8_t out[32]) {
   // SHA-256("") -- computed by the same kernel, not on the CPU
+  InOrder turn(&G.dig_order, G.stream);
   int rc;
+  if ((rc = turn.rc)) return rc;
   if ((rc = grow(&G.d_off64, &G.cap_off64, 2))) return rc;
   if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], 8))) return rc;
   if ((rc = grow_bytes(64))) return rc;
@@ -1328,6 +1375,8 @@ int fold_dig(const uint32_t* d_nodes, uint64_t n, uint32_t max_levels, cudaStrea
 // root of n leaves in G.d_bytes (ragged at d_off, else leaf_len bytes each) -> host; leaves and fold time last_merkle_ms
 int staged_root(uint64_t n, const uint64_t* d_off, uint64_t leaf_len, uint8_t out_root[32]) {
   cudaStream_t st = G.stream; const uint32_t* d_root; int rc;
+  InOrder turn(&G.dig_order, st);
+  if ((rc = turn.rc)) return rc;
   if ((rc = size_dig(n))) return rc;
   CU(cudaEventRecord(G.ev0, st));
   count_launches(d_off ? launch_merkle_leaves_var(G.d_bytes, d_off, n, G.d_dig[0], st) : launch_merkle_leaves_fixed(G.d_bytes, leaf_len, n, G.d_dig[0], st));
@@ -1343,6 +1392,8 @@ int staged_root(uint64_t n, const uint64_t* d_off, uint64_t leaf_len, uint8_t ou
 // roots of the aligned 2^block_log2-leaf blocks of n fixed-size leaves in device memory -> d_roots (32 bytes per block)
 int block_roots(const void* d_bytes, uint64_t leaf_len, uint64_t n, uint32_t block_log2, void* d_roots, cudaStream_t st) {
   const uint32_t* d_res; int rc;
+  InOrder turn(&G.dig_order, st);
+  if ((rc = turn.rc)) return rc;
   if ((rc = size_dig(n))) return rc;
   count_launches(launch_merkle_leaves_fixed((const uint8_t*)d_bytes, leaf_len, n, G.d_dig[0], st)); G.stats.merkle_leaves += n;
   if ((rc = fold_dig(G.d_dig[0], n, block_log2, st, &d_res))) return rc;
@@ -1393,6 +1444,8 @@ int cg_merkle_fold(const uint8_t* nodes32, uint64_t m, uint8_t out_root[32]) {
   if (m == 0) return empty_root(out_root);
   if (!nodes32) return fail(CG_ERR_INVALID_ARG, "null argument");
   cudaStream_t st = G.stream; const uint32_t* d_root; int rc;
+  InOrder turn(&G.dig_order, st);
+  if ((rc = turn.rc)) return rc;
   if ((rc = size_dig(m))) return rc;
   CU(cudaMemcpyAsync(G.d_dig[0], nodes32, m * 32, cudaMemcpyHostToDevice, st));
   if ((rc = fold_dig(G.d_dig[0], m, 64, st, &d_root))) return rc;
@@ -1406,6 +1459,8 @@ int cg_merkle_fold_device(const void* d_nodes32, uint64_t m, void* d_out_root32,
   if (int rc = require_ready()) return rc;
   if (!m || !d_nodes32 || !d_out_root32) return fail(CG_ERR_INVALID_ARG, "null or empty input");
   cudaStream_t st = stream ? (cudaStream_t)stream : G.stream; const uint32_t* d_root; int rc;
+  InOrder turn(&G.dig_order, st);
+  if ((rc = turn.rc)) return rc;
   if ((rc = size_dig(m))) return rc;
   // the fold reads the nodes in place, unless they are off the 16-byte alignment of the kernels' loads: then from a copy
   const uint32_t* d_nodes = (const uint32_t*)d_nodes32;
@@ -1701,6 +1756,8 @@ std::vector<std::pair<uint64_t, uint64_t>> proof_ranges(uint64_t i, uint64_t siz
 int log_gather(cg_merkle_log* L, const uint64_t* h_idx, uint32_t m, uint64_t size, uint64_t first, uint8_t* out_paths32, uint32_t stride,
                uint32_t* out_lens) {
   cudaStream_t st = G.stream; int rc;
+  InOrder turn(&G.dig_order, st);
+  if ((rc = turn.rc)) return rc;
   const size_t path_words = (size_t)m * stride * 8, lens_words = ((size_t)m + 7) / 8 * 8;
   if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], path_words + lens_words))) return rc;
   if (h_idx && (rc = grow(&G.d_off64, &G.cap_off64, (size_t)m))) return rc;
@@ -1787,6 +1844,8 @@ int cg_merkle_verify_consistency(uint64_t first_size, uint64_t second_size, cons
   if (int rc = require_ready()) return rc;
   if (!out_ok || !root_first || !root_second || (path_len && !path32) || path_len > 64) return fail(CG_ERR_INVALID_ARG, "bad argument");
   int rc; cudaStream_t st = G.stream;
+  InOrder turn(&G.dig_order, st);
+  if ((rc = turn.rc)) return rc;
   if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)(path_len + 4) * 8))) return rc;
   uint32_t* d_r1 = G.d_dig[0]; uint32_t* d_r2 = d_r1 + 8; uint32_t* d_ok = d_r2 + 8; uint32_t* d_path = d_ok + 8;
   CU(cudaMemcpyAsync(d_r1, root_first, 32, cudaMemcpyHostToDevice, st));
@@ -1816,6 +1875,8 @@ int verify_proofs(const uint8_t* leaf_bytes, const uint64_t* leaf_offsets, const
   const size_t total = leaf_offsets[m];
   if (total && !leaf_bytes) return fail(CG_ERR_INVALID_ARG, "null argument");
   int rc; cudaStream_t st = G.stream;
+  InOrder turn(&G.dig_order, st);
+  if ((rc = turn.rc)) return rc;
   // d_dig[0]: leaf digests | root ; d_dig[1]: paths | indices | lengths | verdicts (every region a multiple of 32 bytes)
   const size_t leaf_words = (size_t)m * 8, path_words = (size_t)m * path_stride * 8, idx_words = ((size_t)m * 2 + 7) / 8 * 8,
                len_words = ((size_t)m + 7) / 8 * 8, ok_words = ((size_t)m + 31) / 32 * 8;
@@ -1945,6 +2006,8 @@ int cg_merkle_root_sharded_device(const void* d_bytes, uint64_t leaf_len, uint64
     if (!G.ready || g_nccl.d_roots != all) return fail(CG_ERR_NOT_INITIALIZED, "the library or the communicator's buffer changed during the all-gather");
   }
   const uint32_t* d_root;                                   // the fold's input: the gathered roots without the empty slots
+  InOrder turn(&G.dig_order, st);                           // (block_roots took its own turn: the lock was let go since)
+  if ((rc = turn.rc)) return rc;
   if ((rc = size_dig(total_blocks))) return rc;
   uint32_t* d = G.d_dig[0];
   for (int r = 0; r < world; r++) if (nblk[(size_t)r]) { CU(cudaMemcpyAsync(d, all + (size_t)r * max_blocks * 8, nblk[(size_t)r] * 32, cudaMemcpyDeviceToDevice, st)); d += nblk[(size_t)r] * 8; }
