@@ -65,11 +65,15 @@ __device__ __forceinline__ uint4 ldg_stream(const uint8_t* p) {
 }
 
 // ------------------------------------------------------------------------------------------
-// level 1: the gram filter.  Position-parallel: a lane owns 16 consecutive bytes of the batch buffer (LDG.128, the warp
-// reads 512 contiguous bytes), no per-message state, so long and ragged messages need no special handling.
+// level 1: the gram filter.  Position-parallel: a warp tile is 1 KB of the batch buffer made of two 512-byte halves; lane
+// l owns 16-byte chunk c = tile base + l of the first half and chunk c + 32 of the second (two LDG.128, each half one
+// coalesced 512-byte sweep), no per-message state, so long and ragged messages need no special handling.
 //   1a  every aligned 4-byte gram (stride 4) or every even-offset gram (stride 2) is folded SWAR-style, hashed with one
 //       IMAD and tested against the bitmap in shared memory (two bits of one word).  Result bits are funnel-shifted
 //       into a per-lane flag word; a warp ballot decides whether anything has to be looked at.
+//       Flag-word layout (flagged_gram_pos decodes it): a tile adds 2 * half_bits bits, its first half's probes above its
+//       second half's, probe 0 of a half highest; a round is as many tiles as fill 32 bits (two at stride 2, four at
+//       stride 4), the oldest tile highest, and the lane's queue entry carries its first-half chunk after the round.
 //   1b  lanes with flagged grams push (chunk, flag word) to a per-warp ring in shared memory, which goes to a queue in HBM
 //       32 entries at a time; confirm_kernel takes it from there (recheck map, level-1b lookup, exact factor, message).  Confirmed factor
 //       occurrences go to the queue in HBM, one atomic each (they are rare).
@@ -77,6 +81,21 @@ __device__ __forceinline__ uint4 ldg_stream(const uint8_t* p) {
 constexpr int kScanThreads = 1024;      // 32 warps, one CTA per SM
 constexpr uint32_t kRing = 64;          // (chunk, flag word) pairs a warp collects before it appends 32 of them to the queue in HBM
 constexpr uint32_t kScanRingBytes = (kScanThreads / 32) * kRing * 8;
+constexpr uint32_t kTileChunks = 64;    // 16-byte chunks per warp tile: two halves of 32
+// probe bits per 16-byte chunk = grams per chunk (stride 2: 8, stride 4: 4); tiles per round = 32 / (2 * half_bits)
+__host__ __device__ constexpr uint32_t half_bits(uint32_t nprobe) { return 4u * nprobe; }
+
+// the byte position of the gram behind bit `bit` of a flag word (scan_kernel's layout above).  newest = 16 x the lane's
+// first-half chunk in the round's last tile = 16 x (queued chunk - cstep); cstep16 = 16 x the chunks between a warp's
+// consecutive tiles (grid x warps per CTA x kTileChunks).  Probe j of a tile (first half first) is j = ~bit mod
+// 2 * half_bits; a chunk's probes are stride bytes apart, so every term is a shift or a mask of the bit number.
+template <int NPROBE>
+__device__ __forceinline__ uint32_t flagged_gram_pos(uint32_t newest, uint32_t bit, uint32_t cstep16) {
+  constexpr uint32_t hb = half_bits(NPROBE), lhb = NPROBE == 2 ? 3u : 2u, stride_shift = NPROBE == 2 ? 1u : 2u;
+  static_assert(hb == 1u << lhb && (hb << stride_shift) == 16u, "half_bits probes, stride bytes apart, cover one 16-byte chunk");
+  const uint32_t j = ~bit;
+  return newest - (bit >> (lhb + 1u)) * cstep16 + ((j >> lhb) & 1u) * (kTileChunks / 2u * 16u) + ((j & (hb - 1u)) << stride_shift);
+}
 
 __device__ __forceinline__ uint32_t lds_u32(uint32_t saddr) { uint32_t v; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(saddr)); return v; }
 
@@ -192,44 +211,44 @@ scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanW
   // folded (z domain) trigger bytes, splatted
   uint32_t splat0 = NTRIG > 0 ? (((rs.trig_byte[0] & 0x5fu) ^ 0x10u) * 0x01010101u) : 0u, splat1 = NTRIG > 1 ? (((rs.trig_byte[1] & 0x5fu) ^ 0x10u) * 0x01010101u) : 0u;
   asm volatile("" : "+r"(splat0), "+r"(splat1));
-  // this lane's chunk in the warp's current tile (32 chunks = 512 bytes); tiles are dealt round-robin to all warps of the grid
-  uint32_t c = first_chunk + (blockIdx.x * wpb + warp) * 32u + lane;
-  uint32_t cstep = gridDim.x * wpb * 32u;
-  uint32_t shl_bits = hk.one << (4u * NPROBE);
+  // this lane's first-half chunk in the warp's current tile (64 chunks = 1 KB); tiles are dealt round-robin to all warps of the grid
+  uint32_t c = first_chunk + (blockIdx.x * wpb + warp) * kTileChunks + lane;
+  uint32_t cstep = gridDim.x * wpb * kTileChunks;
+  uint32_t shl_bits = hk.one << half_bits(NPROBE);
   asm volatile("" : "+r"(end_chunk), "+r"(cstep), "+r"(shl_bits));
   const bool last_lane = lane == 31;
 
-  auto load_chunk = [&](uint4& v, uint32_t& t, uint32_t cc) {
-    v = make_uint4(0, 0, 0, 0); t = 0;
-    if (cc < end_chunk) v = ldg_stream(bytes + (size_t)cc * 16);
-    if (NPROBE == 2 && last_lane && cc + 1 < end_chunk) t = __ldg(reinterpret_cast<const uint32_t*>(bytes + (size_t)(cc + 1) * 16));
+  // a tile in registers: the lane's two chunks (c, c + 32) and, at stride 2, lane 31's first word of chunk c + 33
+  struct Tile { uint4 a, b; uint32_t t; };
+  auto load_tile = [&](Tile& v, uint32_t cc) {
+    v.a = make_uint4(0, 0, 0, 0); v.b = make_uint4(0, 0, 0, 0); v.t = 0;
+    if (cc < end_chunk) v.a = ldg_stream(bytes + (size_t)cc * 16);
+    if (cc + 32u < end_chunk) v.b = ldg_stream(bytes + (size_t)(cc + 32u) * 16);
+    if (NPROBE == 2 && last_lane && cc + 33u < end_chunk) v.t = __ldg(reinterpret_cast<const uint32_t*>(bytes + (size_t)(cc + 33u) * 16));
   };
-  // Four tiles per round through two register buffers, one tile ahead: tile k consumes one buffer and, as its first
-  // action after touching that data, issues the load of tile k + 1 into the other (dead since tile k - 1 folded it).
+  // Tiles go through two register buffers, one tile ahead: tile k consumes one buffer and, as its first action after
+  // touching that data, issues both loads of tile k + 1 into the other (dead since tile k - 1 folded it).  Both halves
+  // are issued together and needed together, so a tile keeps 1 KB per warp in flight behind ONE wait.
   // ptxas tracks every load of this loop on ONE scoreboard, and a wait on a scoreboard waits for everything issued on it:
-  // were the next load issued BEFORE the first use of the current data (where the scheduler hoists it if it may), each
-  // tile would wait for the load it has just issued -- the full HBM latency, exposed once per tile.  The address of the
-  // next load therefore depends on the current data (+ word * 0 with a run-time zero), which pins the order.  With
-  // eight warps per scheduler, "one tile ahead" is well over a thousand cycles.
-  // The probe results of the round's four tiles (4 x 8 bits at stride 2) are collected in one register per lane; after the
-  // round every lane with a non-zero flag word pushes (its chunk, the word) to ring 1 -- one ballot per round, no loop.
-  // Tiles past the end load zeros; whatever those flag is dropped by the position checks of the slow path.
-  constexpr uint32_t kBits = 4u * NPROBE;
+  // were the next loads issued BEFORE the first use of the current data (where the scheduler hoists them if it may), each
+  // tile would wait for the loads it has just issued -- the full HBM latency, exposed once per tile.  The address of the
+  // next tile therefore depends on the current data (+ word * 0 with a run-time zero), which pins the order.
+  // The probe results of a round's tiles (2 x 16 bits at stride 2, 4 x 8 at stride 4) are collected in one register per
+  // lane; after the round every lane with a non-zero flag word pushes (its chunk, the word) to ring 1 -- one ballot per
+  // round, no loop.  Halves past the end load zeros; whatever those flag is dropped by the position checks of the slow path.
+  constexpr uint32_t kTilesPerRound = 32u / (2u * half_bits(NPROBE));
+  static_assert(kTilesPerRound == 2 || kTilesPerRound == 4, "a round alternates the two buffers");
   uint32_t zero = hk.one - 1u;
   asm volatile("" : "+r"(zero));
-  uint4 bA, bB; uint32_t tA, tB;
-  load_chunk(bA, tA, c); bB = make_uint4(0, 0, 0, 0); tB = 0;
+  Tile tA, tB;
+  load_tile(tA, c); tB.a = make_uint4(0, 0, 0, 0); tB.b = tB.a; tB.t = 0;
   uint32_t acc = 0;
-  auto scan_tile = [&](const uint4& buf, const uint32_t& tl, uint4& nbuf, uint32_t& ntl, uint32_t cc) {
-    const uint4 cur = buf; const uint32_t ct = tl;
-    uint32_t ncc = cc + cstep;
-    asm volatile("mad.lo.u32 %0, %1, %2, %0;" : "+r"(ncc) : "r"(cur.x), "r"(zero));       // (waits for the current tile's data)
-    load_chunk(nbuf, ntl, ncc);
+  // the probes and trigger test of one 16-byte chunk (chunk number cc); w4 = the first word of chunk cc + 1 (stride 2)
+  auto scan_half = [&](const uint4& cur, uint32_t w4, uint32_t cc) {
     const uint32_t z0 = fold_z(cur.x, hk), z1 = fold_z(cur.y, hk), z2 = fold_z(cur.z, hk), z3 = fold_z(cur.w, hk);
     const uint32_t f0 = fold_key(z0, hk), f1 = fold_key(z1, hk), f2 = fold_key(z2, hk), f3 = fold_key(z3, hk);
     uint32_t flags = 0;
     if (NPROBE == 2) {
-      uint32_t w4 = __shfl_down_sync(FULL, cur.x, 1); if (last_lane) w4 = ct;
       const uint32_t f4 = fold_key(fold_z(w4, hk), hk);
       gram_probe<BLOOM2>(bm, hk, f0, flags); gram_probe<BLOOM2>(bm, hk, __funnelshift_r(f0, f1, 16), flags);
       gram_probe<BLOOM2>(bm, hk, f1, flags); gram_probe<BLOOM2>(bm, hk, __funnelshift_r(f1, f2, 16), flags);
@@ -239,7 +258,7 @@ scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanW
       gram_probe<BLOOM2>(bm, hk, f0, flags); gram_probe<BLOOM2>(bm, hk, f1, flags);
       gram_probe<BLOOM2>(bm, hk, f2, flags); gram_probe<BLOOM2>(bm, hk, f3, flags);
     }
-    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(acc) : "r"(acc), "r"(shl_bits), "r"(flags));      // acc = acc << kBits | flags, on the FMA pipe
+    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(acc) : "r"(acc), "r"(shl_bits), "r"(flags));      // acc = acc << half_bits | flags, on the FMA pipe
     if (NTRIG > 0) {
       // triggers: d_j has bit 7 of a byte clear where it equals a trigger byte (folded domain)
       uint32_t d0 = differs(z0, splat0, hk.one), d1 = differs(z1, splat0, hk.one), d2 = differs(z2, splat0, hk.one), d3 = differs(z3, splat0, hk.one);
@@ -250,6 +269,21 @@ scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanW
         __syncwarp();
       }
     }
+  };
+  auto scan_tile = [&](const Tile& buf, Tile& nbuf, uint32_t cc) {
+    const Tile cur = buf;
+    uint32_t ncc = cc + cstep;
+    asm volatile("mad.lo.u32 %0, %1, %2, %0;" : "+r"(ncc) : "r"(cur.a.x), "r"(zero));     // (waits for the current tile's data)
+    load_tile(nbuf, ncc);
+    uint32_t wa = 0, wb = 0;
+    if (NPROBE == 2) {
+      // the odd grams' fifth word: first half, chunk cc + 1 = the next lane's first-half word, for lane 31 lane 0's
+      // second-half word (chunk tile base + 32); second half, the next lane's second-half word, for lane 31 chunk cc + 33
+      wa = __shfl_sync(FULL, lane == 0 ? cur.b.x : cur.a.x, (lane + 1u) & 31u);
+      wb = __shfl_down_sync(FULL, cur.b.x, 1); if (last_lane) wb = cur.t;
+    }
+    scan_half(cur.a, wa, cc);
+    scan_half(cur.b, wb, cc + 32u);
   };
   // Nothing is done about a flagged gram here: looking at one means a chain of dependent loads (the gram again, the
   // recheck map, the level-1b bucket, the factor, the text around it), and with 32 warps per SM there is nobody to hide
@@ -269,12 +303,14 @@ scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanW
   };
 #pragma unroll 1
   while (c - lane < end_chunk) {                           // warp-uniform: this warp still has a tile
-    scan_tile(bA, tA, bB, tB, c);
-    scan_tile(bB, tB, bA, tA, c + cstep);
-    scan_tile(bA, tA, bB, tB, c + 2u * cstep);
-    scan_tile(bB, tB, bA, tA, c + 3u * cstep);
-    c += 4u * cstep;
-    // acc: bit (i * kBits + kBits - 1 - j) = probe j of the tile scanned i tiles ago, whose chunk was c - (i + 1) * cstep
+    scan_tile(tA, tB, c);
+    scan_tile(tB, tA, c + cstep);
+    if (kTilesPerRound == 4) {
+      scan_tile(tA, tB, c + 2u * cstep);
+      scan_tile(tB, tA, c + 3u * cstep);
+    }
+    c += kTilesPerRound * cstep;
+    // acc: flagged_gram_pos<NPROBE>((c - cstep) * 16, bit, cstep * 16) is the gram behind each set bit
     const uint32_t m = __ballot_sync(FULL, acc != 0);
     if (m) {
       if (acc) asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(ring1 + (((t1 + __popc(m & lt)) & (kRing - 1)) << 3)), "r"(c), "r"(acc) : "memory");
@@ -484,10 +520,12 @@ __device__ __forceinline__ void confirm_gram(ConfirmCtx& c, uint32_t pos, bool a
   }
 }
 
+// NPROBE as scan_kernel's: the flag-word decode is a handful of shifts and masks per bit (flagged_gram_pos)
+template <int NPROBE>
 __global__ void __launch_bounds__(kCfThreads, 1)
 confirm_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, uint32_t cstep) {
   extern __shared__ __align__(16) uint8_t cf_smem[];          // [pair rings][gram rings][tables, when resident]
-  const uint32_t kbits = rs.stride == 2 ? 8u : 4u, kshift = rs.stride == 2 ? 1u : 2u;
+  const uint32_t cstep16 = cstep * 16u;
   const uint32_t nq = (rs.debug_flags & 1u) ? 0u : min(w.counters[kCtrFlagWords + w.q_slot], w.q_cap);
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5, FULL = 0xffffffffu, lt = (1u << lane) - 1u;
   uint2* pring = reinterpret_cast<uint2*>(cf_smem) + warp * kCfRing;
@@ -510,12 +548,13 @@ confirm_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ Sc
     if (base + lane < nq) q = w.fq[base + lane];
     // flag bits -> gram positions, one wave per bit rank (the k-th set bit of every lane's word): at most 32 new positions a wave
     uint32_t bits = q.y;
+    const uint32_t newest = (q.x - cstep) * 16u;
     for (;;) {
       const uint32_t m = __ballot_sync(FULL, bits != 0);
       if (!m) break;
       if (bits) {
         const uint32_t bit = (uint32_t)__ffs((int)bits) - 1u; bits &= bits - 1u;
-        ring[(tail + __popc(m & lt)) & (kCfRing - 1)] = ((q.x - (bit / kbits + 1u) * cstep) * kbits + (kbits - 1u - bit % kbits)) << kshift;
+        ring[(tail + __popc(m & lt)) & (kCfRing - 1)] = flagged_gram_pos<NPROBE>(newest, bit, cstep16);
       }
       tail += __popc(m); flagged += lane == 0 ? __popc(m) : 0u;
       __syncwarp();
@@ -824,7 +863,8 @@ void prepare_scan_kernels() {
   cudaFuncSetAttribute(scan_kernel<P, T, B, 768>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem); cudaFuncSetAttribute(scan_kernel<P, T, B, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
   CG_FOR_SCAN_VARIANTS(CG_PREP)
 #undef CG_PREP
-  cudaFuncSetAttribute(confirm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kCfRingBytes + kConfirmTableBudget));
+  cudaFuncSetAttribute(confirm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kCfRingBytes + kConfirmTableBudget));
+  cudaFuncSetAttribute(confirm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kCfRingBytes + kConfirmTableBudget));
   cudaFuncSetAttribute(verify_small_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVerifySmem);
   cudaFuncSetAttribute(verify_small_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kVerifySmem);
 }
@@ -839,7 +879,7 @@ int launch_scan(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes,
                 uint64_t* d_words, int sm_count, cudaStream_t stream) {
   if (n == 0) return 0;
   const size_t smem = (size_t)rs.image_bytes + kScanRingBytes;
-  // the scanned range is only known on the device (off[0] .. off[n]); a warp tile is 512 bytes, messages are rarely shorter than 16
+  // the scanned range is only known on the device (off[0] .. off[n]); a warp tile is 1 KB, messages are rarely shorter than 16
   const uint32_t grid = scan_grid(n, sm_count);
   const int np = rs.stride == 2 ? 2 : 1, nt = (int)rs.n_trig, bl = rs.bloom2 ? 1 : 0, th = scan_threads();
 #define CG_LAUNCH(P, T, B) if (np == P && nt == T && bl == B) { \
@@ -853,8 +893,10 @@ int launch_scan(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes,
 
 int launch_confirm(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, int sm_count, cudaStream_t stream) {
   if (n == 0) return 0;
-  const uint32_t cstep = scan_grid(n, sm_count) * (uint32_t)(scan_threads() / 32) * 32u;       // (the queue's chunk numbers are decoded with the scan's grid)
-  confirm_kernel<<<scan_grid(n, sm_count), kCfThreads, (size_t)kCfRingBytes + (rs.cf_resident ? rs.cf_bytes : 0u), stream>>>(rs, w, d_bytes, d_off, n, cstep);
+  const uint32_t cstep = scan_grid(n, sm_count) * (uint32_t)(scan_threads() / 32) * kTileChunks;       // (the queue's chunk numbers are decoded with the scan's grid)
+  const size_t smem = (size_t)kCfRingBytes + (rs.cf_resident ? rs.cf_bytes : 0u);
+  if (rs.stride == 2) confirm_kernel<2><<<scan_grid(n, sm_count), kCfThreads, smem, stream>>>(rs, w, d_bytes, d_off, n, cstep);
+  else confirm_kernel<1><<<scan_grid(n, sm_count), kCfThreads, smem, stream>>>(rs, w, d_bytes, d_off, n, cstep);
   return 1;
 }
 int launch_resolve(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, bool want_spans, int sm_count, cudaStream_t stream,
