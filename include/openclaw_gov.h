@@ -177,8 +177,10 @@ CG_API int cg_redact_one(cg_ruleset *rs, const uint8_t *bytes, uint32_t len, uin
  * single-message or device-resident) run in the order they were issued, whatever stream each one is on: a call on another
  * stream than the rule set's previous call waits for that call on the device, never on the host, and a blocking call returns
  * after it.  So do the calls that share the library's digest scratch: cg_sha256_batch, cg_merkle_root[_fixed],
- * cg_merkle_fold[_device], cg_merkle_block_roots_device, cg_merkle_root_sharded_device, the tree log's proof calls and the
- * proof verifiers.  Other calls may overlap.
+ * cg_merkle_fold[_device], cg_merkle_block_roots_device, cg_merkle_root_sharded_device, the tree log's proof calls (host-buffer
+ * and device-resident), the proof verifiers (cg_merkle_verify_proofs[_device], cg_merkle_verify_proof,
+ * cg_merkle_verify_consistency).  So do the calls on one Merkle log (every cg_merkle_log_* call on it
+ * but _size and _destroy, host-buffer or device-resident).  Other calls may overlap.
  * d_bytes must be 16-byte aligned and readable for 16 bytes past offsets[n] (padding; any content).
  * Queue capacities: a batch that overflows an internal queue (far more candidates than usual) cannot be re-run by the
  * library (the call has long returned).  Instead EVERY result word of that batch is set to 0xffffffffffffffff
@@ -313,7 +315,9 @@ CG_API void cg_merkle_log_destroy(cg_merkle_log *log);
 CG_API int cg_merkle_log_append(cg_merkle_log *log, const uint8_t *bytes, const uint64_t *offsets, uint64_t n);   /* host buffers */
 /* the day file itself (src/audit-trail.ts:151-179: JSON lines joined with "\n", trailing "\n" per flush): split at '\n' on the
  * device, every line without its '\n' is one leaf (an unterminated last line counts); *out_lines = leaves appended */
-/* capacity for n_leaves more leaves / n_bytes of leaf bytes per append, allocated now instead of by the appends */
+/* capacity for n_leaves more leaves / n_bytes of leaf bytes per append, allocated now instead of by the appends.  On a log
+ * without a node store (cg_merkle_log_create) this includes the buffers that fold a block of up to n_leaves leaves: 24 bytes per
+ * leaf on top of the 32 of a kept leaf digest (a tree log folds into its store and needs none). */
 CG_API int cg_merkle_log_reserve(cg_merkle_log *log, uint64_t n_leaves, uint64_t n_bytes);
 CG_API int cg_merkle_log_append_jsonl(cg_merkle_log *log, const uint8_t *bytes, uint64_t len, uint64_t *out_lines);
 CG_API int cg_merkle_log_size(const cg_merkle_log *log, uint64_t *out_n);
@@ -357,6 +361,43 @@ CG_API int cg_merkle_log_consistency_between(cg_merkle_log *log, uint64_t first_
 CG_API int cg_merkle_verify_proofs(const uint8_t *leaf_bytes, const uint64_t *leaf_offsets, const uint64_t *indices, uint32_t m,
                                    uint64_t tree_size, const uint8_t *paths32, uint32_t path_stride, const uint32_t *path_lens,
                                    const uint8_t root[32], uint8_t *out_ok);
+
+/* ---- device-resident Merkle log calls: leaves, indices, paths and verdicts already in HBM (event records a caller built on the
+ * device, proofs served to or checked for a consumer on the device).  Each call writes exactly what its host twin returns --
+ * the same roots, frontier, node store, path bytes, lengths and verdicts -- and touches only the caller's device buffers and the
+ * log's or the library's scratch.  Asynchronous on `stream` (NULL = the library's stream): a call waits on the host only when a
+ * log or library buffer has to grow (cg_merkle_log_reserve sizes the log's buffers up front).  Calls on one log run in the order
+ * they were issued, host-buffer and device-resident alike, whatever stream each is on; calls on different logs overlap.
+ * cg_merkle_log_size counts the leaves enqueued so far.  Every argument the host can see is checked as the host twin checks it,
+ * and pointer alignment too, before anything is enqueued (CG_ERR_INVALID_ARG): ragged byte buffers 16-byte aligned and readable
+ * 16 bytes past their last offset, paths 16-byte aligned, offsets and indices 8-byte, lengths 4-byte.  What only the device can
+ * see is checked in band, per item, leaving the other items alone: */
+/* leaf i = d_bytes[d_offsets[i], d_offsets[i+1]) (uint64 offsets).  A decreasing pair goes in as the empty leaf without being
+ * read and marks the log: cg_merkle_log_join reports CG_ERR_INVALID_ARG once, and from then on every call on the log but
+ * _size and _destroy returns CG_ERR_INVALID_ARG (a log that holds a wrong leaf must not keep going quietly). */
+CG_API int cg_merkle_log_append_device(cg_merkle_log *log, const void *d_bytes, const void *d_offsets /* uint64[m+1] */,
+                                       uint64_t m, void *stream);
+/* m leaves of leaf_len bytes each at d_bytes, any alignment (the leaves and kernels of cg_merkle_block_roots_device, e.g.
+ * fixed-size event records) */
+CG_API int cg_merkle_log_append_fixed_device(cg_merkle_log *log, const void *d_bytes, uint64_t leaf_len, uint64_t m, void *stream);
+/* cg_merkle_log_root into 32 bytes of HBM (any alignment) */
+CG_API int cg_merkle_log_root_device(cg_merkle_log *log, void *d_out_root32, void *stream);
+/* cg_merkle_log_proofs from and into HBM (the same argument checks); an index >= tree_size gets length 0xffffffff and an
+ * all-zero stride */
+CG_API int cg_merkle_log_proofs_device(cg_merkle_log *log, const void *d_indices /* uint64[m] */, uint32_t m, uint64_t tree_size,
+                                       void *d_out_paths32, uint32_t path_stride, void *d_out_lens /* uint32[m] */, void *stream);
+/* cg_merkle_log_consistency_between into HBM: the path's digests at d_out_path32, its length (uint32) at *d_out_len */
+CG_API int cg_merkle_log_consistency_between_device(cg_merkle_log *log, uint64_t first_size, uint64_t second_size,
+                                                    void *d_out_path32, uint32_t path_cap, void *d_out_len, void *stream);
+/* cg_merkle_verify_proofs from and into HBM (leaves ragged as for cg_merkle_log_append_device, root: 32 bytes, any alignment,
+ * d_out_ok: one uint8 per proof).  A decreasing leaf offset pair, a path length above 64 or above path_stride, or an index >=
+ * tree_size gives ok = 0 without reading that leaf or path. */
+CG_API int cg_merkle_verify_proofs_device(const void *d_leaf_bytes, const void *d_leaf_offsets, const void *d_indices, uint32_t m,
+                                          uint64_t tree_size, const void *d_paths32, uint32_t path_stride, const void *d_path_lens,
+                                          const void *d_root32, void *d_out_ok, void *stream);
+/* waits for `stream` and for every call issued on the log; CG_ERR_INVALID_ARG (once, then on every call) when a device append
+ * read a decreasing offset pair, else CG_OK */
+CG_API int cg_merkle_log_join(cg_merkle_log *log, void *stream);
 
 #ifdef __cplusplus
 }

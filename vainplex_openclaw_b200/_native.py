@@ -60,7 +60,9 @@ EXPORTS = ["cg_init", "cg_shutdown", "cg_last_error", "cg_version", "cg_device_c
            "cg_merkle_log_create_tree", "cg_merkle_log_proofs", "cg_merkle_log_consistency_between", "cg_merkle_verify_proofs",
            "cg_ruleset_set_views", "cg_scan_batch_views", "cg_find_matches_batch_views", "cg_redact_batch_views",
            "cg_policy_verdict_batch_views", "cg_scan_hits_batch_device_views", "cg_find_matches_batch_device_views",
-           "cg_redact_batch_device_views", "cg_policy_verdict_batch_device_views"]
+           "cg_redact_batch_device_views", "cg_policy_verdict_batch_device_views",
+           "cg_merkle_log_append_device", "cg_merkle_log_append_fixed_device", "cg_merkle_log_root_device", "cg_merkle_log_proofs_device",
+           "cg_merkle_log_consistency_between_device", "cg_merkle_verify_proofs_device", "cg_merkle_log_join"]
 
 _lib = None
 
@@ -147,6 +149,13 @@ def load():
     L.cg_find_matches_batch_device_views.argtypes = [vp, vp, vp, vp, u32, vp, u32, vp, vp]; L.cg_find_matches_batch_device_views.restype = i32
     L.cg_redact_batch_device_views.argtypes = [vp, vp, vp, vp, u32, vp, u64, vp, vp, u32, vp, vp, vp]; L.cg_redact_batch_device_views.restype = i32
     L.cg_policy_verdict_batch_device_views.argtypes = [vp, vp, vp, vp, u32, vp, vp]; L.cg_policy_verdict_batch_device_views.restype = i32
+    L.cg_merkle_log_append_device.argtypes = [vp, vp, vp, u64, vp]; L.cg_merkle_log_append_device.restype = i32
+    L.cg_merkle_log_append_fixed_device.argtypes = [vp, vp, u64, u64, vp]; L.cg_merkle_log_append_fixed_device.restype = i32
+    L.cg_merkle_log_root_device.argtypes = [vp, vp, vp]; L.cg_merkle_log_root_device.restype = i32
+    L.cg_merkle_log_proofs_device.argtypes = [vp, vp, u32, u64, vp, u32, vp, vp]; L.cg_merkle_log_proofs_device.restype = i32
+    L.cg_merkle_log_consistency_between_device.argtypes = [vp, u64, u64, vp, u32, vp, vp]; L.cg_merkle_log_consistency_between_device.restype = i32
+    L.cg_merkle_verify_proofs_device.argtypes = [vp, vp, vp, u32, u64, vp, u32, vp, vp, vp, vp]; L.cg_merkle_verify_proofs_device.restype = i32
+    L.cg_merkle_log_join.argtypes = [vp, vp]; L.cg_merkle_log_join.restype = i32
     _lib = L
     return L
 
@@ -595,6 +604,34 @@ class MerkleLog:
         check(load().cg_merkle_log_consistency_between(self.handle, first_size, second_size, out.ctypes.data, 65, C.byref(k)))
         return [out[i].tobytes() for i in range(k.value)]
 
+    # device-resident twins: integer device pointers, asynchronous on `stream` (a cudaStream_t as an integer, 0 = the library's
+    # stream); their in-band status comes from join
+    def append_device(self, d_bytes: int, d_off: int, m: int, stream: int = 0):
+        """cg_merkle_log_append_device: leaf i = d_bytes[d_off[i], d_off[i+1]) (uint64 offsets in HBM)."""
+        check(load().cg_merkle_log_append_device(self.handle, d_bytes or None, d_off or None, m, stream))
+
+    def append_fixed_device(self, d_bytes: int, leaf_len: int, m: int, stream: int = 0):
+        """cg_merkle_log_append_fixed_device: m leaves of leaf_len bytes each at d_bytes."""
+        check(load().cg_merkle_log_append_fixed_device(self.handle, d_bytes or None, leaf_len, m, stream))
+
+    def root_device(self, d_root: int, stream: int = 0):
+        """cg_merkle_log_root_device: the root into 32 bytes at d_root."""
+        check(load().cg_merkle_log_root_device(self.handle, d_root or None, stream))
+
+    def proofs_device(self, d_idx: int, m: int, tree_size: int, d_paths: int, stride: int, d_lens: int, stream: int = 0):
+        """cg_merkle_log_proofs_device: paths of the m leaves at d_idx (uint64) into d_paths (stride digests each), lengths
+        (uint32) into d_lens; an index >= tree_size gets length 0xffffffff and a zero stride."""
+        check(load().cg_merkle_log_proofs_device(self.handle, d_idx or None, m, tree_size, d_paths or None, stride, d_lens or None, stream))
+
+    def consistency_between_device(self, first_size: int, second_size: int, d_path: int, path_cap: int, d_len: int, stream: int = 0):
+        """cg_merkle_log_consistency_between_device: the proof's digests into d_path, its length (uint32) into d_len."""
+        check(load().cg_merkle_log_consistency_between_device(self.handle, first_size, second_size, d_path or None, path_cap, d_len or None, stream))
+
+    def join(self, stream: int = 0):
+        """cg_merkle_log_join: wait for `stream` and every call on the log; raises GovError(INVALID_ARG) once a device append
+        read a decreasing offset pair (and on every call after that)."""
+        check(load().cg_merkle_log_join(self.handle, stream))
+
     def close(self):
         if self.handle:
             load().cg_merkle_log_destroy(self.handle)
@@ -672,3 +709,13 @@ def merkle_verify_proofs(leaves, indices, tree_size: int, paths, root: bytes) ->
     check(load().cg_merkle_verify_proofs(data.ctypes.data, off.ctypes.data, idx.ctypes.data, m, tree_size, p.ctypes.data, p.shape[1],
                                          lens.ctypes.data, r.ctypes.data, ok.ctypes.data))
     return ok[:m].astype(bool)
+
+
+def merkle_verify_proofs_device(d_bytes: int, d_off: int, d_idx: int, m: int, tree_size: int, d_paths: int, stride: int, d_lens: int,
+                                d_root: int, d_ok: int, stream: int = 0):
+    """cg_merkle_verify_proofs_device on integer device pointers (asynchronous on `stream`): one uint8 verdict per proof into d_ok.
+    A decreasing leaf offset pair, a path length above min(64, stride) or an index >= tree_size gives 0."""
+    if not _inited:
+        init()
+    check(load().cg_merkle_verify_proofs_device(d_bytes or None, d_off or None, d_idx or None, m, tree_size, d_paths or None, stride,
+                                                d_lens or None, d_root or None, d_ok or None, stream))

@@ -1485,9 +1485,15 @@ struct cg_merkle_log {
   bool tree = false;
   uint32_t* d_lvl[64] = {}; uint64_t cap_lvl[64] = {};
   uint32_t* d_spine = nullptr;
+  IssueOrder order;               // every call on the log, host-buffer or device-resident, on the library's stream or the caller's
+  // set by the device when an append read a decreasing offset pair (that leaf went in as the empty leaf); cg_merkle_log_join
+  // reports it once and from then on the log refuses every call (failed)
+  uint32_t* d_err = nullptr;
+  bool failed = false;
   ~cg_merkle_log() {
-    cudaFree(d_slots); cudaFree(d_tmp); cudaFree(d_leaves); cudaFree(d_new); cudaFree(d_a); cudaFree(d_b); cudaFree(d_spine);
+    cudaFree(d_slots); cudaFree(d_tmp); cudaFree(d_leaves); cudaFree(d_new); cudaFree(d_a); cudaFree(d_b); cudaFree(d_spine); cudaFree(d_err);
     for (uint32_t* p : d_lvl) cudaFree(p);
+    if (order.ev) cudaEventDestroy(order.ev);
   }
 };
 
@@ -1510,6 +1516,7 @@ int log_range_root(cg_merkle_log* L, const uint32_t* d_in, uint64_t cnt, uint32_
 int log_check(cg_merkle_log* L) {
   if (int rc = require_ready()) return rc;
   if (!L) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (L->failed) return fail(CG_ERR_INVALID_ARG, "a device append put a leaf with a decreasing offset pair into this log (reported by cg_merkle_log_join): it refuses every call");
   return CG_OK;
 }
 // root of the current tree -> d_tmp[64]
@@ -1529,8 +1536,9 @@ int log_new(cg_merkle_log** out, bool keep, bool tree) {
   if (!out) return fail(CG_ERR_INVALID_ARG, "null argument");
   std::unique_ptr<cg_merkle_log> L(new cg_merkle_log());
   L->keep = keep; L->tree = tree;
-  CU(cudaMalloc((void**)&L->d_slots, 64 * 32)); CU(cudaMalloc((void**)&L->d_tmp, 65 * 32));
-  CU(cudaMemset(L->d_slots, 0, 64 * 32));
+  CU(cudaMalloc((void**)&L->d_slots, 64 * 32)); CU(cudaMalloc((void**)&L->d_tmp, 65 * 32)); CU(cudaMalloc((void**)&L->d_err, 4));
+  CU(cudaMemset(L->d_slots, 0, 64 * 32)); CU(cudaMemset(L->d_err, 0, 4));
+  CU(cudaEventCreateWithFlags(&L->order.ev, cudaEventDisableTiming));
   if (tree) CU(cudaMalloc((void**)&L->d_spine, 64 * 32));
   *out = L.release();
   return CG_OK;
@@ -1546,7 +1554,10 @@ int cg_merkle_log_create_tree(cg_merkle_log** out) {
   std::lock_guard<std::mutex> lk(g_mu);
   return log_new(out, true, true);
 }
-void cg_merkle_log_destroy(cg_merkle_log* L) { std::lock_guard<std::mutex> lk(g_mu); if (L) { if (G.ready) cudaStreamSynchronize(G.stream); delete L; } }
+void cg_merkle_log_destroy(cg_merkle_log* L) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (L) { if (G.ready) { cudaStreamSynchronize(G.stream); cudaEventSynchronize(L->order.ev); } delete L; }
+}
 int cg_merkle_log_size(const cg_merkle_log* L, uint64_t* out_n) { if (!L || !out_n) return fail(CG_ERR_INVALID_ARG, "null argument"); *out_n = L->n; return CG_OK; }
 
 int cg_merkle_log_restore(cg_merkle_log** out, uint64_t n, const uint8_t* frontier32, uint32_t count) {
@@ -1564,6 +1575,8 @@ int cg_merkle_log_frontier(cg_merkle_log* L, uint8_t* out_frontier32, uint32_t* 
   std::lock_guard<std::mutex> lk(g_mu);
   int rc = log_check(L); if (rc) return rc;
   if (!out_count) return fail(CG_ERR_INVALID_ARG, "null argument");
+  InOrder turn(&L->order, G.stream);
+  if ((rc = turn.rc)) return rc;
   uint32_t k = 0;
   for (int h = 63; h >= 0; h--) if ((L->n >> h) & 1ull) { if (out_frontier32) CU(cudaMemcpyAsync(out_frontier32 + 32 * (size_t)k, L->d_slots + 8 * h, 32, cudaMemcpyDeviceToHost, G.stream)); k++; }
   CU(cudaStreamSynchronize(G.stream));
@@ -1600,8 +1613,10 @@ int log_digest_room(cg_merkle_log* L, uint64_t m, cudaStream_t st, uint32_t** ou
 }
 // m new leaf digests at d_dig: cut [n, n+m) into aligned perfect blocks (block size <= lowest set bit of its position),
 // reduce each, carry into the frontier.  On a tree log the block's fold writes its levels into the store (its root is node
-// (h, pos >> h)) and every carry makes the complete node (top, pos >> top) under the next occupied slot.
-int log_absorb(cg_merkle_log* L, const uint32_t* d_dig, uint64_t m, cudaStream_t st) {
+// (h, pos >> h)) and every carry makes the complete node (top, pos >> top) under the next occupied slot.  The plan depends on
+// n and m only; with wait the host waits for st before the log counts the leaves (host-buffer appends), without it the
+// launches stay in flight (device-resident appends: the size counts enqueued leaves).
+int log_absorb(cg_merkle_log* L, const uint32_t* d_dig, uint64_t m, cudaStream_t st, bool wait = true) {
   int rc;
   uint64_t pos = L->n, rem = m;
   while (rem) {
@@ -1620,19 +1635,23 @@ int log_absorb(cg_merkle_log* L, const uint32_t* d_dig, uint64_t m, cudaStream_t
     pos += s; rem -= s;
   }
   CU(cudaGetLastError());
-  CU(cudaStreamSynchronize(st));
+  if (wait) CU(cudaStreamSynchronize(st));
   L->n += m;
   return CG_OK;
 }
 }  // namespace
 
 /* room for n_leaves more leaf digests and their bytes up front (an append that has to grow the digest store pays a device
- * allocation and a copy of everything kept so far) */
+ * allocation and a copy of everything kept so far); on a log without a node store also the fold ping-pong for a block of
+ * n_leaves (24 bytes per leaf), which its appends would otherwise grow themselves */
 int cg_merkle_log_reserve(cg_merkle_log* L, uint64_t n_leaves, uint64_t n_bytes) {
   std::lock_guard<std::mutex> lk(g_mu);
   int rc = log_check(L); if (rc) return rc;
+  InOrder turn(&L->order, G.stream);
+  if ((rc = turn.rc)) return rc;
   uint32_t* unused;
   if (n_leaves && (rc = log_digest_room(L, n_leaves, G.stream, &unused))) return rc;
+  if (n_leaves > 1 && !L->tree && (rc = log_fold_room(L, n_leaves))) return rc;     // (a tree log folds into its store)
   if (n_bytes && (rc = grow_bytes((size_t)n_bytes + 64))) return rc;
   if (n_leaves && (rc = grow(&G.d_off64, &G.cap_off64, (size_t)n_leaves + 1))) return rc;
   return CG_OK;
@@ -1646,6 +1665,8 @@ int cg_merkle_log_append(cg_merkle_log* L, const uint8_t* bytes, const uint64_t*
   for (uint64_t i = 0; i < m; i++) if (offsets[i + 1] < offsets[i]) return fail(CG_ERR_INVALID_ARG, "offsets must be non-decreasing");
   if (L->n + m < L->n) return fail(CG_ERR_TOO_LARGE, "log size overflows 64 bits");
   cudaStream_t st = G.stream;
+  InOrder turn(&L->order, st);
+  if ((rc = turn.rc)) return rc;
   const size_t first = offsets[0], total = offsets[m];
   if ((rc = grow_bytes(total + 64))) return rc;
   if ((rc = grow(&G.d_off64, &G.cap_off64, (size_t)m + 1))) return rc;
@@ -1680,6 +1701,8 @@ int cg_merkle_log_append_jsonl(cg_merkle_log* L, const uint8_t* bytes, uint64_t 
   if (!len) return CG_OK;
   if (!bytes) return fail(CG_ERR_INVALID_ARG, "null argument");
   cudaStream_t st = G.stream;
+  InOrder turn(&L->order, st);
+  if ((rc = turn.rc)) return rc;
   const uint32_t n_pieces = (uint32_t)((len + 4095) / 4096);
   if ((rc = grow_bytes((size_t)len + 64))) return rc;
   if ((rc = grow(&G.d_off32, &G.cap_off32, (size_t)n_pieces + 4))) return rc;          // newline counts per 4 KB piece
@@ -1707,6 +1730,8 @@ int cg_merkle_log_root(cg_merkle_log* L, uint8_t out_root[32]) {
     std::lock_guard<std::mutex> lk(g_mu);
     int rc = log_check(L); if (rc) return rc;
     if (!out_root) return fail(CG_ERR_INVALID_ARG, "null argument");
+    InOrder turn(&L->order, G.stream);
+    if ((rc = turn.rc)) return rc;
     if (L->n) {
       if ((rc = log_root_device(L, G.stream))) return rc;
       CU(cudaMemcpyAsync(out_root, L->d_tmp + 8 * 64, 32, cudaMemcpyDeviceToHost, G.stream));
@@ -1795,6 +1820,8 @@ int cg_merkle_log_proofs(cg_merkle_log* L, const uint64_t* indices, uint32_t m, 
   for (uint32_t i = 0; i < m; i++) if (indices[i] >= tree_size) return fail(CG_ERR_INVALID_ARG, "leaf index out of range");
   const uint32_t longest = tree_size > 1 ? 64 - (uint32_t)__builtin_clzll(tree_size - 1) : 0;       // ceil(log2 tree_size)
   if (path_stride < longest) return fail(CG_ERR_CAPACITY, "path_stride is below ceil(log2 tree_size)");
+  InOrder turn(&L->order, G.stream);
+  if ((rc = turn.rc)) return rc;
   return log_gather(L, indices, m, tree_size, 0, out_paths32, path_stride, out_lens);
 }
 
@@ -1808,6 +1835,8 @@ int cg_merkle_log_consistency_between(cg_merkle_log* L, uint64_t first_size, uin
   const uint32_t len = (uint32_t)proof_ranges(0, second_size, first_size).size();
   if (len > path_cap || (len && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
   *out_len = len;
+  InOrder turn(&L->order, G.stream);
+  if ((rc = turn.rc)) return rc;
   return len ? log_gather(L, nullptr, 1, second_size, first_size, out_path32, len, nullptr) : CG_OK;
 }
 
@@ -1820,6 +1849,8 @@ int cg_merkle_log_proof(cg_merkle_log* L, uint64_t index, uint8_t* out_path32, u
   const auto ranges = proof_ranges(index, L->n, 0);
   *out_len = (uint32_t)ranges.size();
   if (ranges.size() > path_cap || (ranges.size() && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
+  InOrder turn(&L->order, G.stream);
+  if ((rc = turn.rc)) return rc;
   return log_proof(L, ranges, &index, 0, out_path32);
 }
 
@@ -1833,6 +1864,8 @@ int cg_merkle_log_consistency(cg_merkle_log* L, uint64_t first_size, uint8_t* ou
   const auto ranges = proof_ranges(0, L->n, first_size);
   *out_len = (uint32_t)ranges.size();
   if (ranges.size() > path_cap || ranges.size() > 64 || (ranges.size() && !out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
+  InOrder turn(&L->order, G.stream);
+  if ((rc = turn.rc)) return rc;
   return log_proof(L, ranges, nullptr, first_size, out_path32);
 }
 
@@ -1919,6 +1952,158 @@ int cg_merkle_verify_proofs(const uint8_t* leaf_bytes, const uint64_t* leaf_offs
   std::lock_guard<std::mutex> lk(g_mu);
   if (int rc = require_ready()) return rc;
   return verify_proofs(leaf_bytes, leaf_offsets, indices, m, tree_size, paths32, path_stride, path_lens, root, out_ok);
+}
+
+// ---------------------------------------------------------------------------------- Merkle log, device-resident
+// The host twins' results from buffers in HBM, asynchronous on the caller's stream: the absorb plan, the proof ranges' spine and
+// every argument the host can see are worked out on the host, so a call enqueues the twin's launches and waits only when a
+// buffer has to grow.  What only the device can see (offsets, indices, path lengths in HBM) is checked by the kernels in band.
+namespace {
+// a pointer the kernels load from or store to with a width of `align` bytes (null passes: the callers check for null first)
+int check_aligned(const void* p, uintptr_t align, const char* what) {
+  if ((uintptr_t)p & (align - 1)) return fail(CG_ERR_INVALID_ARG, std::string(what) + " must be " + std::to_string(align) + "-byte aligned");
+  return CG_OK;
+}
+cudaStream_t caller_stream(void* stream) { return stream ? (cudaStream_t)stream : G.stream; }
+// m leaves in HBM hashed into the log's digest room (one launch: ragged at d_off, else leaf_len bytes each), then absorbed
+// without a final synchronise
+int log_append_device(cg_merkle_log* L, const uint8_t* d_bytes, const uint64_t* d_off, uint64_t leaf_len, uint64_t m, void* stream) {
+  if (L->n + m < L->n) return fail(CG_ERR_TOO_LARGE, "log size overflows 64 bits");
+  const cudaStream_t st = caller_stream(stream); int rc;
+  InOrder turn(&L->order, st);
+  if ((rc = turn.rc)) return rc;
+  uint32_t* d_dig;
+  if ((rc = log_digest_room(L, m, st, &d_dig))) return rc;
+  count_launches(d_off ? launch_merkle_leaves_guarded(d_bytes, d_off, m, d_dig, L->d_err, st) : launch_merkle_leaves_fixed(d_bytes, leaf_len, m, d_dig, st));
+  G.stats.merkle_leaves += m;
+  return log_absorb(L, d_dig, m, st, /*wait=*/false);
+}
+}  // namespace
+
+int cg_merkle_log_append_device(cg_merkle_log* L, const void* d_bytes, const void* d_offsets, uint64_t m, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  int rc = log_check(L); if (rc) return rc;
+  if (!m) return CG_OK;
+  if (!d_bytes || !d_offsets) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if ((rc = check_aligned(d_bytes, 16, "d_bytes")) || (rc = check_aligned(d_offsets, 8, "d_offsets"))) return rc;
+  return log_append_device(L, (const uint8_t*)d_bytes, (const uint64_t*)d_offsets, 0, m, stream);
+}
+
+int cg_merkle_log_append_fixed_device(cg_merkle_log* L, const void* d_bytes, uint64_t leaf_len, uint64_t m, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  int rc = log_check(L); if (rc) return rc;
+  if (!m) return CG_OK;
+  if (!d_bytes) return fail(CG_ERR_INVALID_ARG, "null argument");
+  // (any alignment: launch_merkle_leaves_fixed takes the byte-granular kernel off the word kernel's alignment, as for
+  // cg_merkle_block_roots_device)
+  if (leaf_len && m > UINT64_MAX / leaf_len) return fail(CG_ERR_INVALID_ARG, "m * leaf_len overflows 64 bits");
+  return log_append_device(L, (const uint8_t*)d_bytes, nullptr, leaf_len, m, stream);
+}
+
+int cg_merkle_log_root_device(cg_merkle_log* L, void* d_out_root32, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  int rc = log_check(L); if (rc) return rc;
+  if (!d_out_root32) return fail(CG_ERR_INVALID_ARG, "null argument");
+  const cudaStream_t st = caller_stream(stream);
+  InOrder turn(&L->order, st);
+  if ((rc = turn.rc)) return rc;
+  if (L->n) {
+    if ((rc = log_root_device(L, st))) return rc;
+  } else {
+    // SHA-256("") by the same kernel as the host twin's, but from the log's own scratch, never the library's staging (whose
+    // other users take no turn before they write it): 16 zero bytes of d_tmp are both the offsets pair and the word it loads
+    CU(cudaMemsetAsync(L->d_tmp, 0, 32, st));
+    count_launches(launch_sha256_batch((const uint8_t*)L->d_tmp, (const uint64_t*)L->d_tmp, 1, (uint8_t*)(L->d_tmp + 8 * 64), st));
+  }
+  CU(cudaMemcpyAsync(d_out_root32, L->d_tmp + 8 * 64, 32, cudaMemcpyDeviceToDevice, st));
+  CU(cudaGetLastError());
+  return CG_OK;
+}
+
+int cg_merkle_log_proofs_device(cg_merkle_log* L, const void* d_indices, uint32_t m, uint64_t tree_size, void* d_out_paths32, uint32_t path_stride,
+                                void* d_out_lens, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  int rc = log_check(L); if (rc) return rc;
+  if (!L->tree) return fail(CG_ERR_UNSUPPORTED, "proofs at any tree size need a log made by cg_merkle_log_create_tree");
+  if (tree_size == 0 || tree_size > L->n) return fail(CG_ERR_INVALID_ARG, "tree_size must be in [1, size of the log]");
+  if (!m) return CG_OK;
+  if (!d_indices || !d_out_lens || (path_stride && !d_out_paths32)) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if ((rc = check_aligned(d_indices, 8, "d_indices")) || (rc = check_aligned(d_out_paths32, 16, "d_out_paths32")) ||
+      (rc = check_aligned(d_out_lens, 4, "d_out_lens"))) return rc;
+  const uint32_t longest = tree_size > 1 ? 64 - (uint32_t)__builtin_clzll(tree_size - 1) : 0;       // ceil(log2 tree_size)
+  if (path_stride < longest) return fail(CG_ERR_CAPACITY, "path_stride is below ceil(log2 tree_size)");
+  const cudaStream_t st = caller_stream(stream);
+  InOrder turn(&L->order, st), dig(&G.dig_order, st);
+  if ((rc = turn.rc) || (rc = dig.rc)) return rc;
+  if ((rc = log_spine(L, tree_size, st))) return rc;
+  count_launches(launch_merkle_gather(log_store(L), L->d_spine, tree_size, (const uint64_t*)d_indices, 0, m, path_stride, (uint32_t*)d_out_paths32,
+                                      (uint32_t*)d_out_lens, G.sm_count, st, /*checked=*/true));
+  CU(cudaGetLastError());
+  return CG_OK;
+}
+
+int cg_merkle_log_consistency_between_device(cg_merkle_log* L, uint64_t first_size, uint64_t second_size, void* d_out_path32, uint32_t path_cap,
+                                             void* d_out_len, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  int rc = log_check(L); if (rc) return rc;
+  if (!d_out_len) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if ((rc = check_aligned(d_out_len, 4, "d_out_len")) || (rc = check_aligned(d_out_path32, 16, "d_out_path32"))) return rc;
+  if (!L->tree) return fail(CG_ERR_UNSUPPORTED, "proofs at any tree size need a log made by cg_merkle_log_create_tree");
+  if (second_size == 0 || second_size > L->n || first_size == 0 || first_size > second_size)
+    return fail(CG_ERR_INVALID_ARG, "need 1 <= first_size <= second_size <= size of the log");
+  const uint32_t len = (uint32_t)proof_ranges(0, second_size, first_size).size();
+  if (len > path_cap || (len && !d_out_path32)) return fail(CG_ERR_CAPACITY, "path buffer too small");
+  const cudaStream_t st = caller_stream(stream);
+  InOrder turn(&L->order, st), dig(&G.dig_order, st);
+  if ((rc = turn.rc) || (rc = dig.rc)) return rc;
+  if (!len) { CU(cudaMemsetAsync(d_out_len, 0, 4, st)); return CG_OK; }
+  if ((rc = log_spine(L, second_size, st))) return rc;
+  count_launches(launch_merkle_gather(log_store(L), L->d_spine, second_size, nullptr, first_size, 1, len, (uint32_t*)d_out_path32, (uint32_t*)d_out_len,
+                                      G.sm_count, st));
+  CU(cudaGetLastError());
+  return CG_OK;
+}
+
+int cg_merkle_verify_proofs_device(const void* d_leaf_bytes, const void* d_leaf_offsets, const void* d_indices, uint32_t m, uint64_t tree_size,
+                                   const void* d_paths32, uint32_t path_stride, const void* d_path_lens, const void* d_root32, void* d_out_ok, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  if (!m) return CG_OK;
+  if (!d_leaf_bytes || !d_leaf_offsets || !d_indices || !d_path_lens || !d_root32 || !d_out_ok || (path_stride && !d_paths32))
+    return fail(CG_ERR_INVALID_ARG, "null argument");
+  int rc;
+  if ((rc = check_aligned(d_leaf_bytes, 16, "d_leaf_bytes")) || (rc = check_aligned(d_leaf_offsets, 8, "d_leaf_offsets")) ||
+      (rc = check_aligned(d_indices, 8, "d_indices")) || (rc = check_aligned(d_paths32, 16, "d_paths32")) ||
+      (rc = check_aligned(d_path_lens, 4, "d_path_lens"))) return rc;
+  const cudaStream_t st = caller_stream(stream);
+  InOrder turn(&G.dig_order, st);
+  if ((rc = turn.rc)) return rc;
+  // d_dig[0]: leaf digests | root (the caller's root copied, so that it may have any alignment)
+  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)m * 8 + 8))) return rc;
+  uint32_t* d_leaf = G.d_dig[0]; uint32_t* d_root = d_leaf + (size_t)m * 8;
+  CU(cudaMemcpyAsync(d_root, d_root32, 32, cudaMemcpyDeviceToDevice, st));
+  const uint64_t* d_off = (const uint64_t*)d_leaf_offsets;
+  int k = launch_merkle_leaves_guarded((const uint8_t*)d_leaf_bytes, d_off, m, d_leaf, nullptr, st);
+  k += launch_merkle_verify_batch(d_leaf, (const uint64_t*)d_indices, m, tree_size, (const uint32_t*)d_paths32, path_stride, (const uint32_t*)d_path_lens,
+                                  d_root, (uint8_t*)d_out_ok, G.sm_count, st, d_off);
+  count_launches(k);
+  CU(cudaGetLastError());
+  return CG_OK;
+}
+
+int cg_merkle_log_join(cg_merkle_log* L, void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  int rc = log_check(L); if (rc) return rc;
+  CU(cudaStreamSynchronize(caller_stream(stream)));
+  CU(cudaEventSynchronize(L->order.ev));                    // (every call issued on the log has run: each one ran behind the one before)
+  uint32_t err = 0;
+  CU(cudaMemcpyAsync(&err, L->d_err, 4, cudaMemcpyDeviceToHost, G.stream));
+  CU(cudaStreamSynchronize(G.stream));
+  if (err) {
+    L->failed = true;
+    return fail(CG_ERR_INVALID_ARG, "a device append read a decreasing offset pair: that leaf went in as the empty leaf, and the log refuses every further call");
+  }
+  return CG_OK;
 }
 
 // ---------------------------------------------------------------------------------- multi-GPU: one process per GPU

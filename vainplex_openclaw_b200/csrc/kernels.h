@@ -204,6 +204,9 @@ int launch_merkle_leaves_fixed(const uint8_t* d_bytes, uint64_t leaf_len, uint64
 // ragged leaves, word-granular: d_bytes must be one of the library's own buffers (readable 4 bytes before the first leaf and
 // 8 bytes after the last); trim_newline: a final '\n' of a leaf's range is not hashed (JSONL lines)
 int launch_merkle_leaves_var(const uint8_t* d_bytes, const uint64_t* d_off, uint64_t n, uint32_t* d_out, cudaStream_t stream, bool trim_newline = false);
+// ragged leaves in a caller's buffer (16-byte aligned, readable 16 bytes past the last offset; nothing readable in front of
+// it): a decreasing offset pair is hashed as the empty leaf, without reading, and sets *d_err (d_err may be null)
+int launch_merkle_leaves_guarded(const uint8_t* d_bytes, const uint64_t* d_off, uint64_t n, uint32_t* d_out, uint32_t* d_err, cudaStream_t stream);
 // JSONL on the device: newline counts per 4 KB piece + their exclusive scan (d_piece_counts, *d_total_lines), then the line starts
 int launch_newline_split(const uint8_t* d_bytes, uint64_t len, uint32_t* d_piece_counts, uint64_t* d_total_lines, cudaStream_t stream);
 int launch_newline_starts(const uint8_t* d_bytes, uint64_t len, const uint32_t* d_piece_rank, uint64_t* d_starts, uint64_t n_lines, cudaStream_t stream);
@@ -235,13 +238,16 @@ __host__ __device__ inline uint64_t merkle_path_levels(uint64_t i, uint64_t size
 }
 // paths from the store: one warp per path, kGatherWarps per block, at most kGatherBlocksPerSm blocks per SM (grid-stride);
 // d_idx = leaf indices, or null: one consistency proof PROOF(first, D[0:size]).  d_spine: spine of `size` (one chain launch).
+// checked (d_idx in a caller's HBM): an index >= size gets length 0xffffffff and an all-zero stride (first is unused).
 constexpr uint32_t kGatherWarps = 8, kGatherBlocksPerSm = 8;
 int launch_merkle_gather(const NodeStore& st, const uint32_t* d_spine, uint64_t size, const uint64_t* d_idx, uint64_t first, uint32_t m, uint32_t stride,
-                         uint32_t* d_out, uint32_t* d_lens, int sm_count, cudaStream_t stream);
+                         uint32_t* d_out, uint32_t* d_lens, int sm_count, cudaStream_t stream, bool checked = false);
 // RFC 9162 2.1.3.2 for m proofs against one (size, root): one thread per proof, kProofVerifyBlock threads per block, at most
-// kProofVerifyBlocksPerSm blocks per SM (grid-stride); d_ok[i] = 1 iff proof i holds
+// kProofVerifyBlocksPerSm blocks per SM (grid-stride); d_ok[i] = 1 iff proof i holds.  With d_leaf_off (lengths and leaf
+// offsets in a caller's HBM) a length above min(64, stride) or a decreasing offset pair gives 0 without reading the path.
 constexpr uint32_t kProofVerifyBlock = 128, kProofVerifyBlocksPerSm = 16;
 int launch_merkle_verify_batch(const uint32_t* d_leaf32, const uint64_t* d_idx, uint32_t m, uint64_t size, const uint32_t* d_paths, uint32_t stride,
-                               const uint32_t* d_lens, const uint32_t* d_root32, uint8_t* d_ok, int sm_count, cudaStream_t stream);
+                               const uint32_t* d_lens, const uint32_t* d_root32, uint8_t* d_ok, int sm_count, cudaStream_t stream,
+                               const uint64_t* d_leaf_off = nullptr);
 
 }  // namespace cg

@@ -98,14 +98,18 @@ __device__ void sha_bytes(int prefix, const uint8_t* __restrict__ data, uint64_t
 // and one funnel shift.  Only the first word (prefix byte) and the words around the end of the data (0x80, zeros, length)
 // are patched.  The caller guarantees that the aligned words covering [A, data + len) are readable (up to 3 bytes before
 // and 7 bytes after the data: every buffer this is called on is one of the library's own, padded on both sides).
-__device__ void sha_words(int prefix, const uint8_t* __restrict__ data, uint64_t len, uint32_t h[8]) {
+// kGuarded: the data lies in a caller's buffer that starts at buf (16-byte aligned) and has nothing readable in front of it.
+// The aligned word before buf (fetched for a leaf at offset 0) is not loaded, and its bytes are taken as zero: only its last
+// byte is part of the stream, at the prefix position, and the prefix is patched anyway.
+template <bool kGuarded = false>
+__device__ void sha_words(int prefix, const uint8_t* __restrict__ data, uint64_t len, uint32_t h[8], const uint8_t* buf = nullptr) {
   sha_init(h);
   const uint32_t p = prefix >= 0 ? 1u : 0u;
   const uint64_t total = p + len, nblk = (total + 9 + 63) / 64;
   const uintptr_t A = reinterpret_cast<uintptr_t>(data) - p;
   const uint32_t* base = reinterpret_cast<const uint32_t*>(A & ~(uintptr_t)3);
   const uint32_t sh = 8u * (uint32_t)(A & 3u);
-  uint32_t lo = __ldg(base);                           // aligned word holding stream byte 0
+  uint32_t lo = (kGuarded && reinterpret_cast<const uint8_t*>(base) < buf) ? 0u : __ldg(base);   // aligned word holding stream byte 0
   uint64_t q = 1;                                      // next aligned word to fetch
   for (uint64_t blk = 0; blk < nblk; blk++) {
     uint32_t w[16];
@@ -150,6 +154,20 @@ __global__ void __launch_bounds__(128) merkle_leaves_var_kernel(const uint8_t* _
   uint64_t b = off[i], e = off[i + 1];
   if (trim_newline && e > b && bytes[e - 1] == '\n') e--;
   sha_words(0x00, bytes + b, e - b, h);
+  store_digest(out + i * 8, h);
+}
+
+// The same over a caller's buffer (16-byte aligned, readable 16 bytes past the last offset), whose offsets the host has not
+// seen: a leaf at offset 0 goes through sha_words<true>, and a decreasing pair (off[i+1] < off[i]) is hashed as the empty leaf
+// without touching the bytes (sha_words<true> at offset 0 with length 0 loads nothing) and sets *err unless err is null.
+__global__ void __launch_bounds__(128) merkle_leaves_guarded_kernel(const uint8_t* __restrict__ bytes, const uint64_t* __restrict__ off,
+                                                                     uint64_t n, uint32_t* __restrict__ out, uint32_t* __restrict__ err) {
+  uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint32_t h[8];
+  uint64_t b = off[i], e = off[i + 1];
+  if (e < b) { b = e = 0; if (err) *err = 1u; }
+  sha_words<true>(0x00, bytes + b, e - b, h, bytes);
   store_digest(out + i * 8, h);
 }
 
@@ -270,12 +288,30 @@ __device__ bool merkle_verify_path(const uint32_t* __restrict__ leaf32, unsigned
   return eq;
 }
 // m proofs against one (size, root), one thread per proof: proof i = leaf digest leaf32[i], index idx[i], the path_lens[i]
-// digests at paths + 8 i stride.  Grid-stride over the proofs.
+// digests at paths + 8 i stride.  Grid-stride over the proofs.  kChecked (lengths and leaf offsets in a caller's HBM, which
+// the host has not seen): a length above min(64, stride) or a decreasing pair off[i] > off[i+1] gives ok = 0 without reading
+// the path (merkle_verify_path itself rejects an index >= size before it reads anything).
+template <bool kChecked>
+__device__ __forceinline__ void merkle_verify_batch(const uint32_t* __restrict__ leaf32, const uint64_t* __restrict__ idx, uint32_t m, unsigned long long size,
+                                                    const uint32_t* __restrict__ paths, uint32_t stride, const uint32_t* __restrict__ path_lens,
+                                                    const uint32_t* __restrict__ root32, uint8_t* __restrict__ ok, const uint64_t* __restrict__ off) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+    if (kChecked && (path_lens[i] > (stride < 64u ? stride : 64u) || off[i + 1] < off[i])) { ok[i] = 0; continue; }
+    ok[i] = merkle_verify_path(leaf32 + 8 * (size_t)i, idx[i], size, paths + (size_t)i * stride * 8, path_lens[i], root32) ? 1 : 0;
+  }
+}
 __global__ void __launch_bounds__(128) merkle_verify_batch_kernel(const uint32_t* __restrict__ leaf32, const uint64_t* __restrict__ idx, uint32_t m,
                                                                   unsigned long long size, const uint32_t* __restrict__ paths, uint32_t stride,
                                                                   const uint32_t* __restrict__ path_lens, const uint32_t* __restrict__ root32, uint8_t* __restrict__ ok) {
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x)
-    ok[i] = merkle_verify_path(leaf32 + 8 * (size_t)i, idx[i], size, paths + (size_t)i * stride * 8, path_lens[i], root32) ? 1 : 0;
+  merkle_verify_batch<false>(leaf32, idx, m, size, paths, stride, path_lens, root32, ok, nullptr);
+}
+// (at most 64 registers, as the unchecked instantiation has: unbounded, the two checks took it to 71, 7 blocks per SM instead
+// of 8, and 15 % longer on 1 Mi proofs at 2^24 leaves; bounded it spills nothing)
+__global__ void __launch_bounds__(128, 8) merkle_verify_checked_kernel(const uint32_t* __restrict__ leaf32, const uint64_t* __restrict__ idx, uint32_t m,
+                                                                    unsigned long long size, const uint32_t* __restrict__ paths, uint32_t stride,
+                                                                    const uint32_t* __restrict__ path_lens, const uint32_t* __restrict__ root32, uint8_t* __restrict__ ok,
+                                                                    const uint64_t* __restrict__ off) {
+  merkle_verify_batch<true>(leaf32, idx, m, size, paths, stride, path_lens, root32, ok, off);
 }
 
 // Paths from a log's node store.  Element `pos` of the path of leaf i in the tree of `size` leaves (merkle_path_levels: the
@@ -294,14 +330,18 @@ __device__ __forceinline__ const uint32_t* merkle_path_element(const NodeStore& 
 }
 // One warp per path (grid-stride): lane p copies elements p, p + 32, ... into out + 8 (item stride + p) and zeros the
 // stride's unused tail; lens[item] = the path's length.  idx: leaf indices; null: one consistency proof from `first`.
-__global__ void __launch_bounds__(256) merkle_gather_kernel(NodeStore st, const uint32_t* __restrict__ spine, uint64_t size, const uint64_t* __restrict__ idx,
-                                                            uint64_t first, uint32_t m, uint32_t stride, uint32_t* __restrict__ out, uint32_t* __restrict__ lens) {
+// kChecked (indices in a caller's HBM, which the host has not seen): an index >= size gets length 0xffffffff and an all-zero
+// stride, and no element is read for it.
+template <bool kChecked>
+__device__ __forceinline__ void merkle_gather(const NodeStore& st, const uint32_t* __restrict__ spine, uint64_t size, const uint64_t* __restrict__ idx,
+                                              uint64_t first, uint32_t m, uint32_t stride, uint32_t* __restrict__ out, uint32_t* __restrict__ lens) {
   const uint32_t lane = threadIdx.x & 31u, wpb = blockDim.x >> 5;
   for (uint32_t item = blockIdx.x * wpb + (threadIdx.x >> 5); item < m; item += gridDim.x * wpb) {
     uint64_t i; uint32_t lo = 0; bool seed = false;
     if (idx) i = idx[item];
     else { i = first - 1; lo = __ffsll((long long)first) - 1; seed = (first & (first - 1)) != 0; }
-    uint64_t levels = merkle_path_levels(i, size, lo);
+    const bool inside = !kChecked || i < size;
+    uint64_t levels = inside ? merkle_path_levels(i, size, lo) : 0ull;
     if (!idx && first == size) { levels = 0; seed = false; }
     const uint32_t len = __popcll(levels) + (seed ? 1u : 0u);
     for (uint32_t p = lane; p < stride; p += 32u) {
@@ -313,8 +353,16 @@ __global__ void __launch_bounds__(256) merkle_gather_kernel(NodeStore st, const 
       uint4* dst = reinterpret_cast<uint4*>(out + ((size_t)item * stride + p) * 8);
       dst[0] = a; dst[1] = b;
     }
-    if (lane == 0) lens[item] = len;
+    if (lane == 0) lens[item] = inside ? len : 0xffffffffu;
   }
+}
+__global__ void __launch_bounds__(256) merkle_gather_kernel(NodeStore st, const uint32_t* __restrict__ spine, uint64_t size, const uint64_t* __restrict__ idx,
+                                                            uint64_t first, uint32_t m, uint32_t stride, uint32_t* __restrict__ out, uint32_t* __restrict__ lens) {
+  merkle_gather<false>(st, spine, size, idx, first, m, stride, out, lens);
+}
+__global__ void __launch_bounds__(256) merkle_gather_checked_kernel(NodeStore st, const uint32_t* __restrict__ spine, uint64_t size, const uint64_t* __restrict__ idx,
+                                                                    uint32_t m, uint32_t stride, uint32_t* __restrict__ out, uint32_t* __restrict__ lens) {
+  merkle_gather<true>(st, spine, size, idx, 0, m, stride, out, lens);
 }
 // RFC 9162 2.1.4.2: does `path` prove that the tree of `first` leaves with root first32 is a prefix of the tree of
 // `second` leaves with root second32?
@@ -456,17 +504,19 @@ int launch_merkle_chain_keep(const ChainOperands& ops, uint32_t n_left, const ui
   return 1;
 }
 int launch_merkle_verify_batch(const uint32_t* d_leaf32, const uint64_t* d_idx, uint32_t m, uint64_t size, const uint32_t* d_paths, uint32_t stride,
-                               const uint32_t* d_lens, const uint32_t* d_root32, uint8_t* d_ok, int sm_count, cudaStream_t stream) {
+                               const uint32_t* d_lens, const uint32_t* d_root32, uint8_t* d_ok, int sm_count, cudaStream_t stream, const uint64_t* d_leaf_off) {
   if (!m) return 0;
   const uint32_t grid = std::min<uint32_t>((m + kProofVerifyBlock - 1) / kProofVerifyBlock, (uint32_t)sm_count * kProofVerifyBlocksPerSm);
-  merkle_verify_batch_kernel<<<grid, kProofVerifyBlock, 0, stream>>>(d_leaf32, d_idx, m, size, d_paths, stride, d_lens, d_root32, d_ok);
+  if (d_leaf_off) merkle_verify_checked_kernel<<<grid, kProofVerifyBlock, 0, stream>>>(d_leaf32, d_idx, m, size, d_paths, stride, d_lens, d_root32, d_ok, d_leaf_off);
+  else merkle_verify_batch_kernel<<<grid, kProofVerifyBlock, 0, stream>>>(d_leaf32, d_idx, m, size, d_paths, stride, d_lens, d_root32, d_ok);
   return 1;
 }
 int launch_merkle_gather(const NodeStore& st, const uint32_t* d_spine, uint64_t size, const uint64_t* d_idx, uint64_t first, uint32_t m, uint32_t stride,
-                         uint32_t* d_out, uint32_t* d_lens, int sm_count, cudaStream_t stream) {
+                         uint32_t* d_out, uint32_t* d_lens, int sm_count, cudaStream_t stream, bool checked) {
   if (!m) return 0;
   const uint32_t grid = std::min<uint32_t>((m + kGatherWarps - 1) / kGatherWarps, (uint32_t)sm_count * kGatherBlocksPerSm);
-  merkle_gather_kernel<<<grid, kGatherWarps * 32, 0, stream>>>(st, d_spine, size, d_idx, first, m, stride, d_out, d_lens);
+  if (checked) merkle_gather_checked_kernel<<<grid, kGatherWarps * 32, 0, stream>>>(st, d_spine, size, d_idx, m, stride, d_out, d_lens);
+  else merkle_gather_kernel<<<grid, kGatherWarps * 32, 0, stream>>>(st, d_spine, size, d_idx, first, m, stride, d_out, d_lens);
   return 1;
 }
 
@@ -574,6 +624,11 @@ int launch_merkle_leaves_fixed(const uint8_t* d_bytes, uint64_t leaf_len, uint64
 int launch_merkle_leaves_var(const uint8_t* d_bytes, const uint64_t* d_off, uint64_t n, uint32_t* d_out, cudaStream_t stream, bool trim_newline) {
   if (!n) return 0;
   merkle_leaves_var_kernel<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(d_bytes, d_off, n, d_out, trim_newline ? 1 : 0);
+  return 1;
+}
+int launch_merkle_leaves_guarded(const uint8_t* d_bytes, const uint64_t* d_off, uint64_t n, uint32_t* d_out, uint32_t* d_err, cudaStream_t stream) {
+  if (!n) return 0;
+  merkle_leaves_guarded_kernel<<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(d_bytes, d_off, n, d_out, d_err);
   return 1;
 }
 static int launch_merkle_level(const uint32_t* d_in, uint64_t n_in, uint32_t* d_out, cudaStream_t stream) {
