@@ -269,6 +269,59 @@ CG_API int cg_redact_batch_device_views(cg_ruleset *rs, const void *d_bytes, con
 CG_API int cg_policy_verdict_batch_device_views(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, const void *d_views, uint32_t n,
                                                 void *d_out_verdicts, void *stream);
 
+/* ---- whole policy rules (PolicyEvaluator.evaluate, src/policy-evaluator.ts:18-146, and the evaluators of src/conditions) for a batch of
+ * evaluation contexts.  A policy PROGRAM is stored on a rule set; one call scans all texts of all contexts in one policy-mode
+ * step and evaluates the program for every context on the device.
+ *
+ * Split of work.  Regex leaves are device leaves HIT(r, q) = "rule r of this rule set hit some text of the context whose
+ * role is q": messageContains (role 0, the message), conversationContains (role 1, a conversation entry) and a tool param's
+ * `matches` (role 2 + k, param key k as the caller numbers them).  Texts are included as a caller of the reference sees
+ * them: an empty message is left out, every conversation entry and every string param is included, so checkMessage's
+ * `!ctx.messageContent` (context.ts) and matchParam's `typeof value !== "string"` (tool.ts) hold without further leaves; an
+ * invalid `matches` pattern is CONST 0 (tool.ts:39-44).  Every other test is an ATOM a, one bit per context the caller
+ * computes: tool-name and agent-id globs, trustTier, channel, hasMetadata, sessionKey, param equals / contains / startsWith /
+ * in, the rule gates minTrust / maxTrust, a policy's matchesScope (:18-26), time / risk / frequency.  The device evaluates
+ * the boolean structure (conditions = AND, any = OR, not), the first matching rule of each policy (matchPolicy, :129-146)
+ * and aggregateMatches (:44-78).  Policies are stored in evaluation order (priority, then specificity, :36-42: an order that
+ * depends on the policy alone; scope only removes policies, so one global order serves every context).
+ *
+ * Program (uint32 words): [n_policies], then per policy [scope atom, 0xffffffff = none][n_rules], then per rule
+ * [action | has_reason << 2][n_ops][n_ops op words, postfix].  action: 0 allow, 1 audit, 2 2fa, 3 deny; has_reason: the
+ * effect has a non-empty reason.  Program rules are numbered 0, 1, ... across all policies in this order.  Op words (low 3
+ * bits the op): CONST b = 0 | b << 3 (b = 0 or 1); ATOM a = 1 | a << 3; HIT r q = 2 | r << 3 | q << 24 (r < 2^21, q < 256);
+ * AND = 3; OR = 4; NOT = 5.  An empty condition list is CONST 1, an empty `any` CONST 0.
+ * cg_ruleset_set_policy_program checks that every rule leaves exactly one value, that no rule needs a stack deeper than 32
+ * (CG_ERR_TOO_LARGE), that r < the rule set's rules and a < n_atoms, and at most 2^20 - 1 program rules (CG_ERR_TOO_LARGE);
+ * anything else malformed is CG_ERR_INVALID_ARG.  Like cg_ruleset_set_policy it waits for the library's stream and replaces
+ * the tables.
+ *
+ * cg_policy_eval_batch: n_texts texts (bytes / offsets as cg_scan_batch) with one role each (roles[n_texts]); context c owns
+ * the texts [ctx_offsets[c], ctx_offsets[c+1]) (n_ctx + 1 offsets, non-decreasing, at most n_texts; a context may own none,
+ * so n_ctx may exceed n_texts and n_texts may be 0) and atom row atoms[c * ceil(n_atoms / 32) ..] (bit a of the row = atom
+ * a).  out_verdicts[c] = outcome | (matched policies, saturating at 511) << 3 | deciding program rule << 12, outcome 0 no
+ * policy matched, 1 allow, 2 allow with audit, 3 2fa, 4 deny; the deciding rule is the first match of the winning action
+ * (deny or 2fa) with has_reason, else 0xfffff -- the reason is the first non-empty one of that action (:51-60).
+ * out_matches: the (context, program rule) of every policy that matched, sorted by (context, evaluation order) -- the
+ * `matches` list of the result (engine.ts:236,249) -- the first matches_cap written; *out_nmatches = their number
+ * (CG_ERR_CAPACITY past matches_cap, CG_ERR_TOO_LARGE at 2^32 - 1 or more).  out_matches and out_nmatches may both be NULL
+ * (verdicts only).  A context range that is decreasing or past n_texts is CG_ERR_INVALID_ARG before anything is copied. */
+typedef struct cg_policy_match { uint32_t ctx; uint32_t rule; } cg_policy_match;   /* rule = program rule index */
+CG_API int cg_ruleset_set_policy_program(cg_ruleset *rs, const uint32_t *program, uint32_t words, uint32_t n_atoms);
+CG_API int cg_policy_eval_batch(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, const uint8_t *roles, uint32_t n_texts,
+                                const uint32_t *ctx_offsets, const uint32_t *atoms, uint32_t n_ctx, uint32_t *out_verdicts,
+                                cg_policy_match *out_matches, uint32_t matches_cap, uint32_t *out_nmatches);
+/* The same for a batch in HBM (d_bytes 16-byte aligned as for cg_scan_batch_device; every other pointer 4-byte aligned;
+ * d_out_matches may be NULL when matches_cap is 0; d_out_nmatches = NULL: verdicts only).  Asynchronous and in order on
+ * `stream`, status from cg_scan_join: CG_ERR_CAPACITY when there are more than matches_cap matches (the first matches_cap
+ * are written), CG_ERR_TOO_LARGE at 2^32 - 1 or more, and CG_ERR_CAPACITY once after an internal queue overflow (then every
+ * verdict is 0xffffffff, *d_out_nmatches = 0xffffffff and no match is written: issue the batch again).  The host cannot read
+ * the context offsets: a context whose range is decreasing or runs past n_texts gets verdict 0xfffffffe and no match, the
+ * others are unaffected.  n_ctx = 0 writes 0 to *d_out_nmatches and enqueues nothing else.  Launches: the step, then one
+ * kernel (verdicts only) or count + exclusive scan + emit, on grids that depend on n_ctx and the SM count only. */
+CG_API int cg_policy_eval_batch_device(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, const void *d_roles, uint32_t n_texts,
+                                       const void *d_ctx_offsets, const void *d_atoms, uint32_t n_ctx, void *d_out_verdicts,
+                                       void *d_out_matches, uint32_t matches_cap, void *d_out_nmatches, void *stream);
+
 /* ---- SHA-256.  Replaces createHash("sha256").update(s).digest() at src/util.ts:77-79,
  * src/redaction/vault.ts:26-28 (and nats/src/hooks.ts:90-94) for a batch of n byte strings. */
 CG_API int cg_sha256_batch(const uint8_t *bytes, const uint64_t *offsets, uint32_t n, uint8_t *out_digests32);

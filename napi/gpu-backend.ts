@@ -38,6 +38,10 @@ type Addon = {
   findMatchesBatchViews(handle: unknown, bytes: Uint8Array, offsets: Uint32Array, views: Uint8Array): Uint32Array;
   redactBatchViews(handle: unknown, bytes: Uint8Array, offsets: Uint32Array, views: Uint8Array): { bytes: Uint8Array; offsets: Uint32Array; spans: Uint32Array; digests: Uint8Array };
   verdictBatchViews(handle: unknown, bytes: Uint8Array, offsets: Uint32Array, views: Uint8Array): Uint32Array;
+  // whole policies on the device (openclaw_gov.h: program layout): one verdict per context, (ctx, program rule) match pairs
+  setPolicyProgram(handle: unknown, program: Uint32Array, nAtoms: number): void;
+  policyEvalBatch(handle: unknown, bytes: Uint8Array, offsets: Uint32Array, roles: Uint8Array, ctxOffsets: Uint32Array, atoms: Uint32Array,
+                  nAtoms: number): { verdicts: Uint32Array; matches: Uint32Array };
   sha256Batch(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array;
   merkleRoot(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array;
   logCreate(keepLeafDigests: boolean): unknown;
@@ -140,6 +144,81 @@ export class GpuRuleScanner {
     for (let k = 0; k < hits.length; k += 2) out[hits[k]].add(this.ruleOfPattern[hits[k + 1]]);
     return out.map((s) => [...s].sort((a, b) => a - b));
   }
+}
+
+/** A policy list compiled for setPolicyProgram, as plugin.PolicyEvaluator._compile_program compiles it: policies in
+ * sortPolicies order (src/policy-evaluator.ts:36-42), regex tests as HIT(rule, role) leaves (role 0 message, 1 conversation
+ * entry, 2 + k tool param paramRole[k]), every other test an atom evaluated on the host by the reference's own condition code
+ * (evalCondition = evaluateConditions over one condition, src/conditions/index.ts).  patternRule / toolRule: the rule of each
+ * messageContains / conversationContains pattern and of each valid `matches` pattern in the scanner's rule set. */
+type Ctx = Record<string, any>;
+type Cond = Record<string, any>;
+const OP = { CONST: 0, ATOM: 1, HIT: 2, AND: 3, OR: 4, NOT: 5 };
+const ACTION: Record<string, number> = { allow: 0, audit: 1, "2fa": 2, deny: 3 };
+const TIERS = ["untrusted", "restricted", "standard", "trusted", "elevated"];
+export function compilePolicyProgram(policies: any[], patternRule: Map<string, number>, toolRule: Map<string, number>,
+                                     evalCondition: (c: Cond, ctx: Ctx) => boolean) {
+  const atomId = new Map<string, number>();
+  const atoms: ((ctx: Ctx) => boolean)[] = [];
+  const paramRole = new Map<string, number>();
+  const atomIndex = (key: string, fn: (ctx: Ctx) => boolean) => {
+    if (!atomId.has(key)) { atomId.set(key, atoms.length); atoms.push(fn); }
+    return atomId.get(key)!;
+  };
+  const atom = (c: Cond) => [OP.ATOM | (atomIndex(JSON.stringify(c), (ctx) => evalCondition(c, ctx)) << 3)];
+  const hit = (rule: number, role: number) => [(OP.HIT | (rule << 3) | (role << 24)) >>> 0];
+  const fold = (parts: number[][], op: number, empty: number) =>
+    parts.length ? parts.slice(1).reduce((acc, q) => [...acc, ...q, op], parts[0]) : [OP.CONST | (empty << 3)];
+  const list = (v: any) => (Array.isArray(v) ? v : [v]);
+  const cond = (c: Cond): number[] => {
+    const parts: number[][] = [];
+    if (c.type === "context") {
+      for (const [key, role] of [["conversationContains", 1], ["messageContains", 0]] as const)
+        if (c[key] != null) parts.push(fold(list(c[key]).map((p: string) => hit(patternRule.get(p)!, role)), OP.OR, 0));
+      for (const key of ["hasMetadata", "channel", "sessionKey"]) if (c[key] != null) parts.push(atom({ type: "context", [key]: c[key] }));
+      return fold(parts, OP.AND, 1);
+    }
+    if (c.type === "tool") {
+      if (c.name != null) parts.push(atom({ type: "tool", name: c.name }));
+      if (c.params && Object.keys(c.params).length) {
+        for (const [key, m] of Object.entries<any>(c.params)) {
+          if ("matches" in m && !("equals" in m) && !("contains" in m)) {
+            if (!paramRole.has(key)) paramRole.set(key, 2 + paramRole.size);
+            parts.push(toolRule.has(m.matches) ? hit(toolRule.get(m.matches)!, paramRole.get(key)!) : [OP.CONST]);
+          } else parts.push(atom({ type: "tool", params: { [key]: m } }));
+        }
+      }
+      return fold(parts, OP.AND, 1);
+    }
+    if (c.type === "agent") {
+      for (const key of ["id", "trustTier"]) if (c[key] != null) parts.push(atom({ type: "agent", [key]: c[key] }));
+      return fold(parts, OP.AND, 1);
+    }
+    if (c.type === "any") return fold((c.conditions ?? []).map(cond), OP.OR, 0);
+    if (c.type === "not") return [...cond(c.condition), OP.NOT];
+    return atom(c);                                           // time / risk / frequency
+  };
+  const spec = (p: any) => (p.scope?.agents?.length ? 10 : 0) + (p.scope?.channels?.length ? 5 : 0) + (p.scope?.hooks?.length ? 3 : 0);
+  const order = [...policies].sort((a, b) => (b.priority ?? 0) - (a.priority ?? 0) || spec(b) - spec(a));
+  const words: number[] = [order.length];
+  const rules: [any, any][] = [];
+  for (const p of order) {
+    const sc = p.scope ?? {};
+    words.push(sc.excludeAgents?.length || sc.channels?.length
+      ? atomIndex("scope:" + JSON.stringify([sc.excludeAgents, sc.channels]), (ctx) =>
+          !sc.excludeAgents?.includes(ctx.agentId) && !(sc.channels?.length && (!ctx.channel || !sc.channels.includes(ctx.channel))))
+      : 0xffffffff, p.rules.length);
+    for (const r of p.rules) {
+      const tier = (ctx: Ctx) => TIERS.indexOf(ctx.trust?.session?.tier ?? "standard");
+      const gates: number[][] = [];
+      if (r.minTrust) gates.push([OP.ATOM | (atomIndex("minTrust:" + r.minTrust, (ctx) => tier(ctx) >= TIERS.indexOf(r.minTrust)) << 3)]);
+      if (r.maxTrust) gates.push([OP.ATOM | (atomIndex("maxTrust:" + r.maxTrust, (ctx) => tier(ctx) <= TIERS.indexOf(r.maxTrust)) << 3)]);
+      const ops = fold([...gates, ...(r.conditions ?? []).map(cond)], OP.AND, 1);
+      words.push((ACTION[r.effect?.action] ?? 0) | (r.effect?.reason ? 4 : 0), ops.length, ...ops);
+      rules.push([p, r]);
+    }
+  }
+  return { program: Uint32Array.from(words), atoms, paramRole, rules };
 }
 
 /** sha256 (src/util.ts:77-79) for a batch of strings, hex digests. */

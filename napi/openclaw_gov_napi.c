@@ -25,6 +25,9 @@
  *   setViews(handle, rows: Uint32Array, nViews: number): void  // nViews rows of ceil(nRules / 32) words, bit r = rule r in the view
  *   scanBatchViews / findMatchesBatchViews / redactBatchViews / verdictBatchViews(handle, bytes, offsets, views: Uint8Array)
  *     // the batch calls above with one view id per message: each message decided on its view's rules alone
+ *   setPolicyProgram(handle, program: Uint32Array, nAtoms: number): void  // whole policies (openclaw_gov.h: program layout)
+ *   policyEvalBatch(handle, bytes, offsets, roles: Uint8Array, ctxOffsets: Uint32Array, atoms: Uint32Array, nAtoms: number):
+ *     {verdicts: Uint32Array, matches: Uint32Array}  // one verdict per context; matches: ctx, program rule pairs
  *   sha256Batch(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array  // 32 bytes per item
  *   merkleRoot(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array   // 32 bytes
  *   logCreate(keepLeafDigests: boolean): External ; logRestore(size: bigint, frontier: Uint8Array): External
@@ -277,6 +280,51 @@ static napi_value verdict_batch(napi_env env, napi_callback_info info, int views
 }
 static napi_value js_verdict_batch(napi_env env, napi_callback_info info) { return verdict_batch(env, info, 0); }
 static napi_value js_verdict_batch_views(napi_env env, napi_callback_info info) { return verdict_batch(env, info, 1); }
+
+static napi_value js_set_policy_program(napi_env env, napi_callback_info info) {
+  ARGS(env, info, 3)
+  cg_ruleset *rs; uint8_t *prog; size_t nb; uint32_t n_atoms = 0;
+  NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
+  if (!get_ta(env, argv[1], &prog, &nb, napi_uint32_array) || !nb || napi_get_value_uint32(env, argv[2], &n_atoms) != napi_ok) {
+    napi_throw_type_error(env, NULL, "setPolicyProgram(handle, program: Uint32Array, nAtoms)"); return NULL;
+  }
+  CG_CALL(env, cg_ruleset_set_policy_program(rs, (const uint32_t *)prog, (uint32_t)(nb / 4), n_atoms));
+  return NULL;
+}
+
+/* the texts, their roles, the contexts' text ranges (checked here: the C call trusts them) and ceil(nAtoms / 32) atom words
+ * per context, nAtoms as given to setPolicyProgram */
+static napi_value js_policy_eval_batch(napi_env env, napi_callback_info info) {
+  ARGS(env, info, 7)
+  cg_ruleset *rs; uint8_t *bytes, *offp, *roles, *ctxp, *atoms; size_t nr, nc, na; uint32_t n_atoms = 0;
+  NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
+  const int64_t nn = get_batch(env, argv[1], argv[2], 0, &bytes, &offp); if (nn < 0) return NULL;
+  if (!get_ta(env, argv[3], &roles, &nr, napi_uint8_array) || (int64_t)nr != nn || !get_ta(env, argv[4], &ctxp, &nc, napi_uint32_array) || nc < 4 ||
+      !get_ta(env, argv[5], &atoms, &na, napi_uint32_array) || napi_get_value_uint32(env, argv[6], &n_atoms) != napi_ok) {
+    napi_throw_type_error(env, NULL, "policyEvalBatch(handle, bytes, offsets, roles: Uint8Array (one per text), ctxOffsets: Uint32Array, atoms: Uint32Array, nAtoms)"); return NULL;
+  }
+  const uint32_t n_ctx = (uint32_t)(nc / 4 - 1), *co = (const uint32_t *)ctxp;
+  for (uint32_t c = 0; c < n_ctx; c++)
+    if (co[c] > co[c + 1] || co[c + 1] > (uint64_t)nn) { napi_throw_range_error(env, NULL, "ctxOffsets must be non-decreasing and end inside the texts"); return NULL; }
+  if (na != (size_t)n_ctx * ((n_atoms + 31) / 32) * 4) { napi_throw_type_error(env, NULL, "atoms: ceil(nAtoms / 32) words per context"); return NULL; }
+  napi_value vab, verdicts, mab, matches, out; void *vdata, *mdata;
+  NAPI_CALL(env, napi_create_arraybuffer(env, (size_t)n_ctx * 4, &vdata, &vab));
+  uint32_t nm = 0, cap = 1024; cg_policy_match *tmp = (cg_policy_match *)malloc(sizeof(cg_policy_match) * cap);
+#define EVAL(cap) cg_policy_eval_batch(rs, bytes, (const uint32_t *)offp, nr ? roles : NULL, (uint32_t)nn, co, na ? (const uint32_t *)atoms : NULL, n_ctx, \
+                                       (uint32_t *)vdata, tmp, (cap), &nm)
+  int rc = tmp ? EVAL(cap) : CG_ERR_CUDA;
+  if (rc == CG_ERR_CAPACITY) { cap = nm; cg_policy_match *t2 = (cg_policy_match *)realloc(tmp, sizeof(cg_policy_match) * cap); if (t2) { tmp = t2; rc = EVAL(cap); } }
+#undef EVAL
+  if (rc != CG_OK) { free(tmp); napi_throw_error(env, NULL, cg_last_error()); return NULL; }
+  if (napi_create_arraybuffer(env, (size_t)nm * 8, &mdata, &mab) != napi_ok) { free(tmp); napi_throw_error(env, NULL, "N-API call failed"); return NULL; }
+  memcpy(mdata, tmp, (size_t)nm * 8); free(tmp);
+  NAPI_CALL(env, napi_create_typedarray(env, napi_uint32_array, n_ctx, vab, 0, &verdicts));
+  NAPI_CALL(env, napi_create_typedarray(env, napi_uint32_array, (size_t)nm * 2, mab, 0, &matches));
+  NAPI_CALL(env, napi_create_object(env, &out));
+  NAPI_CALL(env, napi_set_named_property(env, out, "verdicts", verdicts));
+  NAPI_CALL(env, napi_set_named_property(env, out, "matches", matches));
+  return out;
+}
 
 static napi_value js_sha256_batch(napi_env env, napi_callback_info info) {
   ARGS(env, info, 2)
@@ -537,6 +585,7 @@ static napi_value module_init(napi_env env, napi_value exports) {
     FN("setPolicy", js_set_policy), FN("verdictBatch", js_verdict_batch),
     FN("setViews", js_set_views), FN("scanBatchViews", js_scan_batch_views), FN("findMatchesBatchViews", js_find_matches_batch_views),
     FN("redactBatchViews", js_redact_batch_views), FN("verdictBatchViews", js_verdict_batch_views),
+    FN("setPolicyProgram", js_set_policy_program), FN("policyEvalBatch", js_policy_eval_batch),
     FN("sha256Batch", js_sha256_batch), FN("merkleRoot", js_merkle_root),
     FN("logCreate", js_log_create), FN("logRestore", js_log_restore), FN("logAppend", js_log_append), FN("logAppendJsonl", js_log_append_jsonl),
     FN("logReserve", js_log_reserve), FN("logSize", js_log_size), FN("logRoot", js_log_root), FN("logFrontier", js_log_frontier),

@@ -44,6 +44,8 @@ class cg_stats(C.Structure):
 
 
 HIT_DTYPE = np.dtype([("msg", np.uint32), ("rule", np.uint32)])
+POLICY_MATCH_DTYPE = np.dtype([("ctx", np.uint32), ("rule", np.uint32)])          # cg_policy_match
+POL_CONST, POL_ATOM, POL_HIT, POL_AND, POL_OR, POL_NOT = 0, 1, 2, 3, 4, 5          # policy program ops (openclaw_gov.h)
 SPAN_DTYPE = np.dtype([("msg", np.uint32), ("rule", np.uint32), ("start_byte", np.uint32), ("end_byte", np.uint32),
                        ("start16", np.uint32), ("end16", np.uint32)])
 
@@ -62,7 +64,8 @@ EXPORTS = ["cg_init", "cg_shutdown", "cg_last_error", "cg_version", "cg_device_c
            "cg_policy_verdict_batch_views", "cg_scan_hits_batch_device_views", "cg_find_matches_batch_device_views",
            "cg_redact_batch_device_views", "cg_policy_verdict_batch_device_views",
            "cg_merkle_log_append_device", "cg_merkle_log_append_fixed_device", "cg_merkle_log_root_device", "cg_merkle_log_proofs_device",
-           "cg_merkle_log_consistency_between_device", "cg_merkle_verify_proofs_device", "cg_merkle_log_join"]
+           "cg_merkle_log_consistency_between_device", "cg_merkle_verify_proofs_device", "cg_merkle_log_join",
+           "cg_ruleset_set_policy_program", "cg_policy_eval_batch", "cg_policy_eval_batch_device"]
 
 _lib = None
 
@@ -156,6 +159,9 @@ def load():
     L.cg_merkle_log_consistency_between_device.argtypes = [vp, u64, u64, vp, u32, vp, vp]; L.cg_merkle_log_consistency_between_device.restype = i32
     L.cg_merkle_verify_proofs_device.argtypes = [vp, vp, vp, u32, u64, vp, u32, vp, vp, vp, vp]; L.cg_merkle_verify_proofs_device.restype = i32
     L.cg_merkle_log_join.argtypes = [vp, vp]; L.cg_merkle_log_join.restype = i32
+    L.cg_ruleset_set_policy_program.argtypes = [vp, vp, u32, u32]; L.cg_ruleset_set_policy_program.restype = i32
+    L.cg_policy_eval_batch.argtypes = [vp, vp, vp, vp, u32, vp, vp, u32, vp, vp, u32, C.POINTER(u32)]; L.cg_policy_eval_batch.restype = i32
+    L.cg_policy_eval_batch_device.argtypes = [vp, vp, vp, vp, u32, vp, vp, u32, vp, vp, u32, vp, vp]; L.cg_policy_eval_batch_device.restype = i32
     _lib = L
     return L
 
@@ -360,6 +366,49 @@ class Ruleset:
             ids = _ids(views, n)
             check(load().cg_policy_verdict_batch_views(self.handle, data.ctypes.data, off.ctypes.data, ids.ctypes.data, n, out.ctypes.data))
         return out[:n]
+
+    def set_policy_program(self, program, n_atoms: int):
+        """cg_ruleset_set_policy_program: program = uint32 words (layout in openclaw_gov.h), n_atoms = atom bits per context."""
+        prog = np.ascontiguousarray(program, dtype=np.uint32)
+        check(load().cg_ruleset_set_policy_program(self.handle, prog.ctypes.data, len(prog), n_atoms))
+        self.n_atoms = int(n_atoms)
+
+    def eval_batch(self, data: np.ndarray, off: np.ndarray, roles, ctx_off, atoms, want_matches: bool = True):
+        """cg_policy_eval_batch: texts (data, off) with one role each, contexts = ranges ctx_off[n_ctx + 1] of the texts, atom
+        rows atoms[n_ctx, ceil(n_atoms / 32)] (uint32).  -> (verdict words uint32[n_ctx], matches POLICY_MATCH_DTYPE sorted by
+        (ctx, program rule); empty without want_matches)."""
+        n = len(off) - 1
+        roles = np.ascontiguousarray(roles, dtype=np.uint8).reshape(-1)
+        ctx_off = np.ascontiguousarray(ctx_off, dtype=np.uint32)
+        atoms = np.ascontiguousarray(atoms, dtype=np.uint32)
+        if len(roles) != n:
+            raise ValueError("roles: %d for a batch of %d texts" % (len(roles), n))
+        n_ctx = len(ctx_off) - 1
+        aw = (getattr(self, "n_atoms", 0) + 31) // 32
+        if atoms.size != n_ctx * aw:
+            raise ValueError("atoms: %d words for %d contexts of %d words" % (atoms.size, n_ctx, aw))
+        verdicts = np.zeros(max(n_ctx, 1), dtype=np.uint32)
+        nm = C.c_uint32(0)
+        cap = 1024
+        while True:
+            matches = np.zeros(cap, dtype=POLICY_MATCH_DTYPE)
+            rc = load().cg_policy_eval_batch(self.handle, data.ctypes.data, off.ctypes.data, roles.ctypes.data if n else None, n,
+                                             ctx_off.ctypes.data, atoms.ctypes.data if atoms.size else None, n_ctx, verdicts.ctypes.data,
+                                             matches.ctypes.data if want_matches else None, cap, C.byref(nm) if want_matches else None)
+            if rc == CG_ERR_CAPACITY and nm.value > cap:
+                cap = nm.value
+                continue
+            check(rc)
+            return verdicts[:n_ctx], matches[:nm.value] if want_matches else matches[:0]
+
+    def eval_batch_device(self, d_bytes: int, d_off: int, d_roles: int, n_texts: int, d_ctx_off: int, d_atoms: int, n_ctx: int,
+                          d_verdicts: int, d_matches: int = 0, matches_cap: int = 0, d_nmatches: int = 0, stream: int = 0):
+        """cg_policy_eval_batch_device on raw device pointers (asynchronous; status from scan_join): one uint32 verdict per
+        context into d_verdicts, the (ctx, rule) matches (POLICY_MATCH_DTYPE, at most matches_cap) into d_matches and their
+        number (uint32) into d_nmatches (d_nmatches = 0: verdicts only)."""
+        check(load().cg_policy_eval_batch_device(self.handle, d_bytes or None, d_off or None, d_roles or None, n_texts, d_ctx_off or None,
+                                                 d_atoms or None, n_ctx, d_verdicts or None, d_matches or None, matches_cap,
+                                                 d_nmatches or None, stream))
 
     def redact_batch(self, data: np.ndarray, off: np.ndarray, views=None):
         """RedactionEngine.scanString for a batch, spliced on the device.  views: one view id per message

@@ -54,6 +54,11 @@ struct Ctx {
   uint32_t* d_verdicts = nullptr; size_t cap_verdicts = 0;
   uint32_t* d_hits = nullptr; size_t cap_hits = 0;          // cg_scan_batch's hit list: [count][(msg, rule) pairs]
   uint8_t* d_views = nullptr; size_t cap_views = 0;         // the host-buffer *_views calls' view ids, staged beside the offsets
+  // cg_policy_eval_batch staging: text roles, context offsets, atom rows, [count][(ctx, rule) pairs]
+  uint8_t* d_proles = nullptr; size_t cap_proles = 0;
+  uint32_t* d_pctx = nullptr; size_t cap_pctx = 0;
+  uint32_t* d_patoms = nullptr; size_t cap_patoms = 0;
+  uint32_t* d_pmatch = nullptr; size_t cap_pmatch = 0;
 } G;
 
 int fail(int code, const std::string& msg) { g_err = msg; return code; }
@@ -155,8 +160,10 @@ struct cg_ruleset {
   uint64_t graph_clock = 0;
   // cg_ruleset_set_views: n_views rows of dev.rw words in HBM (bit r of row v = rule r is in view v); none before the first call
   uint32_t* view_rows = nullptr; uint32_t n_views = 0;
+  // cg_ruleset_set_policy_program: the program's words and one rule record per program rule (kernels.h PolicyTable) in HBM
+  uint32_t* prog_ops = nullptr; uint4* prog_rules = nullptr; uint32_t prog_n_rules = 0, prog_n_atoms = 0;
   ~cg_ruleset() {
-    cudaFree(view_rows);
+    cudaFree(view_rows); cudaFree(prog_ops); cudaFree(prog_rules);
     for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     for (auto& g : one.g) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (one.h_pin) cudaFreeHost(one.h_pin);
@@ -279,14 +286,15 @@ void default_caps(const cg_ruleset* rs, uint32_t n, StepKind kind, uint32_t* l1,
   *ev = std::max(std::max<uint32_t>(std::max<uint32_t>(n, 4096), rs->work.event_cap), rs->grow_ev);
   *span = kind == kStepSpans ? std::max(std::max<uint32_t>(std::max<uint32_t>(n, 4096), rs->work.span_cap), rs->grow_span) : 1;
 }
-// the verify grid and the scratch of a step over n messages; growing waits for st (nothing may still use a replaced buffer)
-int prepare_step(cg_ruleset* rs, uint32_t n, StepKind kind, cudaStream_t st) {
+// the verify grid and the scratch of a step over n messages, with per-message scratch for at least res_min items behind a
+// policy step; growing waits for st (nothing may still use a replaced buffer)
+int prepare_step(cg_ruleset* rs, uint32_t n, StepKind kind, cudaStream_t st, uint32_t res_min = 0) {
   rs->size_verify_grid();
   const ScanWork& w = rs->work;
   uint32_t l1, slot, ev, span;
   default_caps(rs, n, kind, &l1, &slot, &ev, &span);
   n = std::max<uint32_t>(n, 1);
-  const uint32_t res = kind != kStepWords ? n : 0;
+  const uint32_t res = kind != kStepWords ? std::max(n, res_min) : 0;
   if (n <= w.msg_cap && l1 <= w.l1_cap && slot <= w.slot_cap && ev <= w.event_cap && span <= w.span_cap && res <= w.res_cap) return CG_OK;
   CU(cudaStreamSynchronize(st));
   return ensure_work(rs, rs->work, n, l1, slot, ev, span, res);
@@ -349,9 +357,10 @@ int check_offsets(const uint32_t* offsets, uint32_t n) {
 // words to G.d_words, a span step's to the scratch), the work after(scratch) enqueues behind it (-> CG_OK or an error; it
 // may copy sizes to the host, never into the caller's buffers), the counter block to the host and one synchronise.  A
 // queue overflow grows the scratch and runs the attempt again.  last_scan_ms times the step alone.  views (one id per message,
-// checked by the caller): staged beside the offsets, the step filtered by them.
+// checked by the caller): staged beside the offsets, the step filtered by them.  res_min: as prepare_step.
 template <typename After>
-int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, StepKind kind, After&& after, const uint8_t* views = nullptr) {
+int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, StepKind kind, After&& after, const uint8_t* views = nullptr,
+              uint32_t res_min = 0) {
   if (int rc = require_ready()) return rc;
   if (!rs || (n && (!bytes || !offsets))) return fail(CG_ERR_INVALID_ARG, "null argument");
   int rc;
@@ -371,7 +380,7 @@ int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uin
   const ViewTable vt{rs->view_rows, G.d_views, rs->n_views};
   uint32_t hc[kCounterWords] = {};
   for (int attempt = 0; attempt < 10; attempt++) {
-    if ((rc = prepare_step(rs, n, kind, st))) return rc;
+    if ((rc = prepare_step(rs, n, kind, st, res_min))) return rc;
     const ScanWork& w = rs->work;
     CU(cudaEventRecord(G.ev0, st));
     if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32, n, kind == kStepSpans ? w.words : G.d_words, kind, st, views ? &vt : nullptr))) return rc;
@@ -544,16 +553,16 @@ int replay_step(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint
 // the step of `kind` (replayed as a graph when `graph`), the work after(scratch) enqueues behind it (-> its launch count)
 // and the counter block into the mirror ring.  Result words go to d_words, or when it is null to the scratch's (looked up
 // after prepare_step, which may replace that buffer).  Never waits for the device except when the scratch must grow.  views:
-// the step filtered by them (never replayed as a graph).
+// the step filtered by them (never replayed as a graph).  res_min: as prepare_step.
 template <typename After>
 int scan_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, uint64_t* d_words, StepKind kind, cudaStream_t st,
-                After&& after, bool graph = false, const ViewTable* views = nullptr) {
+                After&& after, bool graph = false, const ViewTable* views = nullptr, uint32_t res_min = 0) {
   InOrder turn(&rs->order, st);
   int rc;
   if ((rc = turn.rc)) return rc;
   if ((rc = ensure_mirrors(rs))) return rc;
   poll_mirrors(rs, false);                                  // (an earlier batch overflowed?  grow before this one runs)
-  if ((rc = prepare_step(rs, n, kind, st))) return rc;
+  if ((rc = prepare_step(rs, n, kind, st, res_min))) return rc;
   if (!d_words) d_words = rs->work.words;
   const auto step = [&] { return run_scan_device(rs, (const uint8_t*)d_bytes, (const uint32_t*)d_offsets, n, d_words, kind, st, views); };
   if ((rc = graph ? replay_step(rs, d_bytes, d_offsets, n, d_words, st, step) : step())) return rc;
@@ -620,6 +629,7 @@ void cg_shutdown(void) {
   if (!G.ready) return;
   cudaDeviceSynchronize();
   cudaFree(G.d_spans); cudaFree(G.d_redact_out); cudaFree(G.d_redact_meta); cudaFree(G.d_verdicts); cudaFree(G.d_hits); cudaFree(G.d_views);
+  cudaFree(G.d_proles); cudaFree(G.d_pctx); cudaFree(G.d_patoms); cudaFree(G.d_pmatch);
   if (G.h_chunk_counters) cudaFreeHost(G.h_chunk_counters);
   if (G.s_h2d) { cudaStreamDestroy(G.s_h2d); cudaStreamDestroy(G.s_d2h); for (int c = 0; c < Ctx::kChunks; c++) { cudaEventDestroy(G.e_h2d[c]); cudaEventDestroy(G.e_done[c]); } }
   cudaFree(G.d_bytes_raw); cudaFree(G.d_off32); cudaFree(G.d_off64); cudaFree(G.d_words); cudaFree(G.d_dig[0]); cudaFree(G.d_dig[1]);
@@ -1317,6 +1327,151 @@ int cg_policy_verdict_batch_device_views(cg_ruleset* rs, const void* d_bytes, co
   ViewTable vt;
   if (int rc = device_views_args(rs, d_bytes, d_offsets, d_views, &vt)) return rc;
   return verdict_device(rs, d_bytes, d_offsets, n, d_out_verdicts, stream, &vt);
+}
+
+// ---------------------------------------------------------------------------------- policy programs
+
+int cg_ruleset_set_policy_program(cg_ruleset* rs, const uint32_t* program, uint32_t words, uint32_t n_atoms) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  if (int rc = require_ready()) return rc;
+  if (!rs || !program || !words) return fail(CG_ERR_INVALID_ARG, "null argument");
+  const auto bad = [](const std::string& m) { return fail(CG_ERR_INVALID_ARG, "policy program: " + m); };
+  std::vector<uint4> rules;
+  uint32_t at = 1;
+  const uint32_t n_pol = program[0];
+  for (uint32_t p = 0; p < n_pol; p++) {
+    if (words - at < 2) return bad("policy " + std::to_string(p) + " runs past the end");
+    const uint32_t scope = program[at], n_rules = program[at + 1];
+    at += 2;
+    if (scope != 0xffffffffu && scope >= n_atoms) return bad("policy " + std::to_string(p) + ": scope atom >= n_atoms");
+    const uint32_t first = (uint32_t)rules.size();
+    for (uint32_t r = 0; r < n_rules; r++) {
+      const std::string where = "policy " + std::to_string(p) + " rule " + std::to_string(r);
+      if (rules.size() >= (1u << 20) - 1) return fail(CG_ERR_TOO_LARGE, "policy program: more than 2^20 - 1 rules");
+      if (words - at < 2) return bad(where + " runs past the end");
+      const uint32_t head = program[at], n_ops = program[at + 1];
+      at += 2;
+      if (head > 7u) return bad(where + ": effect word must be action | has_reason << 2");
+      if (n_ops > words - at) return bad(where + ": ops run past the end");
+      if (n_ops > 0xffffffu) return fail(CG_ERR_TOO_LARGE, "policy program: " + where + " has 2^24 ops or more");
+      uint32_t depth = 0;
+      for (uint32_t k = 0; k < n_ops; k++) {
+        const uint32_t o = program[at + k], code = o & 7u;
+        if (code == kPolOpConst || code == kPolOpAtom || code == kPolOpHit) {
+          if (code == kPolOpConst && (o >> 3) > 1u) return bad(where + ": CONST takes 0 or 1");
+          if (code == kPolOpAtom && (o >> 3) >= n_atoms) return bad(where + ": atom >= n_atoms");
+          if (code == kPolOpHit && ((o >> 3) & 0x1fffffu) >= rs->dev.n_rules) return bad(where + ": HIT rule >= the rule set's rules");
+          if (++depth > 32) return fail(CG_ERR_TOO_LARGE, "policy program: " + where + " needs a stack deeper than 32");
+        } else if (code == kPolOpAnd || code == kPolOpOr || code == kPolOpNot) {
+          if (o >> 3) return bad(where + ": AND / OR / NOT take no operand");
+          if (depth < (code == kPolOpNot ? 1u : 2u)) return bad(where + ": stack underflow");
+          if (code != kPolOpNot) depth--;
+        } else {
+          return bad(where + ": unknown op " + std::to_string(code));
+        }
+      }
+      if (depth != 1) return bad(where + " must leave exactly one value");
+      rules.push_back(make_uint4(at, n_ops | (head & 3u) << 24 | (head >> 2) << 26, first, scope));
+      at += n_ops;
+    }
+  }
+  if (at != words) return bad("words past the last policy");
+  CU(cudaStreamSynchronize(G.stream));
+  cudaFree(rs->prog_ops); cudaFree(rs->prog_rules); rs->prog_ops = nullptr; rs->prog_rules = nullptr; rs->prog_n_rules = rs->prog_n_atoms = 0;
+  CU(cudaMalloc((void**)&rs->prog_ops, (size_t)words * 4));
+  CU(cudaMalloc((void**)&rs->prog_rules, std::max<size_t>(rules.size(), 1) * sizeof(uint4)));
+  CU(cudaMemcpy(rs->prog_ops, program, (size_t)words * 4, cudaMemcpyHostToDevice));
+  if (!rules.empty()) CU(cudaMemcpy(rs->prog_rules, rules.data(), rules.size() * sizeof(uint4), cudaMemcpyHostToDevice));
+  rs->prog_n_rules = (uint32_t)rules.size(); rs->prog_n_atoms = n_atoms;
+  return CG_OK;
+}
+
+namespace {
+PolicyTable policy_table(const cg_ruleset* rs) { return PolicyTable{rs->prog_ops, rs->prog_rules, rs->prog_n_rules, (rs->prog_n_atoms + 31) / 32}; }
+
+int policy_eval_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, const uint8_t* roles, uint32_t n_texts, const uint32_t* ctx_offsets,
+                     const uint32_t* atoms, uint32_t n_ctx, uint32_t* out_verdicts, cg_policy_match* out_matches, uint32_t matches_cap, uint32_t* out_nmatches) {
+  if (int rc = require_ready()) return rc;
+  if (!rs) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (!rs->prog_ops) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy_program has not been called");
+  const PolicyTable pt = policy_table(rs);
+  if (!ctx_offsets || (n_texts && !roles) || (n_ctx && (!out_verdicts || (pt.aw && !atoms)))) return fail(CG_ERR_INVALID_ARG, "null argument");
+  for (uint32_t c = 0; c < n_ctx; c++)
+    if (ctx_offsets[c] > ctx_offsets[c + 1] || ctx_offsets[c + 1] > n_texts) return fail(CG_ERR_INVALID_ARG, "context " + std::to_string(c) + ": text range decreasing or past n_texts");
+  const bool want = out_matches || out_nmatches;
+  if (!n_ctx) { if (out_nmatches) *out_nmatches = 0; return CG_OK; }
+  cudaStream_t st = G.stream;
+  InOrder turn(&rs->order, st);
+  if (turn.rc) return turn.rc;
+  int rc;
+  if ((rc = grow(&G.d_proles, &G.cap_proles, (size_t)n_texts + 1))) return rc;
+  if ((rc = grow(&G.d_pctx, &G.cap_pctx, (size_t)n_ctx + 1))) return rc;
+  if ((rc = grow(&G.d_patoms, &G.cap_patoms, (size_t)n_ctx * pt.aw + 1))) return rc;
+  if ((rc = grow(&G.d_verdicts, &G.cap_verdicts, (size_t)n_ctx))) return rc;
+  if (n_texts) CU(cudaMemcpyAsync(G.d_proles, roles, n_texts, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(G.d_pctx, ctx_offsets, ((size_t)n_ctx + 1) * 4, cudaMemcpyHostToDevice, st));
+  if (pt.aw) CU(cudaMemcpyAsync(G.d_patoms, atoms, (size_t)n_ctx * pt.aw * 4, cudaMemcpyHostToDevice, st));
+  const PolicyBatch b{G.d_proles, n_texts, G.d_pctx, G.d_patoms, n_ctx};
+  uint64_t total = 0;
+  rc = scan_host(rs, bytes, offsets, n_texts, kStepPolicy, [&](const ScanWork& w) {
+    count_launches(launch_policy_eval(pt, w, rs->dev.rw, b, G.d_verdicts, want, G.sm_count, st));
+    CU(cudaGetLastError());
+    if (want) CU(cudaMemcpyAsync(&total, w.out_off + n_ctx, 8, cudaMemcpyDeviceToHost, st));
+    return CG_OK;
+  }, nullptr, n_ctx);
+  if (rc) return rc;
+  CU(cudaMemcpyAsync(out_verdicts, G.d_verdicts, (size_t)n_ctx * 4, cudaMemcpyDeviceToHost, st));
+  const uint32_t k = out_matches && !(total >> 32) ? (uint32_t)std::min<uint64_t>(total, matches_cap) : 0u;
+  if (want) {                                                // (emit runs whatever the count: launches do not depend on it)
+    if ((rc = grow(&G.d_pmatch, &G.cap_pmatch, 2 * (size_t)k + 1))) return rc;      // [count][pairs]
+    count_launches(launch_policy_emit(pt, rs->work, rs->dev.rw, b, G.d_pmatch + 1, k, G.d_pmatch, G.sm_count, st));
+    CU(cudaGetLastError());
+    if (k) CU(cudaMemcpyAsync(out_matches, G.d_pmatch + 1, (size_t)k * sizeof(cg_policy_match), cudaMemcpyDeviceToHost, st));
+  }
+  CU(cudaStreamSynchronize(st));
+  if (total >> 32) { if (out_nmatches) *out_nmatches = 0xffffffffu; return fail(CG_ERR_TOO_LARGE, "2^32 matches or more in one batch"); }
+  if (out_nmatches) *out_nmatches = (uint32_t)total;
+  if (out_matches && total > matches_cap) return fail(CG_ERR_CAPACITY, "out_matches too small (see *out_nmatches)");
+  return CG_OK;
+}
+
+int policy_eval_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, const void* d_roles, uint32_t n_texts, const void* d_ctx_offsets,
+                       const void* d_atoms, uint32_t n_ctx, void* d_out_verdicts, void* d_out_matches, uint32_t matches_cap, void* d_out_nmatches,
+                       void* stream) {
+  if (int rc = require_ready()) return rc;
+  if (!rs) return fail(CG_ERR_INVALID_ARG, "null argument");
+  if (!rs->prog_ops) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy_program has not been called");
+  const PolicyTable pt = policy_table(rs);
+  if ((n_texts && (!d_bytes || !d_offsets || !d_roles)) || !d_ctx_offsets || (n_ctx && (!d_out_verdicts || (pt.aw && !d_atoms))) ||
+      (matches_cap && !d_out_matches) || (d_out_matches && !d_out_nmatches))
+    return fail(CG_ERR_INVALID_ARG, "null argument");
+  if ((uintptr_t)d_bytes & 15u) return fail(CG_ERR_INVALID_ARG, "d_bytes must be 16-byte aligned");
+  if (((uintptr_t)d_offsets | (uintptr_t)d_ctx_offsets | (uintptr_t)d_atoms | (uintptr_t)d_out_verdicts | (uintptr_t)d_out_matches | (uintptr_t)d_out_nmatches) & 3u)
+    return fail(CG_ERR_INVALID_ARG, "d_offsets, d_ctx_offsets, d_atoms and the outputs must be 4-byte aligned");
+  cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
+  const bool want = d_out_nmatches != nullptr;
+  if (!n_ctx) { if (want) CU(cudaMemsetAsync(d_out_nmatches, 0, 4, st)); return CG_OK; }
+  const PolicyBatch b{(const uint8_t*)d_roles, n_texts, (const uint32_t*)d_ctx_offsets, (const uint32_t*)d_atoms, n_ctx};
+  return scan_device(rs, d_bytes, d_offsets, n_texts, nullptr, kStepPolicy, st, [&](const ScanWork& w) {
+    int k = launch_policy_eval(pt, w, rs->dev.rw, b, (uint32_t*)d_out_verdicts, want, G.sm_count, st);
+    if (want) k += launch_policy_emit(pt, w, rs->dev.rw, b, (uint32_t*)d_out_matches, d_out_matches ? matches_cap : 0u, (uint32_t*)d_out_nmatches, G.sm_count, st);
+    return k;
+  }, false, nullptr, n_ctx);
+}
+}  // namespace
+
+int cg_policy_eval_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, const uint8_t* roles, uint32_t n_texts, const uint32_t* ctx_offsets,
+                         const uint32_t* atoms, uint32_t n_ctx, uint32_t* out_verdicts, cg_policy_match* out_matches, uint32_t matches_cap, uint32_t* out_nmatches) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return policy_eval_host(rs, bytes, offsets, roles, n_texts, ctx_offsets, atoms, n_ctx, out_verdicts, out_matches, matches_cap, out_nmatches);
+}
+
+int cg_policy_eval_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, const void* d_roles, uint32_t n_texts, const void* d_ctx_offsets,
+                                const void* d_atoms, uint32_t n_ctx, void* d_out_verdicts, void* d_out_matches, uint32_t matches_cap, void* d_out_nmatches,
+                                void* stream) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  return policy_eval_device(rs, d_bytes, d_offsets, d_roles, n_texts, d_ctx_offsets, d_atoms, n_ctx, d_out_verdicts, d_out_matches, matches_cap,
+                            d_out_nmatches, stream);
 }
 
 // ---------------------------------------------------------------------------------- SHA / Merkle

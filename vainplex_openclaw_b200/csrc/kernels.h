@@ -150,6 +150,24 @@ int launch_verdicts(const DevRuleset& rs, const ScanWork& w, uint32_t* d_verdict
 int launch_hit_count(const ScanWork& w, const uint64_t* d_words, uint32_t n, int sm_count, cudaStream_t stream);
 int launch_hit_emit(const DevRuleset& rs, const ScanWork& w, uint32_t n, uint32_t* d_out, uint32_t cap, uint32_t* d_count, int sm_count, cudaStream_t stream);
 int launch_finalize(const DevRuleset& rs, const ScanWork& w, uint64_t* d_words, uint32_t n, int sm_count, cudaStream_t stream);
+
+// Policy programs (cg_ruleset_set_policy_program; layout and op words in openclaw_gov.h).  Passed by value to the policy
+// kernels only (policy_eval.cu), as ViewTable is.  rules[j] for program rule j: x = its first op word in ops, y = n_ops |
+// action << 24 | has_reason << 26, z = the first program rule of its policy, w = its policy's scope atom (0xffffffff: none).
+enum : uint32_t { kPolOpConst = 0, kPolOpAtom = 1, kPolOpHit = 2, kPolOpAnd = 3, kPolOpOr = 4, kPolOpNot = 5 };
+struct PolicyTable { const uint32_t* ops; const uint4* rules; uint32_t n_rules; uint32_t aw; /* atom words per context */ };
+// the contexts of a cg_policy_eval_batch call (device pointers): text i has role roles[i]; context c owns texts
+// [ctx_off[c], ctx_off[c + 1]) of the step just run and atom row atoms[c * aw ..]
+struct PolicyBatch { const uint8_t* roles; uint32_t n_texts; const uint32_t* ctx_off; const uint32_t* atoms; uint32_t n_ctx; };
+// behind a finished policy-mode step over the texts (w.res_cap >= n_ctx): one verdict word per context (openclaw_gov.h); with
+// counts also the matches per context into w.out_len and their exclusive scan into w.out_off (w.out_off[n_ctx] = the total)
+int launch_policy_eval(const PolicyTable& pt, const ScanWork& w, uint32_t rw, const PolicyBatch& b, uint32_t* d_verdicts, bool counts, int sm_count,
+                       cudaStream_t stream);
+// then the (context, program rule) matches, the first cap of them, as two u32 each into d_out, the total into *d_count
+// (0xffffffff: incomplete step, or 2^32 - 1 matches or more), the status into counters[kCtrResolveStatus].  Grids depend on
+// n_ctx and the SM count only.
+int launch_policy_emit(const PolicyTable& pt, const ScanWork& w, uint32_t rw, const PolicyBatch& b, uint32_t* d_out, uint32_t cap, uint32_t* d_count,
+                       int sm_count, cudaStream_t stream);
 // start of a step: counters = 0, slot_of_msg = none, candidate / hit rows of the slots the previous step used = 0
 int launch_reset(const DevRuleset& rs, const ScanWork& w, uint32_t n, int sm_count, cudaStream_t stream);
 

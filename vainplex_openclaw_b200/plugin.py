@@ -599,6 +599,10 @@ def _glob_match(pattern: str, value: str) -> bool:
     return re.fullmatch(esc, value) is not None
 
 
+def _as_list(v) -> list:
+    return v if isinstance(v, list) else [v]
+
+
 class PolicyEvaluator:
     """policy-evaluator.ts:18-146 with every text test routed to the device in ONE batch per call:
 
@@ -656,6 +660,180 @@ class PolicyEvaluator:
                 self.tool_rule[pat] = len(rules)
                 rules.append([pat])
         self.scanner = (scanner_cls or RuleScanner)(rules, logger) if rules else None
+        self._compile_program()
+        self._program_rs = None          # the rule set verdict_batch evaluates the program on (the scanner's, or an empty one)
+
+    # -- the policy program (cg_ruleset_set_policy_program, openclaw_gov.h): verdict_batch evaluates every policy on the device
+    ACTION_CODE = {"allow": 0, "audit": 1, "2fa": 2, "deny": 3}
+
+    def _compile_program(self) -> None:
+        """Policies in evaluation order (sortPolicies, policy-evaluator.ts:36-42: it depends on the policy alone and scope
+        only removes policies, so one order serves every context), each rule's gates and conditions as a postfix program over
+        HIT(rule, role) leaves for the regex tests and atoms for every other test (the helpers _cond and _evaluate call).
+        Sets self.program (uint32 words), self.atoms ([ctx -> bool], one per atom id), self.param_role (tool-param key ->
+        role 2 + k) and self.program_rules ((policy, rule) per program rule)."""
+        atom_id: Dict[tuple, int] = {}
+        self.atoms: List[Callable[[dict], bool]] = []
+        self.param_role: Dict[str, int] = {}
+
+        def atom_index(key: tuple, fn) -> int:
+            if key not in atom_id:
+                atom_id[key] = len(self.atoms)
+                self.atoms.append(fn)
+            return atom_id[key]
+
+        def atom(key: tuple, fn) -> List[int]:
+            return [N.POL_ATOM | atom_index(key, fn) << 3]
+
+        def hit(rule: int, role: int) -> List[int]:
+            return [N.POL_HIT | rule << 3 | role << 24]
+
+        def fold(parts: List[List[int]], op: int, empty: int) -> List[int]:
+            if not parts:
+                return [N.POL_CONST | empty << 3]
+            out = list(parts[0])
+            for q in parts[1:]:
+                out += q + [op]
+            return out
+
+        def canon(v) -> str:
+            return json.dumps(v, sort_keys=True, default=repr)
+
+        def role_of(key: str) -> int:
+            if key not in self.param_role:
+                if len(self.param_role) >= 254:
+                    raise ValueError("more than 254 tool-param keys with a `matches` test")
+                self.param_role[key] = 2 + len(self.param_role)
+            return self.param_role[key]
+
+        def cond(c: dict) -> List[int]:
+            t = c.get("type")
+            parts: List[List[int]] = []
+            if t == "context":
+                for key, role in (("conversationContains", 1), ("messageContains", 0)):
+                    if c.get(key) is not None:
+                        parts.append(fold([hit(self.pattern_rule[p], role) for p in _as_list(c[key])], N.POL_OR, 0))
+                if c.get("hasMetadata") is not None:
+                    k = _as_list(c["hasMetadata"])
+                    parts.append(atom(("hasMetadata", canon(k)), lambda ctx, k=k: self._has_metadata(k, ctx)))
+                if c.get("channel") is not None:
+                    k = _as_list(c["channel"])
+                    parts.append(atom(("channel", canon(k)), lambda ctx, k=k: self._in_channel(k, ctx)))
+                if c.get("sessionKey") is not None:
+                    k = c["sessionKey"]
+                    parts.append(atom(("sessionKey", k), lambda ctx, k=k: self._session_key(k, ctx)))
+                return fold(parts, N.POL_AND, 1)
+            if t == "tool":
+                if c.get("name") is not None:
+                    k = _as_list(c["name"])
+                    parts.append(atom(("toolName", canon(k)), lambda ctx, k=k: self._tool_name(k, ctx)))
+                if c.get("params"):
+                    parts.append(atom(("hasParams",), self._has_params))
+                    for key, m in c["params"].items():
+                        if "matches" in m and "equals" not in m and "contains" not in m:
+                            pat = m["matches"]
+                            parts.append(hit(self.tool_rule[pat], role_of(key)) if pat in self.tool_rule else [N.POL_CONST])
+                        else:
+                            parts.append(atom(("param", key, canon(m)), lambda ctx, key=key, m=m: self._param_test(key, m, ctx)))
+                return fold(parts, N.POL_AND, 1)
+            if t == "agent":
+                if c.get("id") is not None:
+                    k = _as_list(c["id"])
+                    parts.append(atom(("agentId", canon(k)), lambda ctx, k=k: self._agent_id_in(k, ctx)))
+                if c.get("trustTier") is not None:
+                    k = _as_list(c["trustTier"])
+                    parts.append(atom(("agentTier", canon(k)), lambda ctx, k=k: self._agent_tier_in(k, ctx)))
+                return fold(parts, N.POL_AND, 1)
+            if t == "any":
+                return fold([cond(sub) for sub in c.get("conditions", [])], N.POL_OR, 0)
+            if t == "not":
+                return cond(c["condition"]) + [N.POL_NOT]
+            return atom(("other", canon(c)), lambda ctx, c=c: bool(self.other(c, ctx)))
+
+        order = sorted(self.policies, key=lambda p: (-(p.get("priority") or 0), -self._specificity(p)))     # stable, as _evaluate
+        words: List[int] = [len(order)]
+        self.program_rules: List[Tuple[dict, dict]] = []
+        for p in order:
+            scope = p.get("scope") or {}
+            if scope.get("excludeAgents") or scope.get("channels"):
+                words.append(atom_index(("scope", canon([scope.get("excludeAgents"), scope.get("channels")])), lambda ctx, p=p: self._matches_scope(p, ctx)))
+            else:
+                words.append(0xffffffff)
+            words.append(len(p.get("rules", [])))
+            for r in p.get("rules", []):
+                parts = []
+                if r.get("minTrust"):
+                    parts.append(atom(("minTrust", r["minTrust"]), lambda ctx, t=r["minTrust"]: self._min_trust(t, ctx)))
+                if r.get("maxTrust"):
+                    parts.append(atom(("maxTrust", r["maxTrust"]), lambda ctx, t=r["maxTrust"]: self._max_trust(t, ctx)))
+                ops = fold(parts + [cond(c) for c in r.get("conditions", [])], N.POL_AND, 1)
+                eff = r.get("effect", {"action": "allow"})
+                words += [self.ACTION_CODE.get(eff.get("action"), 0) | (4 if eff.get("reason") else 0), len(ops)] + ops
+                self.program_rules.append((p, r))
+        self.program = np.array(words, dtype=np.uint32)
+
+    def program_inputs(self, contexts: Sequence[dict]):
+        """The texts of the contexts with their roles (evaluate_batch's inclusions; a string param whose key no `matches` test
+        names feeds no leaf and is left out), the contexts' text ranges and their atom rows.
+        -> (texts, roles uint8[n_texts], ctx_off uint32[n_ctx + 1], atoms uint32[n_ctx, ceil(n_atoms / 32)])"""
+        texts: List[str] = []
+        roles: List[int] = []
+        ctx_off = np.zeros(len(contexts) + 1, dtype=np.uint32)
+        atoms = np.zeros((len(contexts), (len(self.atoms) + 31) // 32), dtype=np.uint32)
+        for ci, ctx in enumerate(contexts):
+            if ctx.get("messageContent"):
+                texts.append(ctx["messageContent"]); roles.append(0)
+            for t in ctx.get("conversationContext") or []:
+                texts.append(t); roles.append(1)
+            for key, val in (ctx.get("toolParams") or {}).items():
+                if isinstance(val, str) and key in self.param_role:
+                    texts.append(val); roles.append(self.param_role[key])
+            ctx_off[ci + 1] = len(texts)
+            for a, fn in enumerate(self.atoms):
+                if fn(ctx):
+                    atoms[ci, a >> 5] |= np.uint32(1 << (a & 31))
+        return texts, np.array(roles, dtype=np.uint8), ctx_off, atoms
+
+    def decode_verdicts(self, words, matches) -> List[dict]:
+        """verdict words and the (ctx, rule) match list -> what evaluate_batch returns per context (action, reason, matches;
+        the reason of a deny / 2fa is the first non-empty one of that action, aggregateMatches, policy-evaluator.ts:51-60)"""
+        first = np.searchsorted(np.asarray(matches["ctx"]), np.arange(len(words) + 1)) if len(matches) else np.zeros(len(words) + 1, np.int64)
+        out = []
+        for c, v in enumerate(int(x) for x in words):
+            if v >= 0xfffffffe:
+                raise N.GovError(N.CG_ERR_CAPACITY, "context %d has no verdict (0x%08x)" % (c, v))
+            ms = []
+            for j in matches["rule"][int(first[c]):int(first[c + 1])]:
+                p, r = self.program_rules[int(j)]
+                ms.append({"policyId": p["id"], "ruleId": r.get("id"), "effect": r.get("effect", {"action": "allow"}), "controls": p.get("controls") or []})
+            outcome, decide = v & 7, v >> 12
+            if outcome >= 3:
+                action = "deny" if outcome == 4 else "2fa"
+                reason = self.program_rules[decide][1]["effect"]["reason"] if decide != 0xfffff else \
+                    ("Denied by governance policy" if outcome == 4 else "Requires 2FA approval")
+            else:
+                action = "allow"
+                reason = ("No matching policies", "Allowed by governance policy", "Allowed with audit logging")[outcome]
+            out.append({"action": action, "reason": reason, "matches": ms})
+        return out
+
+    def verdict_batch(self, contexts: Sequence[dict]) -> List[dict]:
+        """evaluate_batch's result (action, reason, matches) with the policies evaluated on the device: one policy-mode scan of
+        every text of the batch, then the program for every context (cg_policy_eval_batch); only the verdict words and the
+        match list come back.  Atoms are computed here for every context (a time / risk / frequency callback is called for
+        each context and condition, not only where the host walk would reach it)."""
+        if not contexts:
+            return []
+        if self._program_rs is None:
+            rs = getattr(self.scanner, "ruleset", None) if self.scanner is not None else N.Ruleset([], strict=True)
+            if rs is None:
+                raise TypeError("verdict_batch needs the device RuleScanner")
+            rs.set_policy_program(self.program, len(self.atoms))
+            self._program_rs = rs
+        texts, roles, ctx_off, atoms = self.program_inputs(contexts)
+        data, off = N.pack([N.js_utf8(t) for t in texts])
+        words, matches = self._program_rs.eval_batch(data, off, roles, ctx_off, atoms)
+        return self.decode_verdicts(words, matches)
 
     # -- one batch for all contexts
     def evaluate_batch(self, contexts: Sequence[dict]) -> List[dict]:
@@ -700,13 +878,12 @@ class PolicyEvaluator:
     def _evaluate(self, ctx: dict, hit: dict) -> dict:
         applicable = [p for p in self.policies if self._matches_scope(p, ctx)]
         applicable.sort(key=lambda p: (-(p.get("priority") or 0), -self._specificity(p)))        # stable, like Array.prototype.sort
-        tier = TIER_ORDINAL[((ctx.get("trust") or {}).get("session") or {}).get("tier", "standard")]
         matches = []
         for p in applicable:
             for r in p.get("rules", []):
-                if r.get("minTrust") and not tier >= TIER_ORDINAL[r["minTrust"]]:
+                if r.get("minTrust") and not self._min_trust(r["minTrust"], ctx):
                     continue
-                if r.get("maxTrust") and not tier <= TIER_ORDINAL[r["maxTrust"]]:
+                if r.get("maxTrust") and not self._max_trust(r["maxTrust"], ctx):
                     continue
                 if all(self._cond(c, ctx, hit) for c in r.get("conditions", [])):
                     matches.append({"policyId": p["id"], "ruleId": r.get("id"), "effect": r.get("effect", {"action": "allow"}),
@@ -723,6 +900,64 @@ class PolicyEvaluator:
             return {"action": "allow", "reason": "Allowed with audit logging", "matches": matches}
         return {"action": "allow", "reason": "Allowed by governance policy" if matches else "No matching policies", "matches": matches}
 
+    # -- the scalar tests of conditions/*.ts and the rule gates (matchPolicy, :135-140): _cond / _evaluate call them, and
+    # each distinct one is an atom of the policy program (verdict_batch)
+    @staticmethod
+    def _session_tier(ctx: dict) -> int:
+        return TIER_ORDINAL[((ctx.get("trust") or {}).get("session") or {}).get("tier", "standard")]
+
+    @staticmethod
+    def _min_trust(tier: str, ctx: dict) -> bool:
+        return PolicyEvaluator._session_tier(ctx) >= TIER_ORDINAL[tier]
+
+    @staticmethod
+    def _max_trust(tier: str, ctx: dict) -> bool:
+        return PolicyEvaluator._session_tier(ctx) <= TIER_ORDINAL[tier]
+
+    @staticmethod
+    def _has_metadata(keys, ctx: dict) -> bool:
+        return all(k in (ctx.get("metadata") or {}) for k in keys)
+
+    @staticmethod
+    def _in_channel(chans, ctx: dict) -> bool:
+        return bool(ctx.get("channel")) and ctx["channel"] in chans
+
+    @staticmethod
+    def _session_key(glob: str, ctx: dict) -> bool:
+        return bool(ctx.get("sessionKey")) and _glob_match(glob, ctx["sessionKey"])
+
+    @staticmethod
+    def _tool_name(names, ctx: dict) -> bool:
+        tn = ctx.get("toolName")
+        return bool(tn) and any(_glob_match(p, tn) if ("*" in p or "?" in p) else p == tn for p in names)
+
+    @staticmethod
+    def _has_params(ctx: dict) -> bool:
+        return bool(ctx.get("toolParams"))
+
+    @staticmethod
+    def _param_test(key: str, m: dict, ctx: dict) -> bool:
+        """a param matcher other than `matches` (tool.ts:30-60); `matches` is a scan leaf"""
+        v = (ctx.get("toolParams") or {}).get(key)
+        if "equals" in m:
+            return v == m["equals"] and type(v) == type(m["equals"])
+        if "contains" in m:
+            return isinstance(v, str) and m["contains"] in v
+        if "startsWith" in m:
+            return isinstance(v, str) and v.startswith(m["startsWith"])
+        if "in" in m:
+            return v in m["in"]
+        return False
+
+    @staticmethod
+    def _agent_id_in(ids, ctx: dict) -> bool:
+        aid = ctx.get("agentId", "")
+        return any(_glob_match(p, aid) if ("*" in p or "?" in p) else p == aid for p in ids)
+
+    @staticmethod
+    def _agent_tier_in(tiers, ctx: dict) -> bool:
+        return ((ctx.get("trust") or {}).get("agent") or {}).get("tier", "standard") in tiers
+
     # -- conditions/*.ts
     def _any_pattern(self, patterns, hitset) -> bool:
         return any(self.pattern_rule[p] in hitset for p in ([patterns] if isinstance(patterns, str) else patterns))
@@ -736,55 +971,34 @@ class PolicyEvaluator:
             if c.get("messageContains") is not None:
                 if not ctx.get("messageContent") or not self._any_pattern(c["messageContains"], hit["msg"]):
                     return False
-            if c.get("hasMetadata") is not None:
-                keys = c["hasMetadata"] if isinstance(c["hasMetadata"], list) else [c["hasMetadata"]]
-                if not all(k in (ctx.get("metadata") or {}) for k in keys):
-                    return False
-            if c.get("channel") is not None:
-                chans = c["channel"] if isinstance(c["channel"], list) else [c["channel"]]
-                if not ctx.get("channel") or ctx["channel"] not in chans:
-                    return False
-            if c.get("sessionKey") is not None:
-                if not ctx.get("sessionKey") or not _glob_match(c["sessionKey"], ctx["sessionKey"]):
-                    return False
+            if c.get("hasMetadata") is not None and not self._has_metadata(_as_list(c["hasMetadata"]), ctx):
+                return False
+            if c.get("channel") is not None and not self._in_channel(_as_list(c["channel"]), ctx):
+                return False
+            if c.get("sessionKey") is not None and not self._session_key(c["sessionKey"], ctx):
+                return False
             return True
         if t == "tool":
-            if c.get("name") is not None:
-                tn = ctx.get("toolName")
-                names = c["name"] if isinstance(c["name"], list) else [c["name"]]
-                if not tn or not any(_glob_match(p, tn) if ("*" in p or "?" in p) else p == tn for p in names):
-                    return False
+            if c.get("name") is not None and not self._tool_name(_as_list(c["name"]), ctx):
+                return False
             if c.get("params"):
-                tp = ctx.get("toolParams")
-                if not tp:
+                if not self._has_params(ctx):
                     return False
+                tp = ctx["toolParams"]
                 for key, m in c["params"].items():
-                    v = tp.get(key)
-                    if "equals" in m:
-                        ok = v == m["equals"] and type(v) == type(m["equals"])
-                    elif "contains" in m:
-                        ok = isinstance(v, str) and m["contains"] in v
-                    elif "matches" in m:
+                    if "matches" in m and "equals" not in m and "contains" not in m:
+                        v = tp.get(key)
                         ok = isinstance(v, str) and m["matches"] in self.tool_rule and self.tool_rule[m["matches"]] in hit["param"].get(key, set())
-                    elif "startsWith" in m:
-                        ok = isinstance(v, str) and v.startswith(m["startsWith"])
-                    elif "in" in m:
-                        ok = v in m["in"]
                     else:
-                        ok = False
+                        ok = self._param_test(key, m, ctx)
                     if not ok:
                         return False
             return True
         if t == "agent":
-            if c.get("id") is not None:
-                ids = c["id"] if isinstance(c["id"], list) else [c["id"]]
-                aid = ctx.get("agentId", "")
-                if not any(_glob_match(p, aid) if ("*" in p or "?" in p) else p == aid for p in ids):
-                    return False
-            if c.get("trustTier") is not None:
-                tiers = c["trustTier"] if isinstance(c["trustTier"], list) else [c["trustTier"]]
-                if ((ctx.get("trust") or {}).get("agent") or {}).get("tier", "standard") not in tiers:
-                    return False
+            if c.get("id") is not None and not self._agent_id_in(_as_list(c["id"]), ctx):
+                return False
+            if c.get("trustTier") is not None and not self._agent_tier_in(_as_list(c["trustTier"]), ctx):
+                return False
             return True
         if t == "any":
             return any(self._cond(sub, ctx, hit) for sub in c.get("conditions", []))
