@@ -321,6 +321,19 @@ CG_API int cg_policy_eval_batch(cg_ruleset *rs, const uint8_t *bytes, const uint
 CG_API int cg_policy_eval_batch_device(cg_ruleset *rs, const void *d_bytes, const void *d_offsets, const void *d_roles, uint32_t n_texts,
                                        const void *d_ctx_offsets, const void *d_atoms, uint32_t n_ctx, void *d_out_verdicts,
                                        void *d_out_matches, uint32_t matches_cap, void *d_out_nmatches, void *stream);
+/* One evaluation context, blocking: PolicyEvaluator.evaluate for the hooks that evaluate one context per event
+ * (before_tool_call, message_sending; src/hooks.ts:173-290).  Returns exactly what cg_policy_eval_batch returns for the
+ * context that owns all n_texts texts (ctx_offsets = {0, n_texts}) with atom row `atoms`: *out_verdict = its verdict word,
+ * out_rules[i] = out_matches[i].rule (program rules of the matched policies, in evaluation order), the first rules_cap of them
+ * written and *out_nrules = their number (CG_ERR_CAPACITY past rules_cap); the same argument checks, error codes and cg_stats
+ * (but kernel_launches and last_scan_ms).  out_rules and out_nrules may be NULL; n_texts = 0 is valid (a tool call without
+ * string params gets a verdict from its atoms).  Up to 64 texts, 64 KB of text, 32 768 atoms and 4096 matched policies (when
+ * the caller wants that many), the call costs one H2D copy, one CUDA graph (the step, then one kernel), one D2H copy and one
+ * synchronise (DESIGN.md section 4.8); anything larger, and a step whose internal queues overflowed, takes the batch call's
+ * path.  In order with the rule set's other calls, like cg_scan_one. */
+CG_API int cg_policy_eval_one(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, const uint8_t *roles,
+                              uint32_t n_texts, const uint32_t *atoms, uint32_t *out_verdict,
+                              uint32_t *out_rules, uint32_t rules_cap, uint32_t *out_nrules);
 
 /* ---- SHA-256.  Replaces createHash("sha256").update(s).digest() at src/util.ts:77-79,
  * src/redaction/vault.ts:26-28 (and nats/src/hooks.ts:90-94) for a batch of n byte strings. */

@@ -7,6 +7,7 @@
  *   matchesAny                    src/conditions/context.ts:9-25              -> scanBatch over every pattern of the policy set
  *   ResponseGate mustMatch / mustNotMatch  src/response-gate.ts:104-149       -> scanBatch
  *   tool param `matches`          src/conditions/tool.ts:36-45                -> scanBatch
+ *   PolicyEvaluator.evaluate      src/policy-evaluator.ts:18-146              -> policyEvalOne (GpuPolicyEvaluator)
  *   sha256                        src/util.ts:77-79, src/redaction/vault.ts:26-28 -> sha256Batch
  *   audit JSONL -> Merkle log     src/audit-trail.ts:151-179 (flush)          -> logAppendJsonl / logRoot / logFrontier
  *
@@ -42,6 +43,8 @@ type Addon = {
   setPolicyProgram(handle: unknown, program: Uint32Array, nAtoms: number): void;
   policyEvalBatch(handle: unknown, bytes: Uint8Array, offsets: Uint32Array, roles: Uint8Array, ctxOffsets: Uint32Array, atoms: Uint32Array,
                   nAtoms: number): { verdicts: Uint32Array; matches: Uint32Array };
+  // one context owning every text, blocking, one device round trip: policyEvalBatch's verdict word and program rules for it
+  policyEvalOne(handle: unknown, bytes: Uint8Array, offsets: Uint32Array, roles: Uint8Array, atoms: Uint32Array, nAtoms: number): { verdict: number; rules: Uint32Array };
   sha256Batch(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array;
   merkleRoot(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array;
   logCreate(keepLeafDigests: boolean): unknown;
@@ -219,6 +222,67 @@ export function compilePolicyProgram(policies: any[], patternRule: Map<string, n
     }
   }
   return { program: Uint32Array.from(words), atoms, paramRole, rules };
+}
+
+/** Drop-in for PolicyEvaluator.evaluate (src/policy-evaluator.ts:18-146) on the hooks that evaluate one context per event
+ * (before_tool_call, message_sending): the policies compiled once into a program on one rule set of their regex tests, then
+ * per context its texts and atom row in one blocking call, one device round trip.  evalCondition: the reference's own
+ * condition code for one condition (the atoms), as for compilePolicyProgram. */
+export class GpuPolicyEvaluator {
+  private readonly handle: unknown;
+  private readonly compiled: ReturnType<typeof compilePolicyProgram>;
+
+  constructor(policies: any[], evalCondition: (c: Cond, ctx: Ctx) => boolean) {
+    const enabled = policies.filter((p) => p.enabled !== false);
+    // one rule per messageContains / conversationContains pattern (an invalid one as an escaped literal, the includes()
+    // fallback of context.ts:15-17), then one per valid tool `matches` pattern (an invalid one never matches, tool.ts:39-44)
+    const patternRule = new Map<string, number>(), toolRule = new Map<string, number>(), toolPats = new Set<string>();
+    const sources: { source: string }[] = [];
+    const walk = (c: Cond): void => {
+      if (c.type === "context") {
+        for (const key of ["messageContains", "conversationContains"])
+          for (const p of c[key] == null ? [] : Array.isArray(c[key]) ? c[key] : [c[key]])
+            if (!patternRule.has(p)) {
+              patternRule.set(p, sources.length);
+              sources.push({ source: addon.ruleCheck(p) === -4 /* CG_ERR_SYNTAX */ ? p.replace(/[.*+?^${}()|[\]\\\/-]/g, "\\$&") : p });
+            }
+      } else if (c.type === "tool") {
+        for (const m of Object.values<any>(c.params ?? {})) if ("matches" in m) toolPats.add(m.matches);
+      } else if (c.type === "any") (c.conditions ?? []).forEach(walk);
+      else if (c.type === "not") walk(c.condition);
+    };
+    for (const p of enabled) for (const r of p.rules ?? []) (r.conditions ?? []).forEach(walk);
+    for (const p of [...toolPats].sort())
+      if (addon.ruleCheck(p) === 0) { toolRule.set(p, sources.length); sources.push({ source: p }); }
+    this.handle = addon.createRuleset(sources).handle;
+    this.compiled = compilePolicyProgram(enabled, patternRule, toolRule, evalCondition);
+    addon.setPolicyProgram(this.handle, this.compiled.program, this.compiled.atoms.length);
+  }
+
+  evaluate(ctx: Ctx): { action: string; reason: string; matches: { policyId: string; ruleId: string; effect: any; controls: string[] }[] } {
+    const { atoms, paramRole, rules } = this.compiled;
+    // the texts a leaf can read: a non-empty message (role 0), every conversation entry (1), string params a `matches` test names
+    const texts: string[] = [], roleOf: number[] = [];
+    if (ctx.messageContent) { texts.push(ctx.messageContent); roleOf.push(0); }
+    for (const t of ctx.conversationContext ?? []) { texts.push(t); roleOf.push(1); }
+    for (const [key, val] of Object.entries<any>(ctx.toolParams ?? {}))
+      if (typeof val === "string" && paramRole.has(key)) { texts.push(val); roleOf.push(paramRole.get(key)!); }
+    const row = new Uint32Array((atoms.length + 31) >>> 5);
+    atoms.forEach((fn, a) => { if (fn(ctx)) row[a >>> 5] |= 1 << (a & 31); });
+    const { bytes, offsets } = pack(texts);
+    const { verdict, rules: hit } = addon.policyEvalOne(this.handle, bytes, offsets, Uint8Array.from(roleOf), row, atoms.length);
+    // decode as plugin.PolicyEvaluator.decode_verdicts: outcome, deciding rule, the reference's reason strings
+    const matches = Array.from(hit, (j) => {
+      const [p, r] = rules[j];
+      return { policyId: p.id, ruleId: r.id, effect: r.effect ?? { action: "allow" }, controls: p.controls ?? [] };
+    });
+    const outcome = verdict & 7, decide = verdict >>> 12;
+    if (outcome >= 3) {
+      const reason = decide !== 0xfffff ? rules[decide][1].effect.reason : outcome === 4 ? "Denied by governance policy" : "Requires 2FA approval";
+      return { action: outcome === 4 ? "deny" : "2fa", reason, matches };
+    }
+    return { action: "allow", reason: ["No matching policies", "Allowed by governance policy", "Allowed with audit logging"][outcome], matches };
+  }
 }
 
 /** sha256 (src/util.ts:77-79) for a batch of strings, hex digests. */

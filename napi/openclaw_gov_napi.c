@@ -28,6 +28,8 @@
  *   setPolicyProgram(handle, program: Uint32Array, nAtoms: number): void  // whole policies (openclaw_gov.h: program layout)
  *   policyEvalBatch(handle, bytes, offsets, roles: Uint8Array, ctxOffsets: Uint32Array, atoms: Uint32Array, nAtoms: number):
  *     {verdicts: Uint32Array, matches: Uint32Array}  // one verdict per context; matches: ctx, program rule pairs
+ *   policyEvalOne(handle, bytes, offsets, roles: Uint8Array, atoms: Uint32Array, nAtoms: number): {verdict: number, rules: Uint32Array}
+ *     // one context owning every text, blocking, one device round trip: policyEvalBatch's verdict and program rules
  *   sha256Batch(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array  // 32 bytes per item
  *   merkleRoot(bytes: Uint8Array, offsets: BigUint64Array): Uint8Array   // 32 bytes
  *   logCreate(keepLeafDigests: boolean): External ; logRestore(size: bigint, frontier: Uint8Array): External
@@ -575,6 +577,37 @@ static napi_value js_redact_one(napi_env env, napi_callback_info info) {
   return res;
 }
 
+/* one context owning every text (cg_policy_eval_one): the texts, their roles and ceil(nAtoms / 32) atom words, nAtoms as given to
+ * setPolicyProgram -> {verdict, rules} */
+static napi_value js_policy_eval_one(napi_env env, napi_callback_info info) {
+  ARGS(env, info, 6)
+  cg_ruleset *rs; uint8_t *bytes, *offp, *roles, *atoms; size_t nb, nr, na; uint32_t n_atoms = 0;
+  NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
+  const int64_t nn = get_batch(env, argv[1], argv[2], 0, &bytes, &offp); if (nn < 0) return NULL;
+  if (!get_ta(env, argv[1], &bytes, &nb, napi_uint8_array) || !get_ta(env, argv[3], &roles, &nr, napi_uint8_array) || (int64_t)nr != nn ||
+      !get_ta(env, argv[4], &atoms, &na, napi_uint32_array) || napi_get_value_uint32(env, argv[5], &n_atoms) != napi_ok) {
+    napi_throw_type_error(env, NULL, "policyEvalOne(handle, bytes, offsets, roles: Uint8Array (one per text), atoms: Uint32Array, nAtoms)"); return NULL;
+  }
+  if (na != (size_t)((n_atoms + 31) / 32) * 4) { napi_throw_type_error(env, NULL, "atoms: ceil(nAtoms / 32) words"); return NULL; }
+  if (!nb) bytes = one_empty;                       /* an empty typed array may report NULL: the C ABI rejects a NULL text buffer */
+  uint32_t verdict = 0, nm = 0, cap = 64; uint32_t *tmp = (uint32_t *)malloc(sizeof(uint32_t) * cap);
+#define EVAL(cap) cg_policy_eval_one(rs, bytes, (const uint32_t *)offp, nr ? roles : NULL, (uint32_t)nn, na ? (const uint32_t *)atoms : NULL, &verdict, \
+                                     tmp, (cap), &nm)
+  int rc = tmp ? EVAL(cap) : CG_ERR_NOMEM;
+  if (rc == CG_ERR_CAPACITY && nm > cap) { cap = nm; uint32_t *t2 = (uint32_t *)realloc(tmp, sizeof(uint32_t) * cap); if (t2) { tmp = t2; rc = EVAL(cap); } }
+#undef EVAL
+  if (rc != CG_OK) { free(tmp); napi_throw_error(env, NULL, rc == CG_ERR_NOMEM ? "out of host memory" : cg_last_error()); return NULL; }
+  napi_value ab, rules, v, out; void *data;
+  if (napi_create_arraybuffer(env, (size_t)nm * 4, &data, &ab) != napi_ok) { free(tmp); napi_throw_error(env, NULL, "N-API call failed"); return NULL; }
+  memcpy(data, tmp, (size_t)nm * 4); free(tmp);
+  NAPI_CALL(env, napi_create_typedarray(env, napi_uint32_array, nm, ab, 0, &rules));
+  NAPI_CALL(env, napi_create_double(env, (double)verdict, &v));   /* (a uint32 is exact as a JS number) */
+  NAPI_CALL(env, napi_create_object(env, &out));
+  NAPI_CALL(env, napi_set_named_property(env, out, "verdict", v));
+  NAPI_CALL(env, napi_set_named_property(env, out, "rules", rules));
+  return out;
+}
+
 static napi_value module_init(napi_env env, napi_value exports) {
   napi_property_descriptor d[] = {
 #define FN(name, fn) {name, NULL, fn, NULL, NULL, NULL, napi_default, NULL}
@@ -585,7 +618,7 @@ static napi_value module_init(napi_env env, napi_value exports) {
     FN("setPolicy", js_set_policy), FN("verdictBatch", js_verdict_batch),
     FN("setViews", js_set_views), FN("scanBatchViews", js_scan_batch_views), FN("findMatchesBatchViews", js_find_matches_batch_views),
     FN("redactBatchViews", js_redact_batch_views), FN("verdictBatchViews", js_verdict_batch_views),
-    FN("setPolicyProgram", js_set_policy_program), FN("policyEvalBatch", js_policy_eval_batch),
+    FN("setPolicyProgram", js_set_policy_program), FN("policyEvalBatch", js_policy_eval_batch), FN("policyEvalOne", js_policy_eval_one),
     FN("sha256Batch", js_sha256_batch), FN("merkleRoot", js_merkle_root),
     FN("logCreate", js_log_create), FN("logRestore", js_log_restore), FN("logAppend", js_log_append), FN("logAppendJsonl", js_log_append_jsonl),
     FN("logReserve", js_log_reserve), FN("logSize", js_log_size), FN("logRoot", js_log_root), FN("logFrontier", js_log_frontier),

@@ -65,7 +65,7 @@ EXPORTS = ["cg_init", "cg_shutdown", "cg_last_error", "cg_version", "cg_device_c
            "cg_redact_batch_device_views", "cg_policy_verdict_batch_device_views",
            "cg_merkle_log_append_device", "cg_merkle_log_append_fixed_device", "cg_merkle_log_root_device", "cg_merkle_log_proofs_device",
            "cg_merkle_log_consistency_between_device", "cg_merkle_verify_proofs_device", "cg_merkle_log_join",
-           "cg_ruleset_set_policy_program", "cg_policy_eval_batch", "cg_policy_eval_batch_device"]
+           "cg_ruleset_set_policy_program", "cg_policy_eval_batch", "cg_policy_eval_batch_device", "cg_policy_eval_one"]
 
 _lib = None
 
@@ -162,6 +162,7 @@ def load():
     L.cg_ruleset_set_policy_program.argtypes = [vp, vp, u32, u32]; L.cg_ruleset_set_policy_program.restype = i32
     L.cg_policy_eval_batch.argtypes = [vp, vp, vp, vp, u32, vp, vp, u32, vp, vp, u32, C.POINTER(u32)]; L.cg_policy_eval_batch.restype = i32
     L.cg_policy_eval_batch_device.argtypes = [vp, vp, vp, vp, u32, vp, vp, u32, vp, vp, u32, vp, vp]; L.cg_policy_eval_batch_device.restype = i32
+    L.cg_policy_eval_one.argtypes = [vp, vp, vp, vp, u32, vp, C.POINTER(u32), vp, u32, C.POINTER(u32)]; L.cg_policy_eval_one.restype = i32
     _lib = L
     return L
 
@@ -400,6 +401,30 @@ class Ruleset:
                 continue
             check(rc)
             return verdicts[:n_ctx], matches[:nm.value] if want_matches else matches[:0]
+
+    def eval_one(self, data: np.ndarray, off: np.ndarray, roles, atoms):
+        """cg_policy_eval_one: one context owning every text (data, off), one role per text, its atom row atoms[ceil(n_atoms /
+        32)] (uint32); blocking, one device round trip.  -> (verdict word, [program rules of the matched policies in evaluation
+        order]), what eval_batch returns for a batch of that one context."""
+        n = len(off) - 1
+        roles = np.ascontiguousarray(roles, dtype=np.uint8).reshape(-1)
+        atoms = np.ascontiguousarray(atoms, dtype=np.uint32).reshape(-1)
+        if len(roles) != n:
+            raise ValueError("roles: %d for %d texts" % (len(roles), n))
+        aw = (getattr(self, "n_atoms", 0) + 31) // 32
+        if atoms.size != aw:
+            raise ValueError("atoms: %d words for a row of %d" % (atoms.size, aw))
+        verdict, nr = C.c_uint32(0), C.c_uint32(0)
+        cap = 64
+        while True:
+            rules = np.zeros(cap, dtype=np.uint32)
+            rc = load().cg_policy_eval_one(self.handle, data.ctypes.data, off.ctypes.data, roles.ctypes.data if n else None, n,
+                                           atoms.ctypes.data if atoms.size else None, C.byref(verdict), rules.ctypes.data, cap, C.byref(nr))
+            if rc == CG_ERR_CAPACITY and nr.value > cap:
+                cap = nr.value
+                continue
+            check(rc)
+            return verdict.value, [int(x) for x in rules[:nr.value]]
 
     def eval_batch_device(self, d_bytes: int, d_off: int, d_roles: int, n_texts: int, d_ctx_off: int, d_atoms: int, n_ctx: int,
                           d_verdicts: int, d_matches: int = 0, matches_cap: int = 0, d_nmatches: int = 0, stream: int = 0):

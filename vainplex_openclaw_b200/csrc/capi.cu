@@ -160,12 +160,23 @@ struct cg_ruleset {
   uint64_t graph_clock = 0;
   // cg_ruleset_set_views: n_views rows of dev.rw words in HBM (bit r of row v = rule r is in view v); none before the first call
   uint32_t* view_rows = nullptr; uint32_t n_views = 0;
-  // cg_ruleset_set_policy_program: the program's words and one rule record per program rule (kernels.h PolicyTable) in HBM
+  // cg_ruleset_set_policy_program: the program's words and one rule record per program rule (kernels.h PolicyTable) in HBM;
+  // prog_gen advances with every program set (a captured graph holds the tables by value)
   uint32_t* prog_ops = nullptr; uint4* prog_rules = nullptr; uint32_t prog_n_rules = 0, prog_n_atoms = 0;
+  uint64_t prog_gen = 0;
+  // cg_policy_eval_one: pinned staging + one device block (capi.cu kPe*: [offsets][roles][atom row][text bytes] in,
+  // [verdict][count][counters][rules] out), and the step + policy_eval_one_kernel as graphs over those fixed addresses, one per
+  // text count (the step takes it by value), the least recently used of kPeGraphs replaced
+  static constexpr int kPeGraphs = 8;
+  struct PeGraph { cudaGraphExec_t exec = nullptr; uint32_t n = 0; uint64_t gen = 0, prog = 0, used = 0; int ctas = 0, kernels = 0; };
+  struct PolicyOne { PeGraph g[kPeGraphs]; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint64_t clock = 0; } pone;
   ~cg_ruleset() {
     cudaFree(view_rows); cudaFree(prog_ops); cudaFree(prog_rules);
     for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     for (auto& g : one.g) if (g.exec) cudaGraphExecDestroy(g.exec);
+    for (auto& g : pone.g) if (g.exec) cudaGraphExecDestroy(g.exec);
+    if (pone.h_pin) cudaFreeHost(pone.h_pin);
+    cudaFree(pone.d_buf);
     if (one.h_pin) cudaFreeHost(one.h_pin);
     if (one.h_pack) cudaFreeHost(one.h_pack);
     cudaFree(one.d_buf); cudaFree(one.d_pack);
@@ -1378,6 +1389,7 @@ int cg_ruleset_set_policy_program(cg_ruleset* rs, const uint32_t* program, uint3
   if (at != words) return bad("words past the last policy");
   CU(cudaStreamSynchronize(G.stream));
   cudaFree(rs->prog_ops); cudaFree(rs->prog_rules); rs->prog_ops = nullptr; rs->prog_rules = nullptr; rs->prog_n_rules = rs->prog_n_atoms = 0;
+  rs->prog_gen++;                                           // (cg_policy_eval_one's graphs hold the old tables)
   CU(cudaMalloc((void**)&rs->prog_ops, (size_t)words * 4));
   CU(cudaMalloc((void**)&rs->prog_rules, std::max<size_t>(rules.size(), 1) * sizeof(uint4)));
   CU(cudaMemcpy(rs->prog_ops, program, (size_t)words * 4, cudaMemcpyHostToDevice));
@@ -1472,6 +1484,104 @@ int cg_policy_eval_batch_device(cg_ruleset* rs, const void* d_bytes, const void*
   std::lock_guard<std::mutex> lk(g_mu);
   return policy_eval_device(rs, d_bytes, d_offsets, d_roles, n_texts, d_ctx_offsets, d_atoms, n_ctx, d_out_verdicts, d_out_matches, matches_cap,
                             d_out_nmatches, stream);
+}
+
+namespace {
+// cg_policy_eval_one's staging block, host (pinned) and device: in, [offsets, kPeOneTexts + 1][roles][atom row, kPeOneAtomWords]
+// [text bytes, kPeOneBytes][64 zero bytes] at fixed places (offsets are rebased to kPeTextAt); out, kPeOneRules + kPeOneRulesCap
+// words (kernels.h).  The limits: 64 texts (kPeOneTexts: the kernel keeps the text list in shared memory), 64 KB of text (a tool
+// call's params or a message with its conversation history), 32 768 atoms, 4096 matched policies.
+constexpr uint32_t kPeOneBytes = 65536, kPeOneAtomWords = 1024, kPeOneRulesCap = 4096;
+constexpr uint32_t kPeRolesAt = 512, kPeAtomsAt = kPeRolesAt + 256, kPeTextAt = kPeAtomsAt + 4 * kPeOneAtomWords;
+constexpr uint32_t kPeIn = kPeTextAt + kPeOneBytes + 64, kPeOut = 4 * (kPeOneRules + kPeOneRulesCap);
+static_assert(4 * (kPeOneTexts + 1) <= kPeRolesAt && kPeOneTexts <= 256 && kPeTextAt % 256 == 0, "cg_policy_eval_one staging layout");
+
+// cg_policy_eval_one on the staging block: one H2D copy, one graph (the policy-mode step over the staged texts, then
+// policy_eval_one_kernel), one D2H copy of the header and as many rules as the caller can take, one synchronise.  Outputs,
+// statuses and statistics are those of cg_policy_eval_batch with one context.  -> CG_OK, an error, or 1 = take the batch call
+// (an argument the batch call rejects or judges, no device, profiling, more texts, bytes or atoms than the staging block
+// holds, more matches than it holds and the caller wants, a queue overflowed)
+int policy_one_fast(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, const uint8_t* roles, uint32_t n_texts, const uint32_t* atoms,
+                    uint32_t* out_verdict, uint32_t* out_rules, uint32_t rules_cap, uint32_t* out_nrules) {
+  if (!G.ready || !rs || !rs->prog_ops || !out_verdict || G.profiling || n_texts > kPeOneTexts) return 1;
+  if (n_texts && (!bytes || !offsets || !roles)) return 1;
+  const PolicyTable pt = policy_table(rs);
+  if (pt.aw > kPeOneAtomWords || (pt.aw && !atoms)) return 1;
+  for (uint32_t i = 0; i < n_texts; i++) if (offsets[i + 1] < offsets[i]) return 1;
+  const uint32_t first = n_texts ? offsets[0] : 0, len = n_texts ? offsets[n_texts] - first : 0;
+  if (len > kPeOneBytes) return 1;
+  cg_ruleset::PolicyOne& o = rs->pone;
+  cudaStream_t st = G.stream;
+  InOrder turn(&rs->order, st);
+  int rc;
+  if ((rc = turn.rc)) return rc;
+  if (!o.h_pin) { CU(cudaMallocHost((void**)&o.h_pin, kPeIn + kPeOut)); memset(o.h_pin, 0, kPeIn + kPeOut); }
+  if (!o.d_buf) { CU(cudaMalloc((void**)&o.d_buf, kPeIn + kPeOut)); CU(cudaMemset(o.d_buf, 0, kPeIn + kPeOut)); }
+  if ((rc = prepare_step(rs, n_texts, kStepPolicy, st, 1))) return rc;
+  const ScanWork& w = rs->work;
+  uint32_t* d_out = reinterpret_cast<uint32_t*>(o.d_buf + kPeIn);
+  // the graph of this text count, captured again when the scratch, the verify grid or the program changed since
+  cg_ruleset::PeGraph* g = nullptr;
+  for (auto& e : o.g) if (e.exec && e.n == n_texts && e.gen == rs->scratch_gen && e.ctas == rs->verify_ctas && e.prog == rs->prog_gen) g = &e;
+  if (!g) {
+    g = &o.g[0];
+    for (auto& e : o.g) if (e.used < g->used) g = &e;
+    if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; }
+    const PolicyBatch b{o.d_buf + kPeRolesAt, n_texts, nullptr, reinterpret_cast<const uint32_t*>(o.d_buf + kPeAtomsAt), 1};
+    if ((rc = capture(st, [&] {
+          const int r = run_scan_device(rs, o.d_buf, reinterpret_cast<const uint32_t*>(o.d_buf), n_texts, w.words, kStepPolicy, st);
+          if (r != CG_OK) return r;
+          count_launches(launch_policy_eval_one(pt, w, rs->dev.rw, b, d_out, kPeOneRulesCap, st));
+          CU(cudaGetLastError());
+          return CG_OK;
+        }, &g->exec, &g->kernels))) return rc;
+    g->n = n_texts; g->gen = rs->scratch_gen; g->ctas = rs->verify_ctas; g->prog = rs->prog_gen;
+  }
+  g->used = ++o.clock;
+  uint32_t* hoff = reinterpret_cast<uint32_t*>(o.h_pin);
+  for (uint32_t i = 0; i <= n_texts; i++) hoff[i] = kPeTextAt + (n_texts ? offsets[i] - first : 0);
+  if (n_texts) memcpy(o.h_pin + kPeRolesAt, roles, n_texts);
+  if (pt.aw) memcpy(o.h_pin + kPeAtomsAt, atoms, (size_t)pt.aw * 4);
+  if (len) memcpy(o.h_pin + kPeTextAt, bytes + first, len);
+  memset(o.h_pin + kPeTextAt + len, 0, 64);
+  CU(cudaMemcpyAsync(o.d_buf, o.h_pin, (size_t)kPeTextAt + len + 64, cudaMemcpyHostToDevice, st));
+  CU(cudaGraphLaunch(g->exec, st));
+  // matches <= policies <= program rules: no more of them than the caller takes can be needed
+  const uint32_t want = std::min(std::min(out_rules ? rules_cap : 0u, kPeOneRulesCap), pt.n_rules);
+  uint32_t* ho = reinterpret_cast<uint32_t*>(o.h_pin + kPeIn);
+  CU(cudaMemcpyAsync(ho, d_out, 4 * ((size_t)kPeOneRules + want), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  count_launches(g->kernels);
+  const uint32_t* hc = ho + kPeOneCounters;
+  if ((rc = absorb_counters(rs, hc))) return rc;                 // 1: a queue overflowed, the batch call retries with larger scratch
+  const uint32_t nm = ho[1];
+  if (out_rules && nm > kPeOneRulesCap && rules_cap > kPeOneRulesCap) return 1;
+  count_step(n_texts, len, hc);
+  *out_verdict = ho[0];
+  if (out_nrules) *out_nrules = nm;
+  if (out_rules) memcpy(out_rules, ho + kPeOneRules, (size_t)std::min(nm, rules_cap) * 4);
+  if (out_rules && nm > rules_cap) return fail(CG_ERR_CAPACITY, "out_rules too small (see *out_nrules)");
+  return CG_OK;
+}
+}  // namespace
+
+int cg_policy_eval_one(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, const uint8_t* roles, uint32_t n_texts, const uint32_t* atoms,
+                       uint32_t* out_verdict, uint32_t* out_rules, uint32_t rules_cap, uint32_t* out_nrules) {
+  std::lock_guard<std::mutex> lk(g_mu);
+  const int frc = policy_one_fast(rs, bytes, offsets, roles, n_texts, atoms, out_verdict, out_rules, rules_cap, out_nrules);
+  if (frc != 1) return frc;
+  // the batch call with one context; the match list staged here (matches <= program rules), its rules copied out as the batch
+  // call writes its matches: the first rules_cap on CG_ERR_CAPACITY, none when it fails earlier (nm then stays unwritten)
+  const uint32_t ctx[2] = {0, n_texts};
+  const uint32_t cap = std::min(rules_cap, rs && G.ready ? rs->prog_n_rules : 0u);
+  std::vector<cg_policy_match> m(out_rules ? std::max<uint32_t>(cap, 1u) : 0u);
+  uint32_t nm = 0xffffffffu;
+  const int rc = policy_eval_host(rs, bytes, offsets, roles, n_texts, ctx, atoms, 1, out_verdict, out_rules ? m.data() : nullptr, out_rules ? cap : 0u,
+                                  out_rules || out_nrules ? &nm : nullptr);
+  if (nm == 0xffffffffu) return rc;
+  if (out_nrules) *out_nrules = nm;
+  if (out_rules) for (uint32_t i = 0; i < nm && i < cap; i++) out_rules[i] = m[i].rule;
+  return rc;
 }
 
 // ---------------------------------------------------------------------------------- SHA / Merkle

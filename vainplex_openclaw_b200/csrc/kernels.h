@@ -168,6 +168,14 @@ int launch_policy_eval(const PolicyTable& pt, const ScanWork& w, uint32_t rw, co
 // n_ctx and the SM count only.
 int launch_policy_emit(const PolicyTable& pt, const ScanWork& w, uint32_t rw, const PolicyBatch& b, uint32_t* d_out, uint32_t cap, uint32_t* d_count,
                        int sm_count, cudaStream_t stream);
+// single-context policy path (cg_policy_eval_one): behind a finished policy-mode step over the context's b.n_texts texts (its
+// atom row at b.atoms; b.ctx_off unused), one block packs the result into d_out as u32 words:
+//   [0] verdict word  [1] matched policies  [kPeOneCounters..] counter block  [kPeOneRules..] the program rules of the first
+//   cap matches, in evaluation order
+// (an incomplete step: verdict and count 0xffffffff).  One launch whatever the program, the texts or the hits.
+constexpr uint32_t kPeOneCounters = 2, kPeOneRules = kPeOneCounters + kCounterWords;
+constexpr uint32_t kPeOneTexts = 64;              // texts a context on this path has at most (the kernel keeps them in shared memory)
+int launch_policy_eval_one(const PolicyTable& pt, const ScanWork& w, uint32_t rw, const PolicyBatch& b, uint32_t* d_out, uint32_t cap, cudaStream_t stream);
 // start of a step: counters = 0, slot_of_msg = none, candidate / hit rows of the slots the previous step used = 0
 int launch_reset(const DevRuleset& rs, const ScanWork& w, uint32_t n, int sm_count, cudaStream_t stream);
 

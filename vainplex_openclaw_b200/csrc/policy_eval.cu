@@ -4,56 +4,13 @@
 // change with it.
 #include <algorithm>
 
-#include "kernels.h"
+#include "policy_eval.h"
 
 namespace cg {
 
 namespace {
 
 constexpr uint32_t kPeWarps = 8;         // warps (contexts in flight) per block
-constexpr uint32_t kPeTexts = 64;        // slotted texts of a context kept in shared memory; past that HIT leaves walk the range
-constexpr uint32_t kNoRule = 0xfffffu;
-
-// the texts of one context that have a hit row: (slot, role), collected once per context by its warp
-struct CtxTexts {
-  const uint32_t* slot; const uint8_t* role; uint32_t n;    // n > kPeTexts: read the range itself
-  uint32_t t0, t1;
-};
-
-__device__ __forceinline__ bool row_bit(const ScanWork& w, uint32_t rw, uint32_t slot, uint32_t r) {
-  return (w.hit[(size_t)slot * rw + (r >> 5)] >> (r & 31)) & 1u;
-}
-
-// HIT(r, q): rule r hit a text of the context whose role is q
-__device__ __forceinline__ bool hit_leaf(const ScanWork& w, uint32_t rw, const PolicyBatch& b, const CtxTexts& ct, uint32_t r, uint32_t q) {
-  if (ct.n <= kPeTexts) {
-    for (uint32_t k = 0; k < ct.n; k++) if (ct.role[k] == q && row_bit(w, rw, ct.slot[k], r)) return true;
-    return false;
-  }
-  for (uint32_t i = ct.t0; i < ct.t1; i++) {
-    const uint32_t s = w.slot_of_msg[i];
-    if (s < w.slot_cap && b.roles[i] == q && row_bit(w, rw, s, r)) return true;
-  }
-  return false;
-}
-
-// one rule's postfix program on a bit stack (depth <= 32, checked when the program was set)
-__device__ __forceinline__ bool run_rule(const PolicyTable& pt, const ScanWork& w, uint32_t rw, const PolicyBatch& b, const CtxTexts& ct, const uint32_t* arow,
-                         uint32_t at, uint32_t n_ops) {
-  uint32_t st = 0;
-  for (uint32_t k = 0; k < n_ops; k++) {
-    const uint32_t o = pt.ops[at + k];
-    switch (o & 7u) {
-      case kPolOpConst: st = st << 1 | (o >> 3); break;
-      case kPolOpAtom: { const uint32_t a = o >> 3; st = st << 1 | ((arow[a >> 5] >> (a & 31)) & 1u); break; }
-      case kPolOpHit: st = st << 1 | (hit_leaf(w, rw, b, ct, (o >> 3) & 0x1fffffu, o >> 24) ? 1u : 0u); break;
-      case kPolOpAnd: { const uint32_t t = st & 1u; st >>= 1; st &= ~1u | t; break; }
-      case kPolOpOr: { const uint32_t t = st & 1u; st >>= 1; st |= t; break; }
-      default: st ^= 1u; break;                                   // kPolOpNot
-    }
-  }
-  return st & 1u;
-}
 
 // One warp per context, lanes over the program's rules, 32 at a time in program order (policy order, then rule order).
 // A lane's rule holds when its policy's scope atom (if any) and its program hold; it is its policy's match when no earlier
@@ -97,21 +54,11 @@ __global__ void __launch_bounds__(kPeWarps * 32, 4) policy_eval_kernel(PolicyTab
       continue;
     }
     // the context's texts with a hit row, as (slot, role)
-    uint32_t nt = 0;
-    for (uint32_t i0 = t0; i0 < t1; i0 += 32) {
-      const uint32_t i = i0 + lane;
-      const uint32_t s = i < t1 ? w.slot_of_msg[i] : 0xffffffffu;
-      const bool has = s < w.slot_cap;
-      const uint32_t m = __ballot_sync(0xffffffffu, has);
-      const uint32_t at = nt + __popc(m & below);
-      if (has && at < kPeTexts) { s_slot[wid][at] = s; s_role[wid][at] = b.roles[i]; }
-      nt += __popc(m);
-    }
+    const uint32_t nt = collect_texts(w, b, t0, t1, lane, s_slot[wid], s_role[wid]);
     __syncwarp();
     const CtxTexts ct{s_slot[wid], s_role[wid], nt, t0, t1};
     const uint32_t* arow = b.atoms + (size_t)c * pt.aw;
-    uint32_t carry_first = 0xffffffffu, matched = 0, deny_r = kNoRule, twofa_r = kNoRule;
-    bool carry_hit = false, any_deny = false, any_2fa = false, any_audit = false;
+    PolicyWalk pw;
     uint64_t pos = kMode == 2 ? w.out_off[c] : 0ull;
     for (uint32_t base = 0; base < pt.n_rules; base += 32) {
       const uint32_t j = base + lane;
@@ -119,27 +66,12 @@ __global__ void __launch_bounds__(kPeWarps * 32, 4) policy_eval_kernel(PolicyTab
       bool t = false;
       if (j < pt.n_rules) {
         ri = pt.rules[j];
-        t = ri.w == 0xffffffffu || ((arow[ri.w >> 5] >> (ri.w & 31)) & 1u);
-        if (t) t = run_rule(pt, w, rw, b, ct, arow, ri.x, ri.y & 0xffffffu);
+        t = rule_holds(pt, w, rw, b, ct, arow, ri);
       }
-      const uint32_t tb = __ballot_sync(0xffffffffu, t);
-      const uint32_t from = ri.z > base && ri.z != 0xffffffffu ? ri.z - base : 0u;    // the first lane of this lane's policy
-      const bool first = t && !(tb & below & ~((1u << from) - 1u)) && !(carry_hit && ri.z == carry_first);
-      // the policy of the chunk's last rule: did it match in this chunk or before?
-      const uint32_t last = min(31u, pt.n_rules - 1u - base);
-      const uint32_t z_last = __shfl_sync(0xffffffffu, ri.z, last);
-      const uint32_t from_last = z_last > base ? z_last - base : 0u;
-      const bool hit_last = (tb & ~((1u << from_last) - 1u)) != 0u || (carry_hit && z_last == carry_first);
-      carry_first = z_last; carry_hit = hit_last;
+      const bool first = pw.first(t, ri.z, base, pt.n_rules, lane);
       const uint32_t f = __ballot_sync(0xffffffffu, first);
       if (kMode != 2) {
-        const uint32_t act = (ri.y >> 24) & 3u, reason = (ri.y >> 26) & 1u;
-        const uint32_t fd = __ballot_sync(0xffffffffu, first && act == 3u), fdr = __ballot_sync(0xffffffffu, first && act == 3u && reason);
-        const uint32_t f2 = __ballot_sync(0xffffffffu, first && act == 2u), f2r = __ballot_sync(0xffffffffu, first && act == 2u && reason);
-        matched += __popc(f);
-        any_deny |= fd != 0u; any_2fa |= f2 != 0u; any_audit |= __ballot_sync(0xffffffffu, first && act == 1u) != 0u;
-        if (deny_r == kNoRule && fdr) deny_r = base + __ffs(fdr) - 1;
-        if (twofa_r == kNoRule && f2r) twofa_r = base + __ffs(f2r) - 1;
+        pw.add(first, ri.y, base, f);
       } else {
         const uint64_t p = pos + __popc(f & below);
         if (first && p < cap) { out[2 * p] = c; out[2 * p + 1] = j; }
@@ -148,10 +80,8 @@ __global__ void __launch_bounds__(kPeWarps * 32, 4) policy_eval_kernel(PolicyTab
       }
     }
     if (kMode != 2 && lane == 0) {
-      const uint32_t outcome = any_deny ? 4u : any_2fa ? 3u : any_audit ? 2u : matched ? 1u : 0u;
-      const uint32_t decide = any_deny ? deny_r : any_2fa ? twofa_r : kNoRule;
-      verdicts[c] = outcome | (min(matched, 511u) << 3) | (decide << 12);
-      if (kMode == 1) w.out_len[c] = matched;
+      verdicts[c] = pw.verdict();
+      if (kMode == 1) w.out_len[c] = pw.matched;
     }
     __syncwarp();                                                // (the next context overwrites this warp's texts)
   }

@@ -824,16 +824,31 @@ class PolicyEvaluator:
         each context and condition, not only where the host walk would reach it)."""
         if not contexts:
             return []
+        rs = self._program_ruleset()
+        texts, roles, ctx_off, atoms = self.program_inputs(contexts)
+        data, off = N.pack([N.js_utf8(t) for t in texts])
+        words, matches = rs.eval_batch(data, off, roles, ctx_off, atoms)
+        return self.decode_verdicts(words, matches)
+
+    def verdict_one(self, ctx: dict) -> dict:
+        """verdict_batch([ctx])[0] in one blocking device round trip (cg_policy_eval_one): the hooks that evaluate one context
+        per event (before_tool_call, message_sending)."""
+        rs = self._program_ruleset()
+        texts, roles, _ctx_off, atoms = self.program_inputs([ctx])
+        data, off = N.pack([N.js_utf8(t) for t in texts])
+        word, rules = rs.eval_one(data, off, roles, atoms[0])
+        matches = np.array([(0, r) for r in rules], dtype=N.POLICY_MATCH_DTYPE)
+        return self.decode_verdicts(np.array([word], dtype=np.uint32), matches)[0]
+
+    def _program_ruleset(self) -> N.Ruleset:
+        """the rule set the program is evaluated on (the scanner's, or an empty one), the program set on it once"""
         if self._program_rs is None:
             rs = getattr(self.scanner, "ruleset", None) if self.scanner is not None else N.Ruleset([], strict=True)
             if rs is None:
                 raise TypeError("verdict_batch needs the device RuleScanner")
             rs.set_policy_program(self.program, len(self.atoms))
             self._program_rs = rs
-        texts, roles, ctx_off, atoms = self.program_inputs(contexts)
-        data, off = N.pack([N.js_utf8(t) for t in texts])
-        words, matches = self._program_rs.eval_batch(data, off, roles, ctx_off, atoms)
-        return self.decode_verdicts(words, matches)
+        return self._program_rs
 
     # -- one batch for all contexts
     def evaluate_batch(self, contexts: Sequence[dict]) -> List[dict]:
