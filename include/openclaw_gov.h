@@ -169,6 +169,19 @@ CG_API int cg_redact_batch(cg_ruleset *rs, const uint8_t *bytes, const uint32_t 
  * Same single-message path as cg_find_matches_one. */
 CG_API int cg_redact_one(cg_ruleset *rs, const uint8_t *bytes, uint32_t len, uint8_t *out_bytes, uint64_t out_cap,
                          uint64_t *out_need, cg_span *out_spans, uint32_t spans_cap, uint32_t *out_nspans, uint8_t *out_digests32);
+/* findMatches / scanString for the few strings of one scanned value, blocking: RedactionEngine.scan / scanValue /
+ * scanStringValue (src/redaction/engine.ts:53-147) redact every string leaf of a tool result, a tool call's params or a
+ * message's metadata (the hooks tool_result_persist, after_tool_call and message_sending, src/redaction/hooks.ts:158-206).
+ * The contract is exactly cg_find_matches_batch's / cg_redact_batch's: signature, spans, bytes, offsets, digests, return
+ * codes, argument checks, partial writes on CG_ERR_CAPACITY and statistics (except kernel_launches and last_scan_ms).  Only
+ * the cost differs: up to 256 strings and 64 KB of text cost one H2D copy, one CUDA graph, one D2H copy and one synchronise
+ * (DESIGN.md section 4.5), as cg_find_matches_one / cg_redact_one do for one string.  More strings or more text, profiling,
+ * a queue overflow and the rare result too long for the staging block take the batch call's path. */
+CG_API int cg_find_matches_few(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, uint32_t n,
+                               cg_span *out_spans, uint32_t spans_cap, uint32_t *out_nspans);
+CG_API int cg_redact_few(cg_ruleset *rs, const uint8_t *bytes, const uint32_t *offsets, uint32_t n,
+                         uint8_t *out_bytes, uint64_t out_cap, uint64_t *out_need, uint32_t *out_offsets,
+                         cg_span *out_spans, uint32_t spans_cap, uint32_t *out_nspans, uint8_t *out_digests32);
 
 /* ---- device-resident variant (inputs/outputs already in HBM; used by bench.py `value` and by callers that pipeline
  * their own copies).  Pointers are CUDA device pointers; `stream` is a cudaStream_t (NULL = the library's own stream);

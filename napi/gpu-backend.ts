@@ -3,7 +3,7 @@
  * (packages/openclaw-governance/src/gpu-backend.ts).  It keeps the plugin's classes and call sites and swaps the two hot
  * loops and the hash for calls into the N-API addon built from napi/openclaw_gov_napi.c:
  *
- *   PatternRegistry.findMatches   src/redaction/registry.ts:212-242,288-316   -> findMatchesOne / findMatchesBatch (spans already resolved)
+ *   PatternRegistry.findMatches   src/redaction/registry.ts:212-242,288-316   -> findMatchesOne / findMatchesFew / findMatchesBatch (spans already resolved)
  *   matchesAny                    src/conditions/context.ts:9-25              -> scanBatch over every pattern of the policy set
  *   ResponseGate mustMatch / mustNotMatch  src/response-gate.ts:104-149       -> scanBatch
  *   tool param `matches`          src/conditions/tool.ts:36-45                -> scanBatch
@@ -30,6 +30,9 @@ type Addon = {
   redactBatch(handle: unknown, bytes: Uint8Array, offsets: Uint32Array): { bytes: Uint8Array; offsets: Uint32Array; spans: Uint32Array; digests: Uint8Array };
   findMatchesOne(handle: unknown, bytes: Uint8Array): Uint32Array;
   redactOne(handle: unknown, bytes: Uint8Array): { bytes: Uint8Array; spans: Uint32Array; digests: Uint8Array };
+  // the strings of one scanned value, blocking, one device round trip (up to 256 strings and 64 KB): the batch calls' results
+  findMatchesFew(handle: unknown, bytes: Uint8Array, offsets: Uint32Array): Uint32Array;
+  redactFew(handle: unknown, bytes: Uint8Array, offsets: Uint32Array): { bytes: Uint8Array; offsets: Uint32Array; spans: Uint32Array; digests: Uint8Array };
   setPolicy(handle: unknown, rulePolicy: Uint32Array, ruleAction: Uint8Array): void;
   verdictBatch(handle: unknown, bytes: Uint8Array, offsets: Uint32Array): Uint32Array;
   // per-message views of one rule set: rows = nViews x ceil(nRules / 32) words (bit r = rule r in the view); views = one id
@@ -116,6 +119,19 @@ export class GpuPatternRegistry {
     for (let k = 0; k < spans.length; k += 6) {
       const [, rule, , , s16, e16] = spans.subarray(k, k + 6);
       out.push({ pattern: this.patterns[rule], match: text.slice(s16, e16), index: s16, length: e16 - s16 });
+    }
+    return out;
+  }
+
+  /** findMatches for every string leaf of one value RedactionEngine.scanValue walks (src/redaction/engine.ts:94-147), collected
+   *  in walk order: one blocking call, one device round trip; per string the same array findMatches returns. */
+  findMatchesFew(texts: string[]): ReturnType<GpuPatternRegistry["findMatchesBatch"]> {
+    const { bytes, offsets } = pack(texts);
+    const spans = addon.findMatchesFew(this.handle, bytes, offsets);    // msg, rule, startByte, endByte, start16, end16
+    const out: ReturnType<GpuPatternRegistry["findMatchesBatch"]> = texts.map(() => []);
+    for (let k = 0; k < spans.length; k += 6) {
+      const [msg, rule, , , s16, e16] = spans.subarray(k, k + 6);
+      out[msg].push({ pattern: this.patterns[rule], match: texts[msg].slice(s16, e16), index: s16, length: e16 - s16 });
     }
     return out;
   }

@@ -21,6 +21,8 @@
  *   redactBatch(handle, bytes, offsets): {bytes, offsets, spans, digests}  // scanString for a batch, spliced on the device
  *   findMatchesOne(handle, bytes: Uint8Array): Uint32Array  // one message, blocking: findMatchesBatch's spans for a batch of one
  *   redactOne(handle, bytes: Uint8Array): {bytes, spans, digests}  // one message, blocking: scanString spliced on the device
+ *   findMatchesFew(handle, bytes, offsets): Uint32Array  // the strings of one scanned value, blocking, one device round trip
+ *   redactFew(handle, bytes, offsets): {bytes, offsets, spans, digests}  //   (up to 256 strings and 64 KB): the batch calls' results
  *   setPolicy(handle, rulePolicy: Uint32Array, ruleAction: Uint8Array): void ; verdictBatch(handle, bytes, offsets): Uint32Array
  *   setViews(handle, rows: Uint32Array, nViews: number): void  // nViews rows of ceil(nRules / 32) words, bit r = rule r in the view
  *   scanBatchViews / findMatchesBatchViews / redactBatchViews / verdictBatchViews(handle, bytes, offsets, views: Uint8Array)
@@ -577,6 +579,59 @@ static napi_value js_redact_one(napi_env env, napi_callback_info info) {
   return res;
 }
 
+/* ---- the few strings of one scanned value, blocking: RedactionEngine.scan's findMatches / scanString for all its string
+ * leaves in one device round trip (cg_find_matches_few / cg_redact_few); results as findMatchesBatch / redactBatch */
+static napi_value js_find_matches_few(napi_env env, napi_callback_info info) {
+  BATCH_ARGS(env, info, 0)
+  cg_ruleset *rs; uint8_t *bytes, *offp;
+  NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
+  const int64_t nn = get_batch(env, argv[1], argv[2], 0, &bytes, &offp); if (nn < 0) return NULL;
+  const uint32_t n = (uint32_t)nn;
+  if (!bytes) bytes = one_empty;                    /* an empty typed array may report NULL: the C ABI rejects a NULL byte buffer */
+  uint32_t ns = 0, cap = 64; cg_span *tmp = (cg_span *)malloc(sizeof(cg_span) * cap);
+  int rc = tmp ? cg_find_matches_few(rs, bytes, (const uint32_t *)offp, n, tmp, cap, &ns) : CG_ERR_NOMEM;
+  if (rc == CG_ERR_CAPACITY) { cap = ns; cg_span *t2 = (cg_span *)realloc(tmp, sizeof(cg_span) * cap); if (t2) { tmp = t2; rc = cg_find_matches_few(rs, bytes, (const uint32_t *)offp, n, tmp, cap, &ns); } }
+  if (rc != CG_OK) { free(tmp); napi_throw_error(env, NULL, rc == CG_ERR_NOMEM ? "out of host memory" : cg_last_error()); return NULL; }
+  napi_value ab, arr; void *data;
+  if (napi_create_arraybuffer(env, (size_t)ns * sizeof(cg_span), &data, &ab) != napi_ok) { free(tmp); napi_throw_error(env, NULL, "N-API call failed"); return NULL; }
+  memcpy(data, tmp, (size_t)ns * sizeof(cg_span)); free(tmp);
+  NAPI_CALL(env, napi_create_typedarray(env, napi_uint32_array, (size_t)ns * 6, ab, 0, &arr));
+  return arr;
+}
+
+static napi_value js_redact_few(napi_env env, napi_callback_info info) {
+  BATCH_ARGS(env, info, 0)
+  cg_ruleset *rs; uint8_t *bytes, *offp;
+  NAPI_CALL(env, napi_get_value_external(env, argv[0], (void **)&rs));
+  const int64_t nn = get_batch(env, argv[1], argv[2], 0, &bytes, &offp); if (nn < 0) return NULL;
+  const uint32_t n = (uint32_t)nn;
+  if (!bytes) bytes = one_empty;
+  const uint32_t *off = (const uint32_t *)offp;
+  uint32_t ns = 0, cap_spans = 64; uint64_t need = 0, cap_bytes = (uint64_t)(off[n] - off[0]) + 1024;
+  napi_value off_ab, off_arr; void *off_data;
+  NAPI_CALL(env, napi_create_arraybuffer(env, (size_t)(n + 1) * 4, &off_data, &off_ab));
+  uint8_t *out = NULL, *dig = NULL; cg_span *spans = NULL; int rc = CG_ERR_NOMEM;
+  for (;;) {
+    uint8_t *o2 = (uint8_t *)realloc(out, cap_bytes + 64); cg_span *s2 = (cg_span *)realloc(spans, sizeof(cg_span) * cap_spans); uint8_t *d2 = (uint8_t *)realloc(dig, (size_t)cap_spans * 32);
+    if (o2) out = o2;
+    if (s2) spans = s2;
+    if (d2) dig = d2;
+    if (!o2 || !s2 || !d2) { rc = CG_ERR_NOMEM; break; }
+    rc = cg_redact_few(rs, bytes, off, n, out, cap_bytes, &need, (uint32_t *)off_data, spans, cap_spans, &ns, dig);
+    if (rc == CG_ERR_CAPACITY && (need > cap_bytes || ns > cap_spans)) { if (need > cap_bytes) cap_bytes = need; if (ns > cap_spans) cap_spans = ns; continue; }
+    break;
+  }
+  if (rc != CG_OK) { free(out); free(spans); free(dig); napi_throw_error(env, NULL, rc == CG_ERR_NOMEM ? "out of host memory" : cg_last_error()); return NULL; }
+  napi_value res = NULL, b_arr = make_u8(env, out, (size_t)need), d_arr = make_u8(env, dig, (size_t)ns * 32), s_ab, s_arr = NULL; void *p;
+  int ok = b_arr && d_arr && napi_create_arraybuffer(env, (size_t)ns * sizeof(cg_span), &p, &s_ab) == napi_ok;
+  if (ok) { memcpy(p, spans, (size_t)ns * sizeof(cg_span)); ok = napi_create_typedarray(env, napi_uint32_array, (size_t)ns * 6, s_ab, 0, &s_arr) == napi_ok; }
+  free(out); free(spans); free(dig);
+  if (!ok || napi_create_typedarray(env, napi_uint32_array, (size_t)n + 1, off_ab, 0, &off_arr) != napi_ok || napi_create_object(env, &res) != napi_ok) { napi_throw_error(env, NULL, "N-API call failed"); return NULL; }
+  NAPI_CALL(env, napi_set_named_property(env, res, "bytes", b_arr)); NAPI_CALL(env, napi_set_named_property(env, res, "offsets", off_arr));
+  NAPI_CALL(env, napi_set_named_property(env, res, "spans", s_arr)); NAPI_CALL(env, napi_set_named_property(env, res, "digests", d_arr));
+  return res;
+}
+
 /* one context owning every text (cg_policy_eval_one): the texts, their roles and ceil(nAtoms / 32) atom words, nAtoms as given to
  * setPolicyProgram -> {verdict, rules} */
 static napi_value js_policy_eval_one(napi_env env, napi_callback_info info) {
@@ -615,6 +670,7 @@ static napi_value module_init(napi_env env, napi_value exports) {
     FN("createRuleset", js_create_ruleset), FN("scanBatch", js_scan_batch), FN("scanOne", js_scan_one),
     FN("findMatchesBatch", js_find_matches_batch), FN("redactBatch", js_redact_batch),
     FN("findMatchesOne", js_find_matches_one), FN("redactOne", js_redact_one),
+    FN("findMatchesFew", js_find_matches_few), FN("redactFew", js_redact_few),
     FN("setPolicy", js_set_policy), FN("verdictBatch", js_verdict_batch),
     FN("setViews", js_set_views), FN("scanBatchViews", js_scan_batch_views), FN("findMatchesBatchViews", js_find_matches_batch_views),
     FN("redactBatchViews", js_redact_batch_views), FN("verdictBatchViews", js_verdict_batch_views),

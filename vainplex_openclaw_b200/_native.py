@@ -65,7 +65,8 @@ EXPORTS = ["cg_init", "cg_shutdown", "cg_last_error", "cg_version", "cg_device_c
            "cg_redact_batch_device_views", "cg_policy_verdict_batch_device_views",
            "cg_merkle_log_append_device", "cg_merkle_log_append_fixed_device", "cg_merkle_log_root_device", "cg_merkle_log_proofs_device",
            "cg_merkle_log_consistency_between_device", "cg_merkle_verify_proofs_device", "cg_merkle_log_join",
-           "cg_ruleset_set_policy_program", "cg_policy_eval_batch", "cg_policy_eval_batch_device", "cg_policy_eval_one"]
+           "cg_ruleset_set_policy_program", "cg_policy_eval_batch", "cg_policy_eval_batch_device", "cg_policy_eval_one",
+           "cg_find_matches_few", "cg_redact_few"]
 
 _lib = None
 
@@ -128,6 +129,8 @@ def load():
     L.cg_find_matches_batch.argtypes = [vp, vp, vp, u32, vp, u32, C.POINTER(u32)]; L.cg_find_matches_batch.restype = i32
     L.cg_find_matches_one.argtypes = [vp, vp, u32, vp, u32, C.POINTER(u32)]; L.cg_find_matches_one.restype = i32
     L.cg_redact_one.argtypes = [vp, vp, u32, vp, u64, C.POINTER(u64), vp, u32, C.POINTER(u32), vp]; L.cg_redact_one.restype = i32
+    L.cg_find_matches_few.argtypes = [vp, vp, vp, u32, vp, u32, C.POINTER(u32)]; L.cg_find_matches_few.restype = i32
+    L.cg_redact_few.argtypes = [vp, vp, vp, u32, vp, u64, C.POINTER(u64), vp, vp, u32, C.POINTER(u32), vp]; L.cg_redact_few.restype = i32
     L.cg_scan_batch_device.argtypes = [vp, vp, vp, u32, vp, vp]; L.cg_scan_batch_device.restype = i32
     L.cg_find_matches_batch_device.argtypes = [vp, vp, vp, u32, vp, u32, vp, vp]; L.cg_find_matches_batch_device.restype = i32
     L.cg_redact_batch_device.argtypes = [vp, vp, vp, u32, vp, u64, vp, vp, u32, vp, vp, vp]; L.cg_redact_batch_device.restype = i32
@@ -350,6 +353,41 @@ class Ruleset:
                 continue
             check(rc)
             return out[:need.value].tobytes(), spans[:ns.value], dig[:ns.value]
+
+    def find_matches_few(self, data: np.ndarray, off: np.ndarray):
+        """findMatches for the few strings of one scanned value, blocking, one device round trip up to 256 strings and 64 KB
+        (cg_find_matches_few): -> what find_matches_batch returns."""
+        n = len(off) - 1
+        ns = C.c_uint32(0)
+        cap = 64
+        while True:
+            spans = np.zeros(cap, dtype=SPAN_DTYPE)
+            rc = load().cg_find_matches_few(self.handle, data.ctypes.data, off.ctypes.data, n, spans.ctypes.data, cap, C.byref(ns))
+            if rc == CG_ERR_CAPACITY and ns.value > cap:
+                cap = ns.value
+                continue
+            check(rc)
+            return spans[:ns.value]
+
+    def redact_few(self, data: np.ndarray, off: np.ndarray):
+        """RedactionEngine.scanString for the few strings of one scanned value, blocking, spliced on the device, one round
+        trip up to 256 strings and 64 KB (cg_redact_few): -> what redact_batch returns."""
+        n = len(off) - 1
+        total = int(off[n] - off[0]) if n else 0
+        out_off = np.zeros(n + 1, dtype=np.uint32)
+        need, ns = C.c_uint64(0), C.c_uint32(0)
+        cap_bytes, cap_spans = total + 1024, 64
+        while True:
+            out = np.zeros(cap_bytes + 64, dtype=np.uint8)
+            spans = np.zeros(cap_spans, dtype=SPAN_DTYPE)
+            dig = np.zeros((cap_spans, 32), dtype=np.uint8)
+            rc = load().cg_redact_few(self.handle, data.ctypes.data, off.ctypes.data, n, out.ctypes.data, cap_bytes, C.byref(need),
+                                      out_off.ctypes.data, spans.ctypes.data, cap_spans, C.byref(ns), dig.ctypes.data)
+            if rc == CG_ERR_CAPACITY and (need.value > cap_bytes or ns.value > cap_spans):
+                cap_bytes, cap_spans = max(cap_bytes, need.value), max(cap_spans, ns.value)
+                continue
+            check(rc)
+            return out[:need.value], out_off, spans[:ns.value], dig[:ns.value]
 
     def set_policy(self, rule_policy, rule_action):
         """rule i belongs to policy rule_policy[i] (evaluation order, non-decreasing) with effect rule_action[i] (0 allow, 1 audit, 2 deny)."""

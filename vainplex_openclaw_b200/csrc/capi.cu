@@ -150,12 +150,18 @@ struct cg_ruleset {
   uint64_t scratch_gen = 0;       // advanced by every change to what a captured step holds (scratch buffers, DevRuleset)
   // the device-resident step replayed as one CUDA graph (keyed on its arguments, the scratch generation and the verify grid)
   struct CachedGraph { int kernels = 0; cudaGraphExec_t exec = nullptr; const void* bytes = nullptr; const void* off = nullptr; void* words = nullptr; uint32_t n = 0; uint64_t gen = 0; int ctas = 0; uint64_t used = 0; };
-  // cg_scan_one / cg_find_matches_one / cg_redact_one: pinned staging + one device block ([offsets][message bytes] in,
-  // [word][counters][hit row] out), for the span calls a second pair (the packed result, and on the device its scratch;
-  // capi.cu kOne*), and per mode the step as a graph over those fixed addresses (the message length is data, so one graph
-  // serves every message)
+  // cg_scan_one: pinned staging + one device block ([offsets][message bytes] in, [word][counters][hit row] out) and the step
+  // as a graph over those fixed addresses (the message length is data, so one graph serves every message); for the span
+  // calls a second pair (the packed result, and on the device its scratch; capi.cu kOne*)
   struct OneGraph { cudaGraphExec_t exec = nullptr; uint64_t gen = 0; int ctas = 0; int kernels = 0; };
-  struct OnePath { OneGraph g[3]; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint8_t* h_pack = nullptr; uint8_t* d_pack = nullptr; } one;
+  struct OnePath { OneGraph g; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint8_t* h_pack = nullptr; uint8_t* d_pack = nullptr; } one;
+  // cg_find_matches_one / cg_redact_one / cg_find_matches_few / cg_redact_few: pinned staging + one device block ([offsets]
+  // [text bytes] in, capi.cu kFew*), and the step + resolver (+ digests and splice) + pack as graphs over those fixed
+  // addresses and one.d_pack, one per (mode, message count) (the step takes the count by value), the least recently used
+  // of kSpanGraphs re-targeted
+  static constexpr int kSpanGraphs = 16;
+  struct SpanGraph { cudaGraphExec_t exec = nullptr; uint32_t n = 0; bool redact = false; uint64_t gen = 0, used = 0; int ctas = 0, kernels = 0; };
+  struct SpanFew { SpanGraph g[kSpanGraphs]; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint64_t clock = 0; } few;
   CachedGraph graphs[2];          // two entries: callers that alternate between two input/output buffer sets replay, never re-capture
   uint64_t graph_clock = 0;
   // cg_ruleset_set_views: n_views rows of dev.rw words in HBM (bit r of row v = rule r is in view v); none before the first call
@@ -173,7 +179,10 @@ struct cg_ruleset {
   ~cg_ruleset() {
     cudaFree(view_rows); cudaFree(prog_ops); cudaFree(prog_rules);
     for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    for (auto& g : one.g) if (g.exec) cudaGraphExecDestroy(g.exec);
+    if (one.g.exec) cudaGraphExecDestroy(one.g.exec);
+    for (auto& g : few.g) if (g.exec) cudaGraphExecDestroy(g.exec);
+    if (few.h_pin) cudaFreeHost(few.h_pin);
+    cudaFree(few.d_buf);
     for (auto& g : pone.g) if (g.exec) cudaGraphExecDestroy(g.exec);
     if (pone.h_pin) cudaFreeHost(pone.h_pin);
     cudaFree(pone.d_buf);
@@ -335,9 +344,10 @@ void count_step(uint32_t n, uint64_t bytes, const uint32_t* hc) {
   G.stats.messages_scanned += n; G.stats.bytes_scanned += bytes;
   G.stats.candidate_events += hc[kCtrEvents]; G.stats.verified_pairs += hc[kCtrEvents];
 }
-// the kernels enqueue() puts on st, captured as one graph; they are counted each time the graph is launched, not here
+// the kernels enqueue() puts on st, recorded as one graph (*graph: the caller's to destroy); they are counted each time an
+// instance is launched, not here
 template <typename Enqueue>
-int capture(cudaStream_t st, Enqueue&& enqueue, cudaGraphExec_t* exec, int* kernels) {
+int record(cudaStream_t st, Enqueue&& enqueue, cudaGraph_t* graph, int* kernels) {
   cudaGraph_t g = nullptr;
   const uint64_t before = G.stats.kernel_launches;
   CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
@@ -345,7 +355,15 @@ int capture(cudaStream_t st, Enqueue&& enqueue, cudaGraphExec_t* exec, int* kern
   cudaError_t e = cudaStreamEndCapture(st, &g);
   *kernels = (int)(G.stats.kernel_launches - before); G.stats.kernel_launches = before;
   if (rc != CG_OK || e != cudaSuccess) { if (g) cudaGraphDestroy(g); cudaGetLastError(); return rc != CG_OK ? rc : cuda_fail(e, "cudaStreamEndCapture"); }
-  e = cudaGraphInstantiate(exec, g, 0);
+  *graph = g;
+  return CG_OK;
+}
+// the same, instantiated
+template <typename Enqueue>
+int capture(cudaStream_t st, Enqueue&& enqueue, cudaGraphExec_t* exec, int* kernels) {
+  cudaGraph_t g = nullptr;
+  if (int rc = record(st, enqueue, &g, kernels)) return rc;
+  const cudaError_t e = cudaGraphInstantiate(exec, g, 0);
   cudaGraphDestroy(g);
   if (e != cudaSuccess) { *exec = nullptr; return cuda_fail(e, "cudaGraphInstantiate"); }
   return CG_OK;
@@ -504,28 +522,35 @@ int mirror_counters(cg_ruleset* rs, cudaStream_t st) {
 }
 
 // The single-message staging block, host (pinned) and device: [offsets, 256 B][message bytes][64 zero bytes] in (kOneIn),
-// [word][counters][hit row] out (kOneOut).  The span calls add, on their first use, the packed result (kOnePack bytes,
-// layout in kernels.h) on both sides and, on the device only, the digests and the redacted bytes before the pack step
-// moves them behind the spans (kOnePack each).
+// [word][counters][hit row] out (kOneOut).  The span calls stage their input in their own block (kFew*) and add, on their
+// first use, the packed result (kOnePack bytes, layout in kernels.h) on both sides and, on the device only, the digests and
+// the redacted bytes before the pack step moves them behind the spans (kOnePack each).
 constexpr uint32_t kOneBytes = 16384, kOneRw = 128, kOneIn = 256 + kOneBytes + 64, kOneOut = (kOneHitRow + kOneRw) * 4;
 constexpr uint32_t kOnePack = 512 * 1024;
-// the resolver's capacities on this path: every resolved span (and, redacting, its digest and the output) must fit the block
-constexpr uint32_t kOneSpansFind = (kOnePack - kPackHeader) / 24, kOneSpansRedact = (kOnePack - kPackHeader) / 56;
-enum { kOneScan = 0, kOneFind = 1, kOneRedact = 2 };
+// The span calls' staging block, host (pinned) and device: [offsets, kFewMsgs + 1][text bytes, kFewBytes][64 zero bytes],
+// the offsets rebased to kFewTextAt.  The limits: 256 strings (kFewMsgs: the resolver keeps its per-message arrays in shared
+// memory) and 64 KB of text (cg_policy_eval_one's limit); the _one calls keep 16 KB (kOneBytes).
+constexpr uint32_t kFewBytes = 65536, kFewTextAt = 1280, kFewIn = kFewTextAt + kFewBytes + 64;
+static_assert(4 * (kFewMsgs + 1) <= kFewTextAt && kFewTextAt % 256 == 0 && pack_spans_at(kFewMsgs) < 4096, "span call staging layout");
 
-// (spans: also the span calls' packed result and scratch)
-int one_staging(cg_ruleset::OnePath& o, bool spans) {
+int one_staging(cg_ruleset::OnePath& o) {
   if (!o.h_pin) { CU(cudaMallocHost((void**)&o.h_pin, kOneIn + kOneOut)); memset(o.h_pin, 0, kOneIn + kOneOut); }
   if (!o.d_buf) { CU(cudaMalloc((void**)&o.d_buf, kOneIn + kOneOut)); CU(cudaMemset(o.d_buf, 0, kOneIn + kOneOut)); }
-  if (!spans) return CG_OK;
+  return CG_OK;
+}
+// the span calls' staging block, packed result and scratch
+int few_staging(cg_ruleset* rs) {
+  cg_ruleset::SpanFew& f = rs->few; cg_ruleset::OnePath& o = rs->one;
+  if (!f.h_pin) { CU(cudaMallocHost((void**)&f.h_pin, kFewIn)); memset(f.h_pin, 0, kFewIn); }
+  if (!f.d_buf) { CU(cudaMalloc((void**)&f.d_buf, kFewIn)); CU(cudaMemset(f.d_buf, 0, kFewIn)); }
   if (!o.h_pack) { CU(cudaMallocHost((void**)&o.h_pack, kOnePack)); memset(o.h_pack, 0, kOnePack); }
   if (!o.d_pack) { CU(cudaMalloc((void**)&o.d_pack, 3 * (size_t)kOnePack)); CU(cudaMemset(o.d_pack, 0, 3 * (size_t)kOnePack)); }
   return CG_OK;
 }
-// mode m's graph, captured again when the scratch or the verify grid changed since it was captured
+// cg_scan_one's graph, captured again when the scratch or the verify grid changed since it was captured
 template <typename Enqueue>
-int one_graph(cg_ruleset* rs, int m, Enqueue&& enqueue) {
-  cg_ruleset::OneGraph& g = rs->one.g[m];
+int one_graph(cg_ruleset* rs, Enqueue&& enqueue) {
+  cg_ruleset::OneGraph& g = rs->one.g;
   if (g.exec && g.gen == rs->scratch_gen && g.ctas == rs->verify_ctas) return CG_OK;
   if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
   if (int rc = capture(G.stream, enqueue, &g.exec, &g.kernels)) return rc;
@@ -599,6 +624,35 @@ int enqueue_redact_tail(const ScanWork& w, const uint8_t* d_bytes, const uint32_
   const int k = launch_redact_digests(d_bytes, w.sp_start, w.sp_len, w.counters + kCtrDigests, d_digests, G.sm_count, st);
   return k + launch_redact_splice(d_bytes, d_off, d_out_offsets, w.kept_begin, w.sp_start, w.sp_len, w.sp_cat, d_digests, d_out,
                                   w.counters + kCtrSplice, n, G.sm_count, st);
+}
+
+// the span graph of (mode, n), captured when the cache has none for the current scratch and verify grid: recorded afresh and
+// put into the least recently used entry, whose instance is re-targeted (cudaGraphExecUpdate: the launch sequence does not
+// depend on n, so only parameters change) and instantiated anew only when the update is refused
+template <typename Enqueue>
+int few_graph(cg_ruleset* rs, uint32_t n, bool redact, Enqueue&& enqueue, cg_ruleset::SpanGraph** out) {
+  cg_ruleset::SpanFew& f = rs->few;
+  cg_ruleset::SpanGraph* g = nullptr;
+  for (auto& e : f.g) if (e.exec && e.n == n && e.redact == redact && e.gen == rs->scratch_gen && e.ctas == rs->verify_ctas) g = &e;
+  if (!g) {
+    g = &f.g[0];
+    for (auto& e : f.g) if (e.used < g->used) g = &e;
+    cudaGraph_t graph = nullptr;
+    int kernels = 0;
+    if (int rc = record(G.stream, enqueue, &graph, &kernels)) return rc;
+    cudaGraphExecUpdateResultInfo info;
+    if (!g->exec || cudaGraphExecUpdate(g->exec, graph, &info) != cudaSuccess) {
+      cudaGetLastError();                                     // (a refused update is not an error of the call)
+      if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; }
+      const cudaError_t e = cudaGraphInstantiate(&g->exec, graph, 0);
+      if (e != cudaSuccess) { cudaGraphDestroy(graph); g->exec = nullptr; return cuda_fail(e, "cudaGraphInstantiate"); }
+    }
+    cudaGraphDestroy(graph);
+    g->n = n; g->redact = redact; g->gen = rs->scratch_gen; g->ctas = rs->verify_ctas; g->kernels = kernels;
+  }
+  g->used = ++f.clock;
+  *out = g;
+  return CG_OK;
 }
 
 }  // namespace
@@ -891,20 +945,20 @@ int scan_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* 
   InOrder turn(&rs->order, st);
   int rc;
   if ((rc = turn.rc)) return rc;
-  if ((rc = one_staging(o, false))) return rc;
+  if ((rc = one_staging(o))) return rc;
   if ((rc = prepare_step(rs, 1, kStepWords, st))) return rc;
   const uint8_t* d_bytes = o.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(o.d_buf);
   uint32_t* d_out = reinterpret_cast<uint32_t*>(o.d_buf + kOneIn); uint64_t* d_word = reinterpret_cast<uint64_t*>(o.d_buf + kOneIn + kOneOut - 8);   // (the word lands behind the hit row, then is packed to the front)
-  if ((rc = one_graph(rs, kOneScan, [&] {
+  if ((rc = one_graph(rs, [&] {
         const int r = run_scan_device(rs, d_bytes, d_off, 1, d_word, kStepWords, st);
         if (r == CG_OK) count_launches(launch_pack_one(rs->dev, rs->work, d_word, d_out, kOneRw - 2, st));
         return r;
       }))) return rc;
   if ((rc = stage_one(o, bytes, len, st))) return rc;
-  CU(cudaGraphLaunch(o.g[kOneScan].exec, st));
+  CU(cudaGraphLaunch(o.g.exec, st));
   CU(cudaMemcpyAsync(o.h_pin + kOneIn, d_out, (kOneHitRow + rs->dev.rw) * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  count_launches(o.g[kOneScan].kernels);
+  count_launches(o.g.kernels);
   const uint32_t* ho = reinterpret_cast<const uint32_t*>(o.h_pin + kOneIn);
   const uint32_t* hc = ho + kOneCounters;
   if ((rc = absorb_counters(rs, hc))) return rc;                 // 1: a queue overflowed, the general path retries with larger scratch
@@ -1097,58 +1151,68 @@ int cg_redact_batch_views(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* 
 }
 
 namespace {
-struct OneSpanOut { cg_span* spans; uint32_t spans_cap; uint32_t* nspans; uint8_t* bytes; uint64_t out_cap; uint64_t* need; uint8_t* digests; };
-// cg_find_matches_one / cg_redact_one on the staging block: one H2D copy, one graph (span-mode step, one-block resolver,
-// digests and splice when redacting, pack), one D2H copy of the header plus a window sized from len, one synchronise; a
-// second copy and synchronise only for a packed result longer than the window.  Outputs, statuses and statistics are those
-// of the batch call with n = 1.  -> CG_OK, an error, or 1 = take the batch path (an argument the batch call rejects, no
-// device, a long message, profiling, a queue overflowed, or a result longer than the staging block)
-int span_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, bool redact, const OneSpanOut& out) {
-  if (!G.ready || !rs || !bytes || len > kOneBytes || G.profiling) return 1;
-  cg_ruleset::OnePath& o = rs->one;
+struct OneSpanOut { cg_span* spans; uint32_t spans_cap; uint32_t* nspans; uint8_t* bytes; uint64_t out_cap; uint64_t* need; uint8_t* digests; uint32_t* offsets; };
+
+// cg_find_matches_one / cg_redact_one (n = 1) and cg_find_matches_few / cg_redact_few on the staging block: one H2D copy,
+// one graph (span-mode step over the n staged strings, one-block resolver, digests and splice when redacting, pack), one D2H
+// copy of the header plus a window sized from the text length, one synchronise; a second copy and synchronise only for a
+// packed result longer than the window.  Outputs, statuses and statistics are those of the batch call.  -> CG_OK, an error,
+// or 1 = take the batch call (an argument the batch call rejects, no device, more than kFewMsgs strings or max_bytes of
+// text, profiling, a queue overflowed, or a result longer than the packed region)
+int span_few_fast(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint32_t max_bytes, bool redact, const OneSpanOut& out) {
+  if (!G.ready || !rs || G.profiling || n > kFewMsgs || (n && (!bytes || !offsets)) || (redact && !out.offsets)) return 1;
+  for (uint32_t i = 0; i < n; i++) if (offsets[i + 1] < offsets[i]) return 1;
+  const uint32_t first = n ? offsets[0] : 0, len = n ? offsets[n] - first : 0;
+  if (len > max_bytes) return 1;
+  cg_ruleset::SpanFew& f = rs->few;
   cudaStream_t st = G.stream;
   InOrder turn(&rs->order, st);
   int rc;
   if ((rc = turn.rc)) return rc;
-  if ((rc = one_staging(o, true))) return rc;
-  if ((rc = prepare_step(rs, 1, kStepSpans, st))) return rc;
+  if ((rc = few_staging(rs))) return rc;
+  if ((rc = prepare_step(rs, n, kStepSpans, st))) return rc;
   const ScanWork& w = rs->work;
-  const uint8_t* d_bytes = o.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(o.d_buf);
-  uint32_t* d_pack = reinterpret_cast<uint32_t*>(o.d_pack);
-  uint32_t* d_dig = reinterpret_cast<uint32_t*>(o.d_pack + kOnePack);
-  uint8_t* d_out = o.d_pack + 2 * kOnePack;
-  const int m = redact ? kOneRedact : kOneFind;
-  if ((rc = one_graph(rs, m, [&] {
-        const int r = run_scan_device(rs, d_bytes, d_off, 1, w.words, kStepSpans, st);
+  const uint8_t* d_bytes = f.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(f.d_buf);
+  uint32_t* d_pack = reinterpret_cast<uint32_t*>(rs->one.d_pack);
+  uint32_t* d_dig = reinterpret_cast<uint32_t*>(rs->one.d_pack + kOnePack);
+  uint8_t* d_out = rs->one.d_pack + 2 * kOnePack;
+  // the resolver's capacities on this path: every resolved span (and, redacting, its digest and the output) must fit the block
+  const uint32_t at = pack_spans_at(n), room = kOnePack - at;
+  cg_ruleset::SpanGraph* g = nullptr;
+  if ((rc = few_graph(rs, n, redact, [&] {
+        const int r = run_scan_device(rs, d_bytes, d_off, n, w.words, kStepSpans, st);
         if (r != CG_OK) return r;
-        const SpanOutputs so{d_pack + kPackHeader / 4, redact ? kOneSpansRedact : kOneSpansFind, d_pack + kPackOffsets,
-                             redact ? (uint64_t)(kOnePack - kPackHeader) : 0ull, d_pack + kPackSizes, redact};
-        int k = launch_span_resolve_one(w, d_off, so, st);
-        if (redact) k += enqueue_redact_tail(w, d_bytes, d_off, d_pack + kPackOffsets, d_dig, d_out, 1, st);
-        k += launch_span_pack_one(w, d_dig, d_out, d_pack, kOnePack, redact, st);
+        const SpanOutputs so{d_pack + at / 4, room / (redact ? 56u : 24u), d_pack + kPackOffsets, redact ? (uint64_t)room : 0ull, d_pack + kPackSizes, redact};
+        int k = launch_span_resolve_few(w, d_off, n, so, st);
+        if (redact) k += enqueue_redact_tail(w, d_bytes, d_off, d_pack + kPackOffsets, d_dig, d_out, n, st);
+        k += launch_span_pack_few(w, d_dig, d_out, d_pack, kOnePack, n, redact, st);
         count_launches(k);
         CU(cudaGetLastError());
         return CG_OK;
-      }))) return rc;
-  if ((rc = stage_one(o, bytes, len, st))) return rc;
-  CU(cudaGraphLaunch(o.g[m].exec, st));
-  // the window: the header, 1 KB and len / 2 bytes (find-matches) or 2 x len bytes (redaction) of the packed result
-  const uint32_t window = std::min<uint32_t>(kOnePack, kPackHeader + 1024 + (redact ? 2 * len : len / 2));
-  uint8_t* h_pack = o.h_pack;
+      }, &g))) return rc;
+  uint32_t* hoff = reinterpret_cast<uint32_t*>(f.h_pin);
+  for (uint32_t i = 0; i <= n; i++) hoff[i] = kFewTextAt + (n ? offsets[i] - first : 0);
+  if (len) memcpy(f.h_pin + kFewTextAt, bytes + first, len);
+  memset(f.h_pin + kFewTextAt + len, 0, 64);
+  CU(cudaMemcpyAsync(f.d_buf, f.h_pin, (size_t)kFewTextAt + len + 64, cudaMemcpyHostToDevice, st));
+  CU(cudaGraphLaunch(g->exec, st));
+  // the window: the header with the offsets, 1 KB and len / 2 bytes (find-matches) or 2 x len bytes (redaction) of the packed result
+  const uint32_t window = std::min<uint32_t>(kOnePack, at + 1024 + (redact ? 2 * len : len / 2));
+  uint8_t* h_pack = rs->one.h_pack;
   CU(cudaMemcpyAsync(h_pack, d_pack, window, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  count_launches(o.g[m].kernels);
+  count_launches(g->kernels);
   const uint32_t* hp = reinterpret_cast<const uint32_t*>(h_pack);
   const uint32_t* hc = hp + kPackCounters;
   if ((rc = absorb_counters(rs, hc))) return rc;                 // 1: a queue overflowed, the batch call retries with larger scratch
   const uint32_t packed = hp[0];
-  if (!packed) return 1;                                         // longer than the staging block: the batch call has room
+  if (!packed) return 1;                                         // longer than the packed region: the batch call has room
   if (packed > window) {
     CU(cudaMemcpyAsync(h_pack + window, reinterpret_cast<const uint8_t*>(d_pack) + window, packed - window, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
   }
-  count_step(1, len, hc);
-  const uint8_t* body = h_pack + kPackHeader;
+  count_step(n, len, hc);
+  const uint8_t* body = h_pack + at;
   if (!redact) {
     const uint32_t ns = hp[kPackSizes];
     G.stats.spans += ns;
@@ -1164,6 +1228,7 @@ int span_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, bool redac
   G.stats.spans += ns;
   if (out.need) *out.need = need;
   if (out.nspans) *out.nspans = ns;
+  memcpy(out.offsets, hp + kPackOffsets, ((size_t)n + 1) * 4);
   if (need >> 32) return fail(CG_ERR_TOO_LARGE, "redacted batch exceeds 4 GiB");
   if ((out.spans && ns > out.spans_cap) || need > out.out_cap || !out.bytes) return fail(CG_ERR_CAPACITY, "output buffer too small (see *out_need / *out_nspans)");
   G.stats.sha256_items += ns;
@@ -1175,17 +1240,28 @@ int span_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, bool redac
 }  // namespace
 
 int cg_find_matches_one(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans) {
-  { std::lock_guard<std::mutex> lk(g_mu); const int frc = span_one_fast(rs, bytes, len, false, OneSpanOut{out_spans, spans_cap, out_nspans, nullptr, 0, nullptr, nullptr}); if (frc != 1) return frc; }
   const uint32_t off[2] = {0, len};
+  { std::lock_guard<std::mutex> lk(g_mu); const int frc = span_few_fast(rs, bytes, off, 1, kOneBytes, false, OneSpanOut{out_spans, spans_cap, out_nspans, nullptr, 0, nullptr, nullptr, nullptr}); if (frc != 1) return frc; }
   return cg_find_matches_batch(rs, bytes, off, 1, out_spans, spans_cap, out_nspans);
 }
 
 int cg_redact_one(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_need,
                   cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans, uint8_t* out_digests32) {
-  { std::lock_guard<std::mutex> lk(g_mu); const int frc = span_one_fast(rs, bytes, len, true, OneSpanOut{out_spans, spans_cap, out_nspans, out_bytes, out_cap, out_need, out_digests32}); if (frc != 1) return frc; }
   const uint32_t off[2] = {0, len};
   uint32_t out_off[2] = {0, 0};
+  { std::lock_guard<std::mutex> lk(g_mu); const int frc = span_few_fast(rs, bytes, off, 1, kOneBytes, true, OneSpanOut{out_spans, spans_cap, out_nspans, out_bytes, out_cap, out_need, out_digests32, out_off}); if (frc != 1) return frc; }
   return cg_redact_batch(rs, bytes, off, 1, out_bytes, out_cap, out_need, out_off, out_spans, spans_cap, out_nspans, out_digests32);
+}
+
+int cg_find_matches_few(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans) {
+  { std::lock_guard<std::mutex> lk(g_mu); const int frc = span_few_fast(rs, bytes, offsets, n, kFewBytes, false, OneSpanOut{out_spans, spans_cap, out_nspans, nullptr, 0, nullptr, nullptr, nullptr}); if (frc != 1) return frc; }
+  return cg_find_matches_batch(rs, bytes, offsets, n, out_spans, spans_cap, out_nspans);
+}
+
+int cg_redact_few(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uint32_t n, uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_need,
+                  uint32_t* out_offsets, cg_span* out_spans, uint32_t spans_cap, uint32_t* out_nspans, uint8_t* out_digests32) {
+  { std::lock_guard<std::mutex> lk(g_mu); const int frc = span_few_fast(rs, bytes, offsets, n, kFewBytes, true, OneSpanOut{out_spans, spans_cap, out_nspans, out_bytes, out_cap, out_need, out_digests32, out_offsets}); if (frc != 1) return frc; }
+  return cg_redact_batch(rs, bytes, offsets, n, out_bytes, out_cap, out_need, out_offsets, out_spans, spans_cap, out_nspans, out_digests32);
 }
 
 int cg_scan_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_out_words, void* stream) {

@@ -204,16 +204,20 @@ struct SpanOutputs {
 // whatever the span count.  Redact also leaves the splice's input in w.sp_* / w.kept_begin and sets counters[kCtrDigests] / [kCtrSplice] to the
 // spans to digest / messages to splice (0 unless every output fits).
 int launch_span_resolve(const ScanWork& w, const uint32_t* d_off, uint32_t n, const SpanOutputs& o, int sm_count, cudaStream_t stream);
-// the same for a batch of one message in one block (one launch, any raw span count up to w.span_cap)
-int launch_span_resolve_one(const ScanWork& w, const uint32_t* d_off, const SpanOutputs& o, cudaStream_t stream);
-// single-message span path: the result packed into one block for one D2H copy, as u32 words:
+// the same for a batch of n <= kFewMsgs messages in one block (one launch, any raw span count up to w.span_cap)
+constexpr uint32_t kFewMsgs = 256;
+int launch_span_resolve_few(const ScanWork& w, const uint32_t* d_off, uint32_t n, const SpanOutputs& o, cudaStream_t stream);
+// few-message span path (cg_find_matches_one / cg_redact_one at n = 1, cg_find_matches_few / cg_redact_few): the result of n
+// messages packed into one block for one D2H copy, as u32 words:
 //   [0] packed bytes (0: the result is incomplete, not ok, or longer than pack_cap -- the caller takes the batch path)
-//   [1] resolver status  [2..5] sizes (SpanOutputs.sizes)  [6..7] output offsets  [8..39] counter block
-//   then from byte kPackHeader: spans (6 words each), digests (32 bytes each, redact), output bytes (redact)
+//   [1] resolver status  [2..5] sizes (SpanOutputs.sizes)  [6..7] unused  [8..39] counter block
+//   from byte kPackHeader: the n + 1 output offsets (redact)
+//   then from byte pack_spans_at(n): spans (6 words each), digests (32 bytes each, redact), output bytes (redact)
 // The resolver writes the spans, sizes and offsets in place; the pack step adds the rest.
-constexpr uint32_t kPackSizes = 2, kPackOffsets = 6, kPackCounters = 8, kPackHeader = (kPackCounters + kCounterWords) * 4;
-int launch_span_pack_one(const ScanWork& w, const uint32_t* d_digests, const uint8_t* d_out, uint32_t* d_packed, uint32_t pack_cap, bool redact,
-                         cudaStream_t stream);
+constexpr uint32_t kPackSizes = 2, kPackCounters = 8, kPackOffsets = kPackCounters + kCounterWords, kPackHeader = kPackOffsets * 4;
+__host__ __device__ constexpr uint32_t pack_spans_at(uint32_t n) { return (kPackHeader + 4 * (n + 1) + 15) & ~15u; }
+int launch_span_pack_few(const ScanWork& w, const uint32_t* d_digests, const uint8_t* d_out, uint32_t* d_packed, uint32_t pack_cap, uint32_t n,
+                         bool redact, cudaStream_t stream);
 
 // SHA-256 / Merkle
 int launch_sha256_batch(const uint8_t* d_bytes, const uint64_t* d_off, uint32_t n, uint8_t* d_out, cudaStream_t stream);

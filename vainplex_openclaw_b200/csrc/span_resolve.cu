@@ -11,8 +11,9 @@
 //
 // Every launch geometry depends on n and the SM count only; the span count is read from device memory.
 //
-// A batch of one message (cg_find_matches_one / cg_redact_one) skips the chain: span_resolve_one_kernel builds the keys,
-// sorts, keeps and emits in one block, through the same sort_keep_segment as the long segments of a batch.
+// A batch of a few messages (cg_find_matches_one / cg_redact_one, cg_find_matches_few / cg_redact_few) skips the chain:
+// span_resolve_few_kernel runs the same stages in one block, with the per-message arrays in shared memory, through the same
+// warp_sort_keep / sort_keep_segment as the segments of a batch.
 #include <algorithm>
 #include <cstdint>
 
@@ -193,6 +194,56 @@ __device__ uint32_t sort_keep_segment(const ScanWork& w, const uint32_t* __restr
   return kc;
 }
 
+// The same for a segment of 1 .. kWarpSort keys, one warp: bitonic sort in registers, the greedy walk done by all lanes in
+// step.  Returns the number kept and, redacting, *delta (both on every lane).  Call from warp-uniform code.
+__device__ __forceinline__ uint32_t warp_sort_keep(const ScanWork& w, const uint32_t* __restrict__ category, uint32_t s0, uint32_t c, int redact,
+                                                   long long* delta) {
+  const uint32_t lane = threadIdx.x & 31;
+  uint4 v = lane < c ? w.sorted[s0 + lane] : pad_key();
+  for (uint32_t k = 2; k <= 32; k <<= 1)
+    for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+      const uint4 o = shfl_key(v, j, true);
+      const bool keep_min = ((lane & j) == 0) == ((lane & k) == 0);
+      if (keep_min ? key_less(o, v) : key_less(v, o)) v = o;
+    }
+  long long last_end = -1;
+  uint32_t keep = 0;
+  for (uint32_t j = 0; j < c; j++) {
+    const uint32_t s = __shfl_sync(0xffffffffu, v.x, j), e = __shfl_sync(0xffffffffu, key_end(v), j);
+    if ((long long)s >= last_end) { keep |= 1u << j; last_end = e; }
+  }
+  const bool mine = (keep >> lane) & 1u;
+  long long d = 0;
+  if (mine) {
+    w.sorted[s0 + __popc(keep & ((1u << lane) - 1u))] = v;
+    if (redact) d = splice_delta(w, category, v);
+  }
+  for (int k = 16; k; k >>= 1) d += __shfl_xor_sync(0xffffffffu, d, k);
+  *delta = d;
+  return __popc(keep);
+}
+
+// exclusive prefix sums of a[0, count) in place, one block (count <= blockDim.x, a in shared memory); part: 32 elements of
+// shared memory.  Call from block-uniform code.
+template <typename T>
+__device__ __forceinline__ void block_xscan_small(T* a, uint32_t count, T* part) {
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const T v = threadIdx.x < count ? a[threadIdx.x] : (T)0;
+  T incl = v;
+  for (int d = 1; d < 32; d <<= 1) { const T t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= (uint32_t)d) incl += t; }
+  if (lane == 31) part[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    const T wv = lane < blockDim.x / 32 ? part[lane] : (T)0;
+    T wi = wv;
+    for (int d = 1; d < 32; d <<= 1) { const T t = __shfl_up_sync(0xffffffffu, wi, d); if (lane >= (uint32_t)d) wi += t; }
+    part[lane] = wi - wv;
+  }
+  __syncthreads();
+  if (threadIdx.x < count) a[threadIdx.x] = part[warp] + incl - v;
+  __syncthreads();
+}
+
 // ---------------------------------------------------------------------------------------------- kernels
 __global__ void __launch_bounds__(256) span_count_kernel(ScanWork w) {
   const uint32_t ns = min(w.counters[kCtrRawSpans], w.span_cap);
@@ -224,27 +275,9 @@ __global__ void __launch_bounds__(kSortBlock) span_sort_keep_kernel(ScanWork w, 
     if (c > kWarpSort) continue;
     const uint32_t len = off[m + 1] - off[m];
     if (c == 0) { if (lane == 0) { w.kept_cnt[m] = 0; if (redact) w.out_len[m] = len; } continue; }
-    uint4 v = lane < c ? w.sorted[s0 + lane] : pad_key();
-    for (uint32_t k = 2; k <= 32; k <<= 1)
-      for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-        const uint4 o = shfl_key(v, j, true);
-        const bool keep_min = ((lane & j) == 0) == ((lane & k) == 0);
-        if (keep_min ? key_less(o, v) : key_less(v, o)) v = o;
-      }
-    long long last_end = -1;
-    uint32_t keep = 0;
-    for (uint32_t j = 0; j < c; j++) {
-      const uint32_t s = __shfl_sync(0xffffffffu, v.x, j), e = __shfl_sync(0xffffffffu, key_end(v), j);
-      if ((long long)s >= last_end) { keep |= 1u << j; last_end = e; }
-    }
-    const bool mine = (keep >> lane) & 1u;
     long long delta = 0;
-    if (mine) {
-      w.sorted[s0 + __popc(keep & ((1u << lane) - 1u))] = v;
-      if (redact) delta = splice_delta(w, category, v);
-    }
-    for (int d = 16; d; d >>= 1) delta += __shfl_xor_sync(0xffffffffu, delta, d);
-    if (lane == 0) { w.kept_cnt[m] = __popc(keep); if (redact) w.out_len[m] = (uint64_t)((long long)len + delta); }
+    const uint32_t kept = warp_sort_keep(w, category, s0, c, redact, &delta);
+    if (lane == 0) { w.kept_cnt[m] = kept; if (redact) w.out_len[m] = (uint64_t)((long long)len + delta); }
   }
 
   // long segments: one block each (block-uniform branches)
@@ -258,65 +291,100 @@ __global__ void __launch_bounds__(kSortBlock) span_sort_keep_kernel(ScanWork w, 
   }
 }
 
-// The whole resolver for a batch of one message (cg_find_matches_one / cg_redact_one), one block: every raw span belongs to
-// message 0, so the keys are built straight from w.spans (no count, scan or scatter), sorted and kept by sort_keep_segment,
-// and everything span_emit_kernel writes is written here for n = 1.  The span count is read from device memory only.
-__global__ void __launch_bounds__(kSortBlock) span_resolve_one_kernel(ScanWork w, const uint32_t* __restrict__ category,
+// The whole resolver for a batch of a few messages (n <= kFewMsgs: cg_find_matches_one / cg_redact_one and the _few calls),
+// one block, with the per-message arrays in shared memory: count per message -> exclusive scan -> scatter into message order
+// -> each segment sorted and kept (one warp per segment of at most kWarpSort keys, the whole block per longer one, through
+// warp_sort_keep / sort_keep_segment) -> exclusive scans of the kept counts and the output lengths -> everything
+// span_emit_kernel writes for n messages.  The span count is read from device memory only.
+__global__ void __launch_bounds__(kSortBlock) span_resolve_few_kernel(ScanWork w, const uint32_t* __restrict__ category,
                                                                       const uint32_t* __restrict__ rank, const uint32_t* __restrict__ off,
-                                                                      SpanOutputs o) {
+                                                                      uint32_t n, SpanOutputs o) {
+  __shared__ uint32_t seg[kFewMsgs + 1];         // raw spans per message, then the first of its segment
+  __shared__ uint32_t fill[kFewMsgs];            // keys scattered into each segment so far
+  __shared__ uint32_t kept[kFewMsgs + 1];        // spans kept per message, then its first resolved span
+  __shared__ unsigned long long olen[kFewMsgs + 1];   // redacted bytes per message, then its output offset
+  __shared__ unsigned long long part[32];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool incomplete = w.counters[kCtrErrors] != 0;
   const uint32_t c = incomplete ? 0u : min(w.counters[kCtrRawSpans], w.span_cap);
+  const int redact = o.redact ? 1 : 0;
+  for (uint32_t m = threadIdx.x; m <= n; m += blockDim.x) { seg[m] = 0; kept[m] = 0; olen[m] = 0; if (m < n) fill[m] = 0; }
+  __syncthreads();
+  for (uint32_t i = threadIdx.x; i < c; i += blockDim.x) atomicAdd(&seg[w.spans[(size_t)i * 6]], 1u);
+  __syncthreads();
+  block_xscan_small(seg, n + 1, reinterpret_cast<uint32_t*>(part));
   for (uint32_t i = threadIdx.x; i < c; i += blockDim.x) {
     const uint32_t* s = w.spans + (size_t)i * 6;
-    w.sorted[i] = make_uint4(s[4], ~(s[5] - s[4]), rank[s[1]], i);
+    const uint32_t m = s[0];
+    w.sorted[seg[m] + atomicAdd(&fill[m], 1u)] = make_uint4(s[4], ~(s[5] - s[4]), rank[s[1]], i);
   }
   __syncthreads();
-  long long delta = 0;
-  const uint32_t total = sort_keep_segment(w, category, 0, c, o.redact ? 1 : 0, &delta);
-  const uint64_t need = o.redact ? (uint64_t)((long long)(off[1] - off[0]) + delta) : 0;
+  for (uint32_t m = warp; m < n; m += blockDim.x / 32) {              // short segments: one warp each
+    const uint32_t s0 = seg[m], cm = seg[m + 1] - s0;
+    if (cm > kWarpSort) continue;
+    long long delta = 0;
+    const uint32_t k = cm ? warp_sort_keep(w, category, s0, cm, redact, &delta) : 0u;
+    if (lane == 0) { kept[m] = k; if (redact) olen[m] = (unsigned long long)((long long)(off[m + 1] - off[m]) + delta); }
+  }
+  __syncthreads();
+  for (uint32_t m = 0; m < n; m++) {                                   // long ones: the whole block each (block-uniform)
+    const uint32_t s0 = seg[m], cm = seg[m + 1] - s0;
+    if (cm <= kWarpSort) continue;
+    long long delta = 0;
+    const uint32_t k = sort_keep_segment(w, category, s0, cm, redact, &delta);
+    if (threadIdx.x == 0) { kept[m] = k; if (redact) olen[m] = (unsigned long long)((long long)(off[m + 1] - off[m]) + delta); }
+  }
+  __syncthreads();
+  block_xscan_small(kept, n + 1, reinterpret_cast<uint32_t*>(part));
+  if (redact) block_xscan_small(olen, n + 1, part);
+  const uint32_t total = kept[n];
+  const uint64_t need = redact ? olen[n] : 0;
   uint32_t status = kResolveOk;
   if (!incomplete) {
-    if (o.redact && (need >> 32)) status = kResolveTooLarge;
-    else if (total > o.spans_cap || (o.redact && need > o.out_cap)) status = kResolveCapacity;
+    if (redact && (need >> 32)) status = kResolveTooLarge;
+    else if (total > o.spans_cap || (redact && need > o.out_cap)) status = kResolveCapacity;
   }
   const bool go = !incomplete && status == kResolveOk;
   for (uint32_t r = threadIdx.x; r < total; r += blockDim.x) {
-    const uint4 k = w.sorted[r];
+    uint32_t lo = 0, hi = n;                                           // kept[lo] <= r < kept[hi]
+    while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (kept[mid] <= r) lo = mid; else hi = mid; }
+    const uint4 k = w.sorted[seg[lo] + (r - kept[lo])];
     const uint32_t* s = w.spans + (size_t)k.w * 6;
     const uint32_t rule = s[1], sb = s[2], eb = s[3];
     if (r < o.spans_cap) {
       uint32_t* d = o.spans + (size_t)r * 6;
-      d[0] = 0; d[1] = rule; d[2] = sb; d[3] = eb; d[4] = s[4]; d[5] = s[5];
+      d[0] = lo; d[1] = rule; d[2] = sb; d[3] = eb; d[4] = s[4]; d[5] = s[5];
     }
-    if (o.redact) { w.sp_start[r] = off[0] + sb; w.sp_len[r] = eb - sb; w.sp_cat[r] = category[rule]; }
+    if (redact) { w.sp_start[r] = off[lo] + sb; w.sp_len[r] = eb - sb; w.sp_cat[r] = category[rule]; }
+  }
+  for (uint32_t m = threadIdx.x; m <= n; m += blockDim.x) {
+    w.kept_begin[m] = kept[m];
+    if (redact) { w.out_off[m] = olen[m]; o.out_offsets[m] = (uint32_t)olen[m]; }
   }
   if (threadIdx.x == 0) {
-    w.kept_begin[0] = 0; w.kept_begin[1] = total;
-    if (o.redact) {
-      w.out_off[0] = 0; w.out_off[1] = need;
-      o.out_offsets[0] = 0; o.out_offsets[1] = (uint32_t)need;
-      uint64_t* z = reinterpret_cast<uint64_t*>(o.sizes); z[0] = incomplete ? ~0ull : need; z[1] = incomplete ? ~0ull : total;
-    } else *reinterpret_cast<uint32_t*>(o.sizes) = incomplete ? ~0u : total;
+    if (redact) { uint64_t* z = reinterpret_cast<uint64_t*>(o.sizes); z[0] = incomplete ? ~0ull : need; z[1] = incomplete ? ~0ull : total; }
+    else *reinterpret_cast<uint32_t*>(o.sizes) = incomplete ? ~0u : total;
     w.counters[kCtrResolveStatus] = status;
     w.counters[kCtrResolved] = incomplete ? 0u : total;
-    w.counters[kCtrDigests] = go && o.redact ? total : 0u;
-    w.counters[kCtrSplice] = go && o.redact ? 1u : 0u;
+    w.counters[kCtrDigests] = go && redact ? total : 0u;
+    w.counters[kCtrSplice] = go && redact ? n : 0u;
   }
 }
 
-// The one-message result made contiguous for one D2H copy (layout: kernels.h, launch_span_pack_one).  The spans and sizes
-// are already in place (the resolver wrote them there); this adds the status, the packed length, the counter block and,
-// redacting, the digests and the output bytes behind the spans -- when all of it fits in pack_cap bytes.
-__global__ void __launch_bounds__(512) span_pack_one_kernel(ScanWork w, const uint32_t* __restrict__ digests, const uint8_t* __restrict__ out,
-                                                            uint32_t* __restrict__ packed, uint32_t pack_cap, int redact) {
+// The few-message result made contiguous for one D2H copy (layout: kernels.h, launch_span_pack_few).  The spans, sizes and
+// output offsets are already in place (the resolver wrote them there); this adds the status, the packed length, the
+// counter block and, redacting, the digests and the output bytes behind the spans -- when all of it fits in pack_cap bytes.
+__global__ void __launch_bounds__(512) span_pack_few_kernel(ScanWork w, const uint32_t* __restrict__ digests, const uint8_t* __restrict__ out,
+                                                            uint32_t* __restrict__ packed, uint32_t pack_cap, uint32_t n, int redact) {
   const uint32_t flags = w.counters[kCtrErrors], status = w.counters[kCtrResolveStatus];
   uint32_t ns = 0; uint64_t need = 0;
   if (redact) { const uint64_t* z = reinterpret_cast<const uint64_t*>(packed + kPackSizes); need = z[0]; ns = (uint32_t)z[1]; }
   else ns = packed[kPackSizes];
-  const uint64_t len = (uint64_t)kPackHeader + (uint64_t)ns * 24 + (redact ? (uint64_t)ns * 32 + need : 0);
+  const uint32_t at = pack_spans_at(n);
+  const uint64_t len = (uint64_t)at + (uint64_t)ns * 24 + (redact ? (uint64_t)ns * 32 + need : 0);
   const bool fits = !flags && status == kResolveOk && len <= pack_cap;
   if (fits && redact) {
-    uint32_t* dd = packed + kPackHeader / 4 + (size_t)ns * 6;
+    uint32_t* dd = packed + at / 4 + (size_t)ns * 6;
     for (uint32_t i = threadIdx.x; i < ns * 8; i += blockDim.x) dd[i] = digests[i];
     uint8_t* ob = reinterpret_cast<uint8_t*>(dd + (size_t)ns * 8);
     for (uint32_t i = threadIdx.x; i < need; i += blockDim.x) ob[i] = out[i];
@@ -387,14 +455,14 @@ int launch_span_resolve(const ScanWork& w, const uint32_t* d_off, uint32_t n, co
   return k;
 }
 
-int launch_span_resolve_one(const ScanWork& w, const uint32_t* d_off, const SpanOutputs& o, cudaStream_t stream) {
-  span_resolve_one_kernel<<<1, kSortBlock, 0, stream>>>(w, w.rule_category, w.rule_rank, d_off, o);
+int launch_span_resolve_few(const ScanWork& w, const uint32_t* d_off, uint32_t n, const SpanOutputs& o, cudaStream_t stream) {
+  span_resolve_few_kernel<<<1, kSortBlock, 0, stream>>>(w, w.rule_category, w.rule_rank, d_off, n, o);
   return 1;
 }
 
-int launch_span_pack_one(const ScanWork& w, const uint32_t* d_digests, const uint8_t* d_out, uint32_t* d_packed, uint32_t pack_cap, bool redact,
-                         cudaStream_t stream) {
-  span_pack_one_kernel<<<1, 512, 0, stream>>>(w, d_digests, d_out, d_packed, pack_cap, redact ? 1 : 0);
+int launch_span_pack_few(const ScanWork& w, const uint32_t* d_digests, const uint8_t* d_out, uint32_t* d_packed, uint32_t pack_cap, uint32_t n,
+                         bool redact, cudaStream_t stream) {
+  span_pack_few_kernel<<<1, 512, 0, stream>>>(w, d_digests, d_out, d_packed, pack_cap, n, redact ? 1 : 0);
   return 1;
 }
 

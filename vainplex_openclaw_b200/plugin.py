@@ -6,7 +6,8 @@ TypeScript equivalent a maintainer would ship is sketched in INTEGRATION.md).  E
 matches or hashes goes through the C ABI (include/openclaw_gov.h) to the CUDA kernels; this file
 only holds the host logic the reference also keeps on the host:
 
-  PatternRegistry    gov/src/redaction/registry.ts:165-316   (findMatches -> cg_find_matches_one / cg_redact_one)
+  PatternRegistry    gov/src/redaction/registry.ts:165-316   (findMatches -> cg_find_matches_one / cg_redact_one, and
+                     for the strings of one scanned value cg_find_matches_few / cg_redact_few)
   RedactionVault     gov/src/redaction/vault.ts:39-258        (sha256 -> cg_sha256_batch)
   RedactionEngine    gov/src/redaction/engine.ts:38-191
   evaluate_allowlist gov/src/redaction/allowlist.ts:35-85
@@ -111,13 +112,18 @@ class PatternRegistry:
             out[int(sp["msg"])].append({"pattern": self.patterns[int(sp["rule"])], "match": _slice16(s, a, b), "start": a, "end": b})
         return out
 
-    def find_matches(self, input: str, redact: bool = False) -> "Matches":
+    def find_matches(self, input, redact: bool = False):
         """findMatches for one string: one blocking device call.  The result is the list findMatches returns.
 
         redact=False: cg_find_matches_one.  redact=True (RedactionEngine's scanString path): cg_redact_one, which finds the
         same matches and also splices the default placeholders and hashes every match on the device; the result then carries
         that in .redacted (see Matches).  Both go through this method so that a failing device call surfaces here, where
-        the reference's engine calls findMatches."""
+        the reference's engine calls findMatches.
+
+        input may also be a list of strings (the string leaves of one value RedactionEngine.scan walks): one Matches per
+        string, from one blocking device call (cg_find_matches_few / cg_redact_few)."""
+        if not isinstance(input, str):
+            return self._find_matches_few(list(input), redact)
         rs = self._rs()
         if rs is None:
             return Matches()
@@ -132,6 +138,29 @@ class PatternRegistry:
             a, b = int(sp["start16"]), int(sp["end16"])
             out.append({"pattern": self.patterns[int(sp["rule"])], "match": _slice16(input, a, b), "start": a, "end": b})
         return out
+
+
+    def _find_matches_few(self, inputs: List[str], redact: bool) -> List["Matches"]:
+        rs = self._rs()
+        if rs is None or not inputs:
+            return [Matches() for _ in inputs]
+        enc = [N.js_utf8(s) for s in inputs]
+        data, off = N.pack(enc)
+        if redact:
+            out_bytes, out_off, spans, digests = rs.redact_few(data, off)
+        else:
+            spans = rs.find_matches_few(data, off)
+        first = np.searchsorted(spans["msg"], np.arange(len(inputs) + 1))      # (spans come sorted by (msg, start))
+        res = []
+        for m, s in enumerate(inputs):
+            a, b = int(first[m]), int(first[m + 1])
+            redacted = RedactedString(enc[m], bytes(out_bytes[int(out_off[m]):int(out_off[m + 1])]), spans[a:b], digests[a:b]) if redact else None
+            out = Matches(redacted=redacted)
+            for sp in spans[a:b]:
+                x, y = int(sp["start16"]), int(sp["end16"])
+                out.append({"pattern": self.patterns[int(sp["rule"])], "match": _slice16(s, x, y), "start": x, "end": y})
+            res.append(out)
+        return res
 
 
 class RedactedString(NamedTuple):
@@ -279,35 +308,71 @@ class RedactionEngine:
         return {"output": out, "redactionCount": count[0], "categories": cats}
 
     def scan(self, input: Any):
+        """scan / scanValue / scanStringValue (engine.ts:53-147) in three passes: the walk records, in walk order, every string
+        that scanStringValue would redact and a skeleton of the value; one device call (registry.find_matches on the list,
+        cg_redact_few) finds, hashes and splices all of them; the replay stores the matches in the vault string by string in
+        walk order (right to left inside each string, as applyReplacements does) and rebuilds the value.  Output, counts,
+        categories and the vault equal a walk that redacts leaf by leaf.  A value without strings makes no device call; when
+        the call fails nothing reaches the vault."""
         t0 = time.perf_counter()
         cats, count = set(), [0]
-        out = self._scan_value(input, set(), 0, cats, count)
+        leaves: List[str] = []
+        skeleton = self._walk(input, set(), 0, leaves, [])
+        found = self.registry.find_matches(leaves, redact=True) if leaves else []
+        done = []
+        for s, matches in zip(leaves, found):
+            if not matches:
+                done.append(s)
+                continue
+            r = matches.redacted
+            counter = {"redactionCount": 0}
+            done.append(self._store_and_splice(s, r.enc, r.out, r.spans, r.digests, cats, counter))
+            count[0] += counter["redactionCount"]
+        out = self._rebuild(skeleton, done)
         return {"output": out, "redactionCount": count[0], "categories": cats, "elapsedMs": (time.perf_counter() - t0) * 1e3}
 
-    def _scan_value(self, value, seen, depth, cats, count):
+    # skeleton nodes: (_LEAF, i) the i-th recorded string; (_JSON, node) a string that held JSON, dumped again; (_LIST,
+    # [nodes]); (_DICT, [(key, node)]); (_KEEP, value) a value returned as it is
+    _LEAF, _JSON, _LIST, _DICT, _KEEP = range(5)
+
+    def _walk(self, value, seen, depth, leaves: List[str], keep: list):
+        """scanValue's walk (engine.ts:94-126) without the redaction: the same depth limit, the same seen rule (a second
+        reference to an object becomes "[Circular]") and the same JSON-in-string parse.  keep holds the parsed values, so
+        that no id in seen is reused while the walk runs."""
         if depth > MAX_DEPTH or value is None:
-            return value
+            return (self._KEEP, value)
         if isinstance(value, str):
-            return self._scan_string_value(value, seen, depth, cats, count)
+            t = value.lstrip()
+            if _js_len(value) <= MAX_JSON_PARSE_LENGTH and (t.startswith("{") or t.startswith("[")):
+                try:
+                    parsed = json.loads(value)
+                    if isinstance(parsed, (dict, list)):
+                        keep.append(parsed)
+                        return (self._JSON, self._walk(parsed, seen, depth + 1, leaves, keep))
+                except ValueError:
+                    pass
+            leaves.append(value)
+            return (self._LEAF, len(leaves) - 1)
         if isinstance(value, (list, dict)):
             if id(value) in seen:
-                return "[Circular]"
+                return (self._KEEP, "[Circular]")
             seen.add(id(value))
             if isinstance(value, list):
-                return [self._scan_value(v, seen, depth + 1, cats, count) for v in value]
-            return {k: self._scan_value(v, seen, depth + 1, cats, count) for k, v in value.items()}
-        return value
+                return (self._LIST, [self._walk(v, seen, depth + 1, leaves, keep) for v in value])
+            return (self._DICT, [(k, self._walk(v, seen, depth + 1, leaves, keep)) for k, v in value.items()])
+        return (self._KEEP, value)
 
-    def _scan_string_value(self, value: str, seen, depth, cats, count):
-        t = value.lstrip()
-        if _js_len(value) <= MAX_JSON_PARSE_LENGTH and (t.startswith("{") or t.startswith("[")):
-            try:
-                parsed = json.loads(value)
-                if isinstance(parsed, (dict, list)):
-                    return json.dumps(self._scan_value(parsed, seen, depth + 1, cats, count), separators=(",", ":"), ensure_ascii=False)
-            except ValueError:
-                pass
-        return self._redact_string(value, cats, count)
+    def _rebuild(self, node, done: List[str]):
+        kind, x = node
+        if kind == self._LEAF:
+            return done[x]
+        if kind == self._JSON:
+            return json.dumps(self._rebuild(x, done), separators=(",", ":"), ensure_ascii=False)
+        if kind == self._LIST:
+            return [self._rebuild(v, done) for v in x]
+        if kind == self._DICT:
+            return {k: self._rebuild(v, done) for k, v in x}
+        return x
 
     def scan_strings(self, inputs: Sequence[str], credential_only: Optional[Sequence[bool]] = None) -> List[dict]:
         """scanString (engine.ts:74-85) for many strings with the splice done on the device (cg_redact_batch): matches,
