@@ -10,6 +10,7 @@
 #include <dlfcn.h>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/openclaw_gov.h"
@@ -124,6 +125,56 @@ int grow_bytes(size_t need) {
   return CG_OK;
 }
 
+// The single-message staging block, host (pinned) and device: [offsets, 256 B][message bytes][64 zero bytes] in (kOneIn),
+// [word][counters][hit row] out (kOneOut).  The span calls stage their input in their own block (kFew*) and keep the packed
+// result (kOnePack bytes, layout in kernels.h) on both sides and, on the device only, the digests and the redacted bytes
+// before the pack step moves them behind the spans (kOnePack each).
+constexpr uint32_t kOneBytes = 16384, kOneRw = 128, kOneIn = 256 + kOneBytes + 64, kOneOut = (kOneHitRow + kOneRw) * 4;
+constexpr uint32_t kOnePack = 512 * 1024;
+// The span calls' staging block, host (pinned) and device: [offsets, kFewMsgs + 1][text bytes, kFewBytes][64 zero bytes],
+// the offsets rebased to kFewTextAt.  The limits: 256 strings (kFewMsgs: the resolver keeps its per-message arrays in shared
+// memory) and 64 KB of text (cg_policy_eval_one's limit); the _one calls keep 16 KB (kOneBytes).
+constexpr uint32_t kFewBytes = 65536, kFewTextAt = 1280, kFewIn = kFewTextAt + kFewBytes + 64;
+static_assert(4 * (kFewMsgs + 1) <= kFewTextAt && kFewTextAt % 256 == 0 && pack_spans_at(kFewMsgs) < 4096, "span call staging layout");
+// cg_policy_eval_one's staging block, host (pinned) and device: in, [offsets, kPeOneTexts + 1][roles][atom row, kPeOneAtomWords]
+// [text bytes, kPeOneBytes][64 zero bytes] at fixed places (offsets are rebased to kPeTextAt); out, kPeOneRules + kPeOneRulesCap
+// words (kernels.h).  The limits: 64 texts (kPeOneTexts: the kernel keeps the text list in shared memory), 64 KB of text (a tool
+// call's params or a message with its conversation history), 32 768 atoms, 4096 matched policies.
+constexpr uint32_t kPeOneBytes = 65536, kPeOneAtomWords = 1024, kPeOneRulesCap = 4096;
+constexpr uint32_t kPeRolesAt = 512, kPeAtomsAt = kPeRolesAt + 256, kPeTextAt = kPeAtomsAt + 4 * kPeOneAtomWords;
+constexpr uint32_t kPeIn = kPeTextAt + kPeOneBytes + 64, kPeOut = 4 * (kPeOneRules + kPeOneRulesCap);
+static_assert(4 * (kPeOneTexts + 1) <= kPeRolesAt && kPeOneTexts <= 256 && kPeTextAt % 256 == 0, "cg_policy_eval_one staging layout");
+
+// A blocking call family's pinned host block and device block, of sizes fixed by the family's layout, allocated and zeroed
+// by the family's first call
+struct Staging {
+  const size_t host_bytes, dev_bytes;
+  uint8_t* h = nullptr; uint8_t* d = nullptr;
+  Staging(size_t host, size_t dev) : host_bytes(host), dev_bytes(dev) {}
+  Staging(const Staging&) = delete;
+  Staging& operator=(const Staging&) = delete;
+  ~Staging() { if (h) cudaFreeHost(h); cudaFree(d); }
+  int ensure() {
+    if (!h) { CU(cudaMallocHost((void**)&h, host_bytes)); memset(h, 0, host_bytes); }
+    if (!d) { CU(cudaMalloc((void**)&d, dev_bytes)); CU(cudaMemset(d, 0, dev_bytes)); }
+    return CG_OK;
+  }
+};
+
+// A call family's step graphs (cached_graph): Cap instances at most, each replayed only for the key it was recorded with
+// (the family's launch arguments that are not staged data) and under the scratch generation and verify grid current then
+// (a graph holds the scratch pointers, the rule set's device tables and verify_small_kernel's grid by value)
+template <typename Key, int Cap>
+struct GraphCache {
+  struct Entry { cudaGraphExec_t exec = nullptr; int kernels = 0; uint64_t used = 0, gen = 0; int ctas = 0; Key key{}; };
+  Entry e[Cap];
+  uint64_t clock = 0;
+  GraphCache() = default;
+  GraphCache(const GraphCache&) = delete;
+  GraphCache& operator=(const GraphCache&) = delete;
+  ~GraphCache() { for (auto& g : e) if (g.exec) cudaGraphExecDestroy(g.exec); }
+};
+
 }  // namespace
 
 struct cg_ruleset {
@@ -148,47 +199,25 @@ struct cg_ruleset {
   void size_verify_grid() { const uint32_t ev = last_counters[kCtrEvents]; if (ev > 2048u) verify_ctas = 4; else if (ev < 256u) verify_ctas = 1; }
   uint32_t last_counters[kCounterWords] = {};
   uint64_t scratch_gen = 0;       // advanced by every change to what a captured step holds (scratch buffers, DevRuleset)
-  // the device-resident step replayed as one CUDA graph (keyed on its arguments, the scratch generation and the verify grid)
-  struct CachedGraph { int kernels = 0; cudaGraphExec_t exec = nullptr; const void* bytes = nullptr; const void* off = nullptr; void* words = nullptr; uint32_t n = 0; uint64_t gen = 0; int ctas = 0; uint64_t used = 0; };
-  // cg_scan_one: pinned staging + one device block ([offsets][message bytes] in, [word][counters][hit row] out) and the step
-  // as a graph over those fixed addresses (the message length is data, so one graph serves every message); for the span
-  // calls a second pair (the packed result, and on the device its scratch; capi.cu kOne*)
-  struct OneGraph { cudaGraphExec_t exec = nullptr; uint64_t gen = 0; int ctas = 0; int kernels = 0; };
-  struct OnePath { OneGraph g; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint8_t* h_pack = nullptr; uint8_t* d_pack = nullptr; } one;
-  // cg_find_matches_one / cg_redact_one / cg_find_matches_few / cg_redact_few: pinned staging + one device block ([offsets]
-  // [text bytes] in, capi.cu kFew*), and the step + resolver (+ digests and splice) + pack as graphs over those fixed
-  // addresses and one.d_pack, one per (mode, message count) (the step takes the count by value), the least recently used
-  // of kSpanGraphs re-targeted
-  static constexpr int kSpanGraphs = 16;
-  struct SpanGraph { cudaGraphExec_t exec = nullptr; uint32_t n = 0; bool redact = false; uint64_t gen = 0, used = 0; int ctas = 0, kernels = 0; };
-  struct SpanFew { SpanGraph g[kSpanGraphs]; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint64_t clock = 0; } few;
-  CachedGraph graphs[2];          // two entries: callers that alternate between two input/output buffer sets replay, never re-capture
-  uint64_t graph_clock = 0;
+  // cg_scan_batch_device's step as one CUDA graph, keyed on (d_bytes, d_offsets, d_words, n): two entries, so that callers
+  // that alternate between two input/output buffer sets replay, never re-capture
+  GraphCache<std::tuple<const void*, const void*, const void*, uint32_t>, 2> device_graphs;
+  // The blocking calls (blocking_call), each family with its staging and its graphs over the staging's fixed addresses.
+  // cg_scan_one: the message length is data, so one graph serves every message.
+  struct { Staging io{kOneIn + kOneOut, kOneIn + kOneOut}; GraphCache<std::tuple<>, 1> graphs; } one;
+  // cg_find_matches_one / cg_redact_one / cg_find_matches_few / cg_redact_few: the input block and the packed result, and
+  // the step + resolver (+ digests and splice) + pack per (redact, string count) (the step takes the count by value)
+  struct { Staging in{kFewIn, kFewIn}, pack{kOnePack, 3 * (size_t)kOnePack}; GraphCache<std::tuple<bool, uint32_t>, 16> graphs; } span;
+  // cg_policy_eval_one: the step + policy_eval_one_kernel per (text count, prog_gen) (a graph holds PolicyTable by value)
+  struct { Staging io{kPeIn + kPeOut, kPeIn + kPeOut}; GraphCache<std::tuple<uint32_t, uint64_t>, 8> graphs; } pone;
   // cg_ruleset_set_views: n_views rows of dev.rw words in HBM (bit r of row v = rule r is in view v); none before the first call
   uint32_t* view_rows = nullptr; uint32_t n_views = 0;
   // cg_ruleset_set_policy_program: the program's words and one rule record per program rule (kernels.h PolicyTable) in HBM;
   // prog_gen advances with every program set (a captured graph holds the tables by value)
   uint32_t* prog_ops = nullptr; uint4* prog_rules = nullptr; uint32_t prog_n_rules = 0, prog_n_atoms = 0;
   uint64_t prog_gen = 0;
-  // cg_policy_eval_one: pinned staging + one device block (capi.cu kPe*: [offsets][roles][atom row][text bytes] in,
-  // [verdict][count][counters][rules] out), and the step + policy_eval_one_kernel as graphs over those fixed addresses, one per
-  // text count (the step takes it by value), the least recently used of kPeGraphs replaced
-  static constexpr int kPeGraphs = 8;
-  struct PeGraph { cudaGraphExec_t exec = nullptr; uint32_t n = 0; uint64_t gen = 0, prog = 0, used = 0; int ctas = 0, kernels = 0; };
-  struct PolicyOne { PeGraph g[kPeGraphs]; uint8_t* h_pin = nullptr; uint8_t* d_buf = nullptr; uint64_t clock = 0; } pone;
-  ~cg_ruleset() {
+  ~cg_ruleset() {                 // (the graph caches and staging blocks release themselves)
     cudaFree(view_rows); cudaFree(prog_ops); cudaFree(prog_rules);
-    for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    if (one.g.exec) cudaGraphExecDestroy(one.g.exec);
-    for (auto& g : few.g) if (g.exec) cudaGraphExecDestroy(g.exec);
-    if (few.h_pin) cudaFreeHost(few.h_pin);
-    cudaFree(few.d_buf);
-    for (auto& g : pone.g) if (g.exec) cudaGraphExecDestroy(g.exec);
-    if (pone.h_pin) cudaFreeHost(pone.h_pin);
-    cudaFree(pone.d_buf);
-    if (one.h_pin) cudaFreeHost(one.h_pin);
-    if (one.h_pack) cudaFreeHost(one.h_pack);
-    cudaFree(one.d_buf); cudaFree(one.d_pack);
     if (h_counters) cudaFreeHost(h_counters);
     for (auto& e : e_cnt) if (e) cudaEventDestroy(e);
     if (order.ev) cudaEventDestroy(order.ev);
@@ -358,14 +387,31 @@ int record(cudaStream_t st, Enqueue&& enqueue, cudaGraph_t* graph, int* kernels)
   *graph = g;
   return CG_OK;
 }
-// the same, instantiated
-template <typename Enqueue>
-int capture(cudaStream_t st, Enqueue&& enqueue, cudaGraphExec_t* exec, int* kernels) {
-  cudaGraph_t g = nullptr;
-  if (int rc = record(st, enqueue, &g, kernels)) return rc;
-  const cudaError_t e = cudaGraphInstantiate(exec, g, 0);
-  cudaGraphDestroy(g);
-  if (e != cudaSuccess) { *exec = nullptr; return cuda_fail(e, "cudaGraphInstantiate"); }
+// *out = the cache's graph of key for the current scratch and verify grid.  On a miss enqueue() is recorded afresh on st
+// into the least recently used entry, whose instance is re-targeted (cudaGraphExecUpdate: where the launch sequence is the
+// same, only parameters change) and instantiated anew only when the update is refused.
+template <typename Key, int Cap, typename Enqueue>
+int cached_graph(cg_ruleset* rs, GraphCache<Key, Cap>& c, const Key& key, cudaStream_t st, Enqueue&& enqueue, typename GraphCache<Key, Cap>::Entry** out) {
+  typename GraphCache<Key, Cap>::Entry* g = nullptr;
+  for (auto& e : c.e) if (e.exec && e.key == key && e.gen == rs->scratch_gen && e.ctas == rs->verify_ctas) g = &e;
+  if (!g) {
+    g = &c.e[0];
+    for (auto& e : c.e) if (e.used < g->used) g = &e;
+    cudaGraph_t graph = nullptr;
+    int kernels = 0;
+    if (int rc = record(st, enqueue, &graph, &kernels)) return rc;
+    cudaGraphExecUpdateResultInfo info;
+    if (!g->exec || cudaGraphExecUpdate(g->exec, graph, &info) != cudaSuccess) {
+      cudaGetLastError();                                     // (a refused update is not an error of the call)
+      if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; }
+      const cudaError_t e = cudaGraphInstantiate(&g->exec, graph, 0);
+      if (e != cudaSuccess) { cudaGraphDestroy(graph); g->exec = nullptr; return cuda_fail(e, "cudaGraphInstantiate"); }
+    }
+    cudaGraphDestroy(graph);
+    g->key = key; g->gen = rs->scratch_gen; g->ctas = rs->verify_ctas; g->kernels = kernels;
+  }
+  g->used = ++c.clock;
+  *out = g;
   return CG_OK;
 }
 // the rules of one hit row (rw words), lowest first: put(i, rule) for the i-th rule of the output while i < cap; returns nh
@@ -521,67 +567,49 @@ int mirror_counters(cg_ruleset* rs, cudaStream_t st) {
   return CG_OK;
 }
 
-// The single-message staging block, host (pinned) and device: [offsets, 256 B][message bytes][64 zero bytes] in (kOneIn),
-// [word][counters][hit row] out (kOneOut).  The span calls stage their input in their own block (kFew*) and add, on their
-// first use, the packed result (kOnePack bytes, layout in kernels.h) on both sides and, on the device only, the digests and
-// the redacted bytes before the pack step moves them behind the spans (kOnePack each).
-constexpr uint32_t kOneBytes = 16384, kOneRw = 128, kOneIn = 256 + kOneBytes + 64, kOneOut = (kOneHitRow + kOneRw) * 4;
-constexpr uint32_t kOnePack = 512 * 1024;
-// The span calls' staging block, host (pinned) and device: [offsets, kFewMsgs + 1][text bytes, kFewBytes][64 zero bytes],
-// the offsets rebased to kFewTextAt.  The limits: 256 strings (kFewMsgs: the resolver keeps its per-message arrays in shared
-// memory) and 64 KB of text (cg_policy_eval_one's limit); the _one calls keep 16 KB (kOneBytes).
-constexpr uint32_t kFewBytes = 65536, kFewTextAt = 1280, kFewIn = kFewTextAt + kFewBytes + 64;
-static_assert(4 * (kFewMsgs + 1) <= kFewTextAt && kFewTextAt % 256 == 0 && pack_spans_at(kFewMsgs) < 4096, "span call staging layout");
-
-int one_staging(cg_ruleset::OnePath& o) {
-  if (!o.h_pin) { CU(cudaMallocHost((void**)&o.h_pin, kOneIn + kOneOut)); memset(o.h_pin, 0, kOneIn + kOneOut); }
-  if (!o.d_buf) { CU(cudaMalloc((void**)&o.d_buf, kOneIn + kOneOut)); CU(cudaMemset(o.d_buf, 0, kOneIn + kOneOut)); }
-  return CG_OK;
-}
-// the span calls' staging block, packed result and scratch
-int few_staging(cg_ruleset* rs) {
-  cg_ruleset::SpanFew& f = rs->few; cg_ruleset::OnePath& o = rs->one;
-  if (!f.h_pin) { CU(cudaMallocHost((void**)&f.h_pin, kFewIn)); memset(f.h_pin, 0, kFewIn); }
-  if (!f.d_buf) { CU(cudaMalloc((void**)&f.d_buf, kFewIn)); CU(cudaMemset(f.d_buf, 0, kFewIn)); }
-  if (!o.h_pack) { CU(cudaMallocHost((void**)&o.h_pack, kOnePack)); memset(o.h_pack, 0, kOnePack); }
-  if (!o.d_pack) { CU(cudaMalloc((void**)&o.d_pack, 3 * (size_t)kOnePack)); CU(cudaMemset(o.d_pack, 0, 3 * (size_t)kOnePack)); }
-  return CG_OK;
-}
-// cg_scan_one's graph, captured again when the scratch or the verify grid changed since it was captured
-template <typename Enqueue>
-int one_graph(cg_ruleset* rs, Enqueue&& enqueue) {
-  cg_ruleset::OneGraph& g = rs->one.g;
-  if (g.exec && g.gen == rs->scratch_gen && g.ctas == rs->verify_ctas) return CG_OK;
-  if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
-  if (int rc = capture(G.stream, enqueue, &g.exec, &g.kernels)) return rc;
-  g.gen = rs->scratch_gen; g.ctas = rs->verify_ctas;
-  return CG_OK;
-}
-// the message into the staging block (offsets {256, 256 + len}) and one H2D copy
-int stage_one(cg_ruleset::OnePath& o, const uint8_t* bytes, uint32_t len, cudaStream_t st) {
-  uint32_t* hoff = reinterpret_cast<uint32_t*>(o.h_pin); hoff[0] = 256; hoff[1] = 256 + len;
-  if (len) memcpy(o.h_pin + 256, bytes, len);
-  memset(o.h_pin + 256 + len, 0, 64);
-  CU(cudaMemcpyAsync(o.d_buf, o.h_pin, 256 + (size_t)len + 64, cudaMemcpyHostToDevice, st));
-  return CG_OK;
+// n + 1 offsets rebased to text_at, the n strings' bytes from there on and 64 zero bytes behind them into a staging block's
+// host side -> the bytes of it to copy to the device
+size_t stage_texts(uint8_t* h, uint32_t text_at, const uint8_t* bytes, const uint32_t* offsets, uint32_t n) {
+  const uint32_t first = n ? offsets[0] : 0, len = n ? offsets[n] - first : 0;
+  uint32_t* hoff = reinterpret_cast<uint32_t*>(h);
+  for (uint32_t i = 0; i <= n; i++) hoff[i] = text_at + (n ? offsets[i] - first : 0);
+  if (len) memcpy(h + text_at, bytes + first, len);
+  memset(h + text_at + len, 0, 64);
+  return (size_t)text_at + len + 64;
 }
 
-// cg_scan_batch_device's step as a CUDA graph: captured once per (arguments, scratch generation, verify grid) into the
-// least recently used of two entries, then replayed -- one launch per step instead of six, so the host never becomes the
-// bottleneck
+// The blocking calls' driver, one device round trip on the library's stream: the rule set's turn, the family's staging,
+// the scratch of a `kind` step over n items (res_min: as prepare_step), the graph of key from the family's cache (enqueue:
+// the step over the staged input and the family's kernels behind it, recorded on a miss), the first stage(in.h) bytes of
+// `in` to the device, one graph launch, `bytes` bytes at `at` of `out` back to its host side, one synchronise.  -> CG_OK,
+// an error, or 1 = a queue overflowed (counter block at byte `counters` of out.h; the capacities have been learnt): take
+// the batch call.
+template <typename Key, int Cap, typename Stage, typename Enqueue>
+int blocking_call(cg_ruleset* rs, StepKind kind, uint32_t n, uint32_t res_min, GraphCache<Key, Cap>& cache, const Key& key, Staging& in, Stage&& stage,
+                  Enqueue&& enqueue, Staging& out, size_t at, size_t bytes, size_t counters) {
+  cudaStream_t st = G.stream;
+  InOrder turn(&rs->order, st);
+  int rc;
+  if ((rc = turn.rc) || (rc = in.ensure()) || (rc = out.ensure())) return rc;
+  if ((rc = prepare_step(rs, n, kind, st, res_min))) return rc;
+  typename GraphCache<Key, Cap>::Entry* g = nullptr;
+  if ((rc = cached_graph(rs, cache, key, st, enqueue, &g))) return rc;
+  CU(cudaMemcpyAsync(in.d, in.h, stage(in.h), cudaMemcpyHostToDevice, st));
+  CU(cudaGraphLaunch(g->exec, st));
+  CU(cudaMemcpyAsync(out.h + at, out.d + at, bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  count_launches(g->kernels);
+  return absorb_counters(rs, reinterpret_cast<const uint32_t*>(out.h + counters));
+}
+
+// cg_scan_batch_device's step replayed as one CUDA graph -- one launch per step instead of six, so the host never becomes
+// the bottleneck
 template <typename Step>
 int replay_step(cg_ruleset* rs, const void* d_bytes, const void* d_offsets, uint32_t n, void* d_words, cudaStream_t st, Step&& step) {
-  cg_ruleset::CachedGraph* hit = nullptr;
-  for (auto& g : rs->graphs) if (g.exec && g.bytes == d_bytes && g.off == d_offsets && g.words == d_words && g.n == n && g.gen == rs->scratch_gen && g.ctas == rs->verify_ctas) hit = &g;
-  if (!hit) {
-    hit = rs->graphs[0].used <= rs->graphs[1].used ? &rs->graphs[0] : &rs->graphs[1];
-    if (hit->exec) { cudaGraphExecDestroy(hit->exec); hit->exec = nullptr; }
-    if (int rc = capture(st, step, &hit->exec, &hit->kernels)) return rc;
-    hit->bytes = d_bytes; hit->off = d_offsets; hit->words = d_words; hit->n = n; hit->gen = rs->scratch_gen; hit->ctas = rs->verify_ctas;
-  }
-  hit->used = ++rs->graph_clock;
-  CU(cudaGraphLaunch(hit->exec, st));
-  count_launches(hit->kernels);
+  decltype(rs->device_graphs)::Entry* g = nullptr;
+  if (int rc = cached_graph(rs, rs->device_graphs, {d_bytes, d_offsets, d_words, n}, st, step, &g)) return rc;
+  CU(cudaGraphLaunch(g->exec, st));
+  count_launches(g->kernels);
   return CG_OK;
 }
 
@@ -624,35 +652,6 @@ int enqueue_redact_tail(const ScanWork& w, const uint8_t* d_bytes, const uint32_
   const int k = launch_redact_digests(d_bytes, w.sp_start, w.sp_len, w.counters + kCtrDigests, d_digests, G.sm_count, st);
   return k + launch_redact_splice(d_bytes, d_off, d_out_offsets, w.kept_begin, w.sp_start, w.sp_len, w.sp_cat, d_digests, d_out,
                                   w.counters + kCtrSplice, n, G.sm_count, st);
-}
-
-// the span graph of (mode, n), captured when the cache has none for the current scratch and verify grid: recorded afresh and
-// put into the least recently used entry, whose instance is re-targeted (cudaGraphExecUpdate: the launch sequence does not
-// depend on n, so only parameters change) and instantiated anew only when the update is refused
-template <typename Enqueue>
-int few_graph(cg_ruleset* rs, uint32_t n, bool redact, Enqueue&& enqueue, cg_ruleset::SpanGraph** out) {
-  cg_ruleset::SpanFew& f = rs->few;
-  cg_ruleset::SpanGraph* g = nullptr;
-  for (auto& e : f.g) if (e.exec && e.n == n && e.redact == redact && e.gen == rs->scratch_gen && e.ctas == rs->verify_ctas) g = &e;
-  if (!g) {
-    g = &f.g[0];
-    for (auto& e : f.g) if (e.used < g->used) g = &e;
-    cudaGraph_t graph = nullptr;
-    int kernels = 0;
-    if (int rc = record(G.stream, enqueue, &graph, &kernels)) return rc;
-    cudaGraphExecUpdateResultInfo info;
-    if (!g->exec || cudaGraphExecUpdate(g->exec, graph, &info) != cudaSuccess) {
-      cudaGetLastError();                                     // (a refused update is not an error of the call)
-      if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; }
-      const cudaError_t e = cudaGraphInstantiate(&g->exec, graph, 0);
-      if (e != cudaSuccess) { cudaGraphDestroy(graph); g->exec = nullptr; return cuda_fail(e, "cudaGraphInstantiate"); }
-    }
-    cudaGraphDestroy(graph);
-    g->n = n; g->redact = redact; g->gen = rs->scratch_gen; g->ctas = rs->verify_ctas; g->kernels = kernels;
-  }
-  g->used = ++f.clock;
-  *out = g;
-  return CG_OK;
 }
 
 }  // namespace
@@ -940,28 +939,18 @@ namespace {
 int scan_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* out_word, uint32_t* out_rules, uint32_t rules_cap, uint32_t* out_nrules) {
   static const bool off_ = getenv("CG_ONE_FAST") && atoi(getenv("CG_ONE_FAST")) == 0;
   if (off_ || !G.ready || !rs || (len && !bytes) || len > kOneBytes || rs->dev.rw > kOneRw - 2 || G.profiling) return 1;
-  cg_ruleset::OnePath& o = rs->one;
-  cudaStream_t st = G.stream;
-  InOrder turn(&rs->order, st);
-  int rc;
-  if ((rc = turn.rc)) return rc;
-  if ((rc = one_staging(o))) return rc;
-  if ((rc = prepare_step(rs, 1, kStepWords, st))) return rc;
-  const uint8_t* d_bytes = o.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(o.d_buf);
-  uint32_t* d_out = reinterpret_cast<uint32_t*>(o.d_buf + kOneIn); uint64_t* d_word = reinterpret_cast<uint64_t*>(o.d_buf + kOneIn + kOneOut - 8);   // (the word lands behind the hit row, then is packed to the front)
-  if ((rc = one_graph(rs, [&] {
-        const int r = run_scan_device(rs, d_bytes, d_off, 1, d_word, kStepWords, st);
-        if (r == CG_OK) count_launches(launch_pack_one(rs->dev, rs->work, d_word, d_out, kOneRw - 2, st));
+  Staging& s = rs->one.io;
+  const uint32_t off[2] = {0, len};
+  const int rc = blocking_call(rs, kStepWords, 1, 0, rs->one.graphs, {}, s, [&](uint8_t* h) { return stage_texts(h, 256, bytes, off, 1); }, [&] {
+        const uint32_t* d_off = reinterpret_cast<const uint32_t*>(s.d);
+        uint32_t* d_out = reinterpret_cast<uint32_t*>(s.d + kOneIn); uint64_t* d_word = reinterpret_cast<uint64_t*>(s.d + kOneIn + kOneOut - 8);   // (the word lands behind the hit row, then is packed to the front)
+        const int r = run_scan_device(rs, s.d, d_off, 1, d_word, kStepWords, G.stream);
+        if (r == CG_OK) count_launches(launch_pack_one(rs->dev, rs->work, d_word, d_out, kOneRw - 2, G.stream));
         return r;
-      }))) return rc;
-  if ((rc = stage_one(o, bytes, len, st))) return rc;
-  CU(cudaGraphLaunch(o.g.exec, st));
-  CU(cudaMemcpyAsync(o.h_pin + kOneIn, d_out, (kOneHitRow + rs->dev.rw) * 4, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  count_launches(o.g.kernels);
-  const uint32_t* ho = reinterpret_cast<const uint32_t*>(o.h_pin + kOneIn);
+      }, s, kOneIn, (kOneHitRow + rs->dev.rw) * 4, kOneIn + 4 * kOneCounters);
+  if (rc) return rc;                                             // 1: a queue overflowed, the general path retries with larger scratch
+  const uint32_t* ho = reinterpret_cast<const uint32_t*>(s.h + kOneIn);
   const uint32_t* hc = ho + kOneCounters;
-  if ((rc = absorb_counters(rs, hc))) return rc;                 // 1: a queue overflowed, the general path retries with larger scratch
   count_step(1, len, hc);
   if (out_word) *out_word = (uint64_t)ho[0] | ((uint64_t)ho[1] << 32);
   const uint32_t nh = append_hit_row(ho + kOneHitRow, rs->dev.rw, 0, out_rules ? rules_cap : 0, [&](uint32_t i, uint32_t r) { out_rules[i] = r; });
@@ -1164,55 +1153,36 @@ int span_few_fast(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets,
   for (uint32_t i = 0; i < n; i++) if (offsets[i + 1] < offsets[i]) return 1;
   const uint32_t first = n ? offsets[0] : 0, len = n ? offsets[n] - first : 0;
   if (len > max_bytes) return 1;
-  cg_ruleset::SpanFew& f = rs->few;
-  cudaStream_t st = G.stream;
-  InOrder turn(&rs->order, st);
-  int rc;
-  if ((rc = turn.rc)) return rc;
-  if ((rc = few_staging(rs))) return rc;
-  if ((rc = prepare_step(rs, n, kStepSpans, st))) return rc;
-  const ScanWork& w = rs->work;
-  const uint8_t* d_bytes = f.d_buf; const uint32_t* d_off = reinterpret_cast<const uint32_t*>(f.d_buf);
-  uint32_t* d_pack = reinterpret_cast<uint32_t*>(rs->one.d_pack);
-  uint32_t* d_dig = reinterpret_cast<uint32_t*>(rs->one.d_pack + kOnePack);
-  uint8_t* d_out = rs->one.d_pack + 2 * kOnePack;
+  Staging& in = rs->span.in; Staging& pk = rs->span.pack;
   // the resolver's capacities on this path: every resolved span (and, redacting, its digest and the output) must fit the block
   const uint32_t at = pack_spans_at(n), room = kOnePack - at;
-  cg_ruleset::SpanGraph* g = nullptr;
-  if ((rc = few_graph(rs, n, redact, [&] {
-        const int r = run_scan_device(rs, d_bytes, d_off, n, w.words, kStepSpans, st);
+  // the window: the header with the offsets, 1 KB and len / 2 bytes (find-matches) or 2 x len bytes (redaction) of the packed result
+  const uint32_t window = std::min<uint32_t>(kOnePack, at + 1024 + (redact ? 2 * len : len / 2));
+  const int rc = blocking_call(rs, kStepSpans, n, 0, rs->span.graphs, {redact, n}, in, [&](uint8_t* h) { return stage_texts(h, kFewTextAt, bytes, offsets, n); }, [&] {
+        const ScanWork& w = rs->work;
+        const uint32_t* d_off = reinterpret_cast<const uint32_t*>(in.d);
+        uint32_t* d_pack = reinterpret_cast<uint32_t*>(pk.d); uint32_t* d_dig = reinterpret_cast<uint32_t*>(pk.d + kOnePack); uint8_t* d_out = pk.d + 2 * kOnePack;
+        const int r = run_scan_device(rs, in.d, d_off, n, w.words, kStepSpans, G.stream);
         if (r != CG_OK) return r;
         const SpanOutputs so{d_pack + at / 4, room / (redact ? 56u : 24u), d_pack + kPackOffsets, redact ? (uint64_t)room : 0ull, d_pack + kPackSizes, redact};
-        int k = launch_span_resolve_few(w, d_off, n, so, st);
-        if (redact) k += enqueue_redact_tail(w, d_bytes, d_off, d_pack + kPackOffsets, d_dig, d_out, n, st);
-        k += launch_span_pack_few(w, d_dig, d_out, d_pack, kOnePack, n, redact, st);
+        int k = launch_span_resolve_few(w, d_off, n, so, G.stream);
+        if (redact) k += enqueue_redact_tail(w, in.d, d_off, d_pack + kPackOffsets, d_dig, d_out, n, G.stream);
+        k += launch_span_pack_few(w, d_dig, d_out, d_pack, kOnePack, n, redact, G.stream);
         count_launches(k);
         CU(cudaGetLastError());
         return CG_OK;
-      }, &g))) return rc;
-  uint32_t* hoff = reinterpret_cast<uint32_t*>(f.h_pin);
-  for (uint32_t i = 0; i <= n; i++) hoff[i] = kFewTextAt + (n ? offsets[i] - first : 0);
-  if (len) memcpy(f.h_pin + kFewTextAt, bytes + first, len);
-  memset(f.h_pin + kFewTextAt + len, 0, 64);
-  CU(cudaMemcpyAsync(f.d_buf, f.h_pin, (size_t)kFewTextAt + len + 64, cudaMemcpyHostToDevice, st));
-  CU(cudaGraphLaunch(g->exec, st));
-  // the window: the header with the offsets, 1 KB and len / 2 bytes (find-matches) or 2 x len bytes (redaction) of the packed result
-  const uint32_t window = std::min<uint32_t>(kOnePack, at + 1024 + (redact ? 2 * len : len / 2));
-  uint8_t* h_pack = rs->one.h_pack;
-  CU(cudaMemcpyAsync(h_pack, d_pack, window, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  count_launches(g->kernels);
-  const uint32_t* hp = reinterpret_cast<const uint32_t*>(h_pack);
+      }, pk, 0, window, 4 * kPackCounters);
+  if (rc) return rc;                                             // 1: a queue overflowed, the batch call retries with larger scratch
+  const uint32_t* hp = reinterpret_cast<const uint32_t*>(pk.h);
   const uint32_t* hc = hp + kPackCounters;
-  if ((rc = absorb_counters(rs, hc))) return rc;                 // 1: a queue overflowed, the batch call retries with larger scratch
   const uint32_t packed = hp[0];
   if (!packed) return 1;                                         // longer than the packed region: the batch call has room
   if (packed > window) {
-    CU(cudaMemcpyAsync(h_pack + window, reinterpret_cast<const uint8_t*>(d_pack) + window, packed - window, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
+    CU(cudaMemcpyAsync(pk.h + window, pk.d + window, packed - window, cudaMemcpyDeviceToHost, G.stream));
+    CU(cudaStreamSynchronize(G.stream));
   }
   count_step(n, len, hc);
-  const uint8_t* body = h_pack + at;
+  const uint8_t* body = pk.h + at;
   if (!redact) {
     const uint32_t ns = hp[kPackSizes];
     G.stats.spans += ns;
@@ -1563,15 +1533,6 @@ int cg_policy_eval_batch_device(cg_ruleset* rs, const void* d_bytes, const void*
 }
 
 namespace {
-// cg_policy_eval_one's staging block, host (pinned) and device: in, [offsets, kPeOneTexts + 1][roles][atom row, kPeOneAtomWords]
-// [text bytes, kPeOneBytes][64 zero bytes] at fixed places (offsets are rebased to kPeTextAt); out, kPeOneRules + kPeOneRulesCap
-// words (kernels.h).  The limits: 64 texts (kPeOneTexts: the kernel keeps the text list in shared memory), 64 KB of text (a tool
-// call's params or a message with its conversation history), 32 768 atoms, 4096 matched policies.
-constexpr uint32_t kPeOneBytes = 65536, kPeOneAtomWords = 1024, kPeOneRulesCap = 4096;
-constexpr uint32_t kPeRolesAt = 512, kPeAtomsAt = kPeRolesAt + 256, kPeTextAt = kPeAtomsAt + 4 * kPeOneAtomWords;
-constexpr uint32_t kPeIn = kPeTextAt + kPeOneBytes + 64, kPeOut = 4 * (kPeOneRules + kPeOneRulesCap);
-static_assert(4 * (kPeOneTexts + 1) <= kPeRolesAt && kPeOneTexts <= 256 && kPeTextAt % 256 == 0, "cg_policy_eval_one staging layout");
-
 // cg_policy_eval_one on the staging block: one H2D copy, one graph (the policy-mode step over the staged texts, then
 // policy_eval_one_kernel), one D2H copy of the header and as many rules as the caller can take, one synchronise.  Outputs,
 // statuses and statistics are those of cg_policy_eval_batch with one context.  -> CG_OK, an error, or 1 = take the batch call
@@ -1586,50 +1547,25 @@ int policy_one_fast(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offset
   for (uint32_t i = 0; i < n_texts; i++) if (offsets[i + 1] < offsets[i]) return 1;
   const uint32_t first = n_texts ? offsets[0] : 0, len = n_texts ? offsets[n_texts] - first : 0;
   if (len > kPeOneBytes) return 1;
-  cg_ruleset::PolicyOne& o = rs->pone;
-  cudaStream_t st = G.stream;
-  InOrder turn(&rs->order, st);
-  int rc;
-  if ((rc = turn.rc)) return rc;
-  if (!o.h_pin) { CU(cudaMallocHost((void**)&o.h_pin, kPeIn + kPeOut)); memset(o.h_pin, 0, kPeIn + kPeOut); }
-  if (!o.d_buf) { CU(cudaMalloc((void**)&o.d_buf, kPeIn + kPeOut)); CU(cudaMemset(o.d_buf, 0, kPeIn + kPeOut)); }
-  if ((rc = prepare_step(rs, n_texts, kStepPolicy, st, 1))) return rc;
-  const ScanWork& w = rs->work;
-  uint32_t* d_out = reinterpret_cast<uint32_t*>(o.d_buf + kPeIn);
-  // the graph of this text count, captured again when the scratch, the verify grid or the program changed since
-  cg_ruleset::PeGraph* g = nullptr;
-  for (auto& e : o.g) if (e.exec && e.n == n_texts && e.gen == rs->scratch_gen && e.ctas == rs->verify_ctas && e.prog == rs->prog_gen) g = &e;
-  if (!g) {
-    g = &o.g[0];
-    for (auto& e : o.g) if (e.used < g->used) g = &e;
-    if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; }
-    const PolicyBatch b{o.d_buf + kPeRolesAt, n_texts, nullptr, reinterpret_cast<const uint32_t*>(o.d_buf + kPeAtomsAt), 1};
-    if ((rc = capture(st, [&] {
-          const int r = run_scan_device(rs, o.d_buf, reinterpret_cast<const uint32_t*>(o.d_buf), n_texts, w.words, kStepPolicy, st);
-          if (r != CG_OK) return r;
-          count_launches(launch_policy_eval_one(pt, w, rs->dev.rw, b, d_out, kPeOneRulesCap, st));
-          CU(cudaGetLastError());
-          return CG_OK;
-        }, &g->exec, &g->kernels))) return rc;
-    g->n = n_texts; g->gen = rs->scratch_gen; g->ctas = rs->verify_ctas; g->prog = rs->prog_gen;
-  }
-  g->used = ++o.clock;
-  uint32_t* hoff = reinterpret_cast<uint32_t*>(o.h_pin);
-  for (uint32_t i = 0; i <= n_texts; i++) hoff[i] = kPeTextAt + (n_texts ? offsets[i] - first : 0);
-  if (n_texts) memcpy(o.h_pin + kPeRolesAt, roles, n_texts);
-  if (pt.aw) memcpy(o.h_pin + kPeAtomsAt, atoms, (size_t)pt.aw * 4);
-  if (len) memcpy(o.h_pin + kPeTextAt, bytes + first, len);
-  memset(o.h_pin + kPeTextAt + len, 0, 64);
-  CU(cudaMemcpyAsync(o.d_buf, o.h_pin, (size_t)kPeTextAt + len + 64, cudaMemcpyHostToDevice, st));
-  CU(cudaGraphLaunch(g->exec, st));
+  Staging& s = rs->pone.io;
   // matches <= policies <= program rules: no more of them than the caller takes can be needed
   const uint32_t want = std::min(std::min(out_rules ? rules_cap : 0u, kPeOneRulesCap), pt.n_rules);
-  uint32_t* ho = reinterpret_cast<uint32_t*>(o.h_pin + kPeIn);
-  CU(cudaMemcpyAsync(ho, d_out, 4 * ((size_t)kPeOneRules + want), cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  count_launches(g->kernels);
+  const int rc = blocking_call(rs, kStepPolicy, n_texts, 1, rs->pone.graphs, {n_texts, rs->prog_gen}, s, [&](uint8_t* h) {
+        if (n_texts) memcpy(h + kPeRolesAt, roles, n_texts);
+        if (pt.aw) memcpy(h + kPeAtomsAt, atoms, (size_t)pt.aw * 4);
+        return stage_texts(h, kPeTextAt, bytes, offsets, n_texts);
+      }, [&] {
+        const ScanWork& w = rs->work;
+        const PolicyBatch b{s.d + kPeRolesAt, n_texts, nullptr, reinterpret_cast<const uint32_t*>(s.d + kPeAtomsAt), 1};
+        const int r = run_scan_device(rs, s.d, reinterpret_cast<const uint32_t*>(s.d), n_texts, w.words, kStepPolicy, G.stream);
+        if (r != CG_OK) return r;
+        count_launches(launch_policy_eval_one(pt, w, rs->dev.rw, b, reinterpret_cast<uint32_t*>(s.d + kPeIn), kPeOneRulesCap, G.stream));
+        CU(cudaGetLastError());
+        return CG_OK;
+      }, s, kPeIn, 4 * ((size_t)kPeOneRules + want), kPeIn + 4 * kPeOneCounters);
+  if (rc) return rc;                                             // 1: a queue overflowed, the batch call retries with larger scratch
+  const uint32_t* ho = reinterpret_cast<const uint32_t*>(s.h + kPeIn);
   const uint32_t* hc = ho + kPeOneCounters;
-  if ((rc = absorb_counters(rs, hc))) return rc;                 // 1: a queue overflowed, the batch call retries with larger scratch
   const uint32_t nm = ho[1];
   if (out_rules && nm > kPeOneRulesCap && rules_cap > kPeOneRulesCap) return 1;
   count_step(n_texts, len, hc);
