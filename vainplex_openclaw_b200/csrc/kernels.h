@@ -57,7 +57,7 @@ struct DevRuleset {
 // Per-call scratch in HBM.  A "slot" is one message with at least one confirmed candidate.
 struct ScanWork {
   uint32_t* counters;            // kCounterWords words, indexed by kCtr* (below)
-  uint32_t* l1_pos;              // [l1_cap] factor occurrences scan_kernel confirms itself (head check, trigger bytes): buffer offset of the
+  uint32_t* l1_pos;              // [l1_cap] factor occurrences scan_kernel (trigger bytes) and confirm_kernel confirm: buffer offset of the
   uint32_t* l1_fac;              //          factor's first byte, factor id
   uint2* fq;                     // [l1_cap] scan_kernel's flag words: x = the lane's first-half chunk number after the round, y = 32 probe bits (scan_kernels.cu: flagged_gram_pos)
   uint32_t* persist;             // [4] survives the per-step reset: [0] = slots the previous step used (their candidate / hit rows are zeroed by the next step's reset_kernel)

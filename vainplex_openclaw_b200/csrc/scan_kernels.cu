@@ -75,11 +75,12 @@ __device__ __forceinline__ uint4 ldg_stream(const uint8_t* p) {
 //       second half's, probe 0 of a half highest; a round is as many tiles as fill 32 bits (two at stride 2, four at
 //       stride 4), the oldest tile highest, and the lane's queue entry carries its first-half chunk after the round.
 //   1b  lanes with flagged grams push (chunk, flag word) to a per-warp ring in shared memory, which goes to a queue in HBM
-//       32 entries at a time; confirm_kernel takes it from there (recheck map, level-1b lookup, exact factor, message).  Confirmed factor
+//       128 entries at a time; confirm_kernel takes it from there (recheck map, level-1b lookup, exact factor, message).  Confirmed factor
 //       occurrences go to the queue in HBM, one atomic each (they are rare).
 // ------------------------------------------------------------------------------------------
 constexpr int kScanThreads = 1024;      // 32 warps, one CTA per SM
-constexpr uint32_t kRing = 64;          // (chunk, flag word) pairs a warp collects before it appends 32 of them to the queue in HBM
+constexpr uint32_t kAppend = 128;       // (chunk, flag word) pairs a warp collects before it appends them to the queue in HBM, one atomic
+constexpr uint32_t kRing = 256;         // ring entries per warp (a power of two): fewer than kAppend + one round's 32 are ever held
 constexpr uint32_t kScanRingBytes = (kScanThreads / 32) * kRing * 8;
 constexpr uint32_t kTileChunks = 64;    // 16-byte chunks per warp tile: two halves of 32
 // probe bits per 16-byte chunk = grams per chunk (stride 2: 8, stride 4: 4); tiles per round = 32 / (2 * half_bits)
@@ -163,16 +164,6 @@ __device__ __forceinline__ void trigger_chunk(const DevRuleset& rs, const ScanWo
   }
 }
 
-// An occurrence that starts less than three bytes into the scanned range has no gram in front of it: compared directly.
-__device__ __noinline__ void head_check(const DevRuleset& rs, const ScanWork& w, const ScanCtx& c) {
-  QueueEmit emit{w};
-  for (uint32_t i = threadIdx.x; i < 3u * rs.n_factors; i += blockDim.x) {
-    const uint32_t f = i / 3u, t0 = c.begin + i % 3u;
-    const uint32_t* fw = c.T.factors + (size_t)f * 12;
-    if (t0 < c.end && t0 + (fw[1] & 0xffu) <= c.end && factor_at(fw, c.T.bytesets, c.bytes + t0)) emit(t0, f);
-  }
-}
-
 template <int NPROBE, int NTRIG, int BLOOM2, int NT>
 __global__ void __launch_bounds__(NT, 1)
 scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n,
@@ -200,19 +191,20 @@ scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanW
   asm volatile("" : "+r"(lt));                // (loop invariants the compiler would otherwise recompute in every iteration of the hot loop)
   const uint32_t bm = smem_u32(smem);
   const uint32_t ring1 = smem_u32(smem + rs.image_bytes) + warp * (kRing * 8);
-  ctx.T.factors = rs.factors; ctx.T.bytesets = rs.bytesets; ctx.T.bucket_start = rs.bucket_start; ctx.T.entries = rs.entries;    // (head check and triggers only)
-  constexpr uint32_t kShift = NPROBE == 2 ? 1 : 2;             // flagged gram = its byte position >> kShift
+  ctx.T.factors = rs.factors; ctx.T.bytesets = rs.bytesets; ctx.T.bucket_start = rs.bucket_start; ctx.T.entries = rs.entries;    // (triggers only)
   HotConst hk; hk.c5f = rs.hot_c5f; hk.c10 = rs.hot_c10; hk.one = rs.hot_one; hk.mask = rs.bm_mask;
   asm volatile("" : "+r"(hk.c5f), "+r"(hk.c10), "+r"(hk.one), "+r"(hk.mask));
-  if (blockIdx.x == 0) head_check(rs, w, ctx);
 
   const uint32_t first_chunk = begin >> 4;
   uint32_t end_chunk = (end + 15u) >> 4;       // 16-byte chunks [first, end)
   // folded (z domain) trigger bytes, splatted
   uint32_t splat0 = NTRIG > 0 ? (((rs.trig_byte[0] & 0x5fu) ^ 0x10u) * 0x01010101u) : 0u, splat1 = NTRIG > 1 ? (((rs.trig_byte[1] & 0x5fu) ^ 0x10u) * 0x01010101u) : 0u;
   asm volatile("" : "+r"(splat0), "+r"(splat1));
-  // this lane's first-half chunk in the warp's current tile (64 chunks = 1 KB); tiles are dealt round-robin to all warps of the grid
-  uint32_t c = first_chunk + (blockIdx.x * wpb + warp) * kTileChunks + lane;
+  // this lane's first-half chunk in the warp's current tile (64 chunks = 1 KB).  Tiles are dealt round-robin to all warps of
+  // the grid, CTA-interleaved (warp w of CTA b is the grid's warp w x grid + b): the tiles left over after the last full
+  // round then go to one or two warps of every SM, not to every warp of the first few CTAs, whose SMs would stream a whole
+  // extra tile while the others have finished.
+  uint32_t c = first_chunk + (warp * gridDim.x + blockIdx.x) * kTileChunks + lane;
   uint32_t cstep = gridDim.x * wpb * kTileChunks;
   uint32_t shl_bits = hk.one << half_bits(NPROBE);
   asm volatile("" : "+r"(end_chunk), "+r"(cstep), "+r"(shl_bits));
@@ -287,17 +279,21 @@ scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanW
   };
   // Nothing is done about a flagged gram here: looking at one means a chain of dependent loads (the gram again, the
   // recheck map, the level-1b bucket, the factor, the text around it), and with 32 warps per SM there is nobody to hide
-  // that latency behind: a slow path inside this kernel would stall the hot loop, whatever its instruction count.  The flag words go to a queue in HBM, 32 at a time (one atomic per 32), and
-  // confirm_kernel, with one thread per flag word and the whole GPU's worth of warps, does the looking.
+  // that latency behind: a slow path inside this kernel would stall the hot loop, whatever its instruction count.  The
+  // flag words go to a queue in HBM, and confirm_kernel, with one thread per flag word and the whole GPU's worth of warps,
+  // does the looking.  A warp appends kAppend of them at a time behind ONE atomic, whose result every lane waits for while
+  // it issues no new tile, so there are few appends -- one or two per warp on C2 traffic (appends of 32 took the 5000-rule
+  // scan 0.193 ms instead of 0.121).  Reserving the next block one append ahead, so that nobody waits, measured slower.
   uint32_t h1 = 0, t1 = 0;       // the ring holds [h1, t1)
-  auto append32 = [&](uint32_t k) {                         // k <= 32 entries from the ring -> the queue
+  auto append = [&](uint32_t k) {                           // k entries from the ring -> the queue
     uint32_t base = 0;
     if (lane == 0) base = atomicAdd(&w.counters[kCtrFlagWords + w.q_slot], k);
     base = __shfl_sync(FULL, base, 0);
-    if (lane < k) {
+#pragma unroll 1
+    for (uint32_t j = lane; j < k; j += 32u) {
       uint32_t cw, aw;
-      asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(cw), "=r"(aw) : "r"(ring1 + (((h1 + lane) & (kRing - 1)) << 3)));
-      if (base + lane < w.q_cap) w.fq[base + lane] = make_uint2(cw, aw); else atomicOr(&w.counters[kCtrErrors], ERR_L1_OVERFLOW);
+      asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(cw), "=r"(aw) : "r"(ring1 + (((h1 + j) & (kRing - 1)) << 3)));
+      if (base + j < w.q_cap) w.fq[base + j] = make_uint2(cw, aw); else atomicOr(&w.counters[kCtrErrors], ERR_L1_OVERFLOW);
     }
     h1 += k;
   };
@@ -315,11 +311,11 @@ scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanW
     if (m) {
       if (acc) asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(ring1 + (((t1 + __popc(m & lt)) & (kRing - 1)) << 3)), "r"(c), "r"(acc) : "memory");
       t1 += __popc(m); acc = 0;
-      if (t1 - h1 >= 32u) { __syncwarp(); append32(32u); }
+      if (t1 - h1 >= kAppend) { __syncwarp(); append(kAppend); }
     }
   }
   __syncwarp();
-  if (t1 != h1) append32(t1 - h1);
+  if (t1 != h1) append(t1 - h1);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -396,7 +392,7 @@ struct SlotSink {
 // thread.  So it runs in launches of its own:
 //   confirm_kernel  flag word -> gram positions -> gram reloaded, folded, recheck map, table probes -> exact factor  -> factor occurrences
 //   resolve_kernel  message of the occurrence (no straddling), slot, island matcher / candidate for the VM / direct hit; also the
-//                   occurrences scan_kernel found itself (head check, trigger bytes) and the rules every message is a candidate for
+//                   occurrences of trigger bytes and of the head check, and the rules every message is a candidate for
 // ------------------------------------------------------------------------------------------
 // What bounds this work is not re-reading the flagged places of the batch (a random gather, profiles/micro/gather_micro.cu)
 // but the number of uncoalesced loads behind each item: a gram, its recheck word and slots, then the entry, factor words,
@@ -520,6 +516,20 @@ __device__ __forceinline__ void confirm_gram(ConfirmCtx& c, uint32_t pos, bool a
   }
 }
 
+// An occurrence that starts less than three bytes into the scanned range has no gram in front of it: compared directly,
+// here rather than in scan_kernel, where the block that did it started streaming late and set the kernel's end.  The 3 x
+// n_factors checks are spread over the grid and, inside a block, over its warps (the block's j-th check goes to lane
+// j / wpb of warp j mod wpb), so that no warp pays more than a few of these chains of dependent loads before its queue work.
+__device__ __noinline__ void head_check(const DevRuleset& rs, const ScanWork& w, const uint8_t* __restrict__ bytes, uint32_t begin, uint32_t end) {
+  QueueEmit emit{w};
+  const uint32_t wpb = blockDim.x >> 5, t = (threadIdx.x & 31u) * wpb + (threadIdx.x >> 5);
+  for (uint32_t i = t * gridDim.x + blockIdx.x; i < 3u * rs.n_factors; i += gridDim.x * blockDim.x) {
+    const uint32_t f = i / 3u, t0 = begin + i % 3u;
+    const uint32_t* fw = rs.factors + (size_t)f * 12;
+    if (t0 < end && t0 + (fw[1] & 0xffu) <= end && factor_at(fw, rs.bytesets, bytes + t0)) emit(t0, f);
+  }
+}
+
 // NPROBE as scan_kernel's: the flag-word decode is a handful of shifts and masks per bit (flagged_gram_pos)
 template <int NPROBE>
 __global__ void __launch_bounds__(kCfThreads, 1)
@@ -539,6 +549,7 @@ confirm_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ Sc
     T = st;
     __syncthreads();
   }
+  head_check(rs, w, bytes, off[0], off[n]);
   const uint32_t gwarp = blockIdx.x * wpb + warp, nwarps = gridDim.x * wpb;
   ConfirmCtx c{rs, w, bytes, T, reinterpret_cast<const uint4*>(T + rs.cf_slots_off), reinterpret_cast<const uint32_t*>(T + rs.cf_ge_off),
                reinterpret_cast<const uint32_t*>(T + rs.cf_fac_off), reinterpret_cast<const uint32_t*>(T + rs.cf_bs_off), pring, 0u, 0u, off[0], off[n], rs.n_shapes, 0u, lane};
