@@ -407,16 +407,35 @@ struct SlotSink {
 //     entries a gram hits become (position, entry) pairs, in WAVES of at most one item per lane that are compacted with a
 //     ballot into a 64-entry ring per warp in shared memory; whenever a ring holds 32 items, all 32 lanes run the next stage
 //     as a straight line (gram -> recheck -> probes | quick test -> whole factor).  Leftovers wait for the next wave.
+//   * confirmed occurrences are as rare as one or two per wave of 32 pairs, and an atomicAdd per occurrence on the one
+//     counter word queues every lane of the grid at one L2 slice: they collect in a 32-entry buffer per warp, which goes to
+//     the queue behind ONE atomic whenever the next wave would not fit, and at the end.
 constexpr uint32_t kCfRing = 64;                  // entries per warp and ring (a power of two): 31 leftovers + one wave of 32
+constexpr uint32_t kCfOcc = 32;                   // confirmed (position, factor) pairs a warp holds before it appends them
 constexpr int kCfThreads = 1024;
-constexpr uint32_t kCfRingBytes = (kCfThreads / 32) * kCfRing * (4 + 8);     // gram positions (4 B) and (position, entry) pairs (8 B)
+constexpr uint32_t kCfWarpBytes = kCfRing * (4 + 8) + kCfOcc * 8;    // gram positions (4 B), (position, entry) pairs (8 B), occurrences (8 B)
+constexpr uint32_t kCfRingBytes = (kCfThreads / 32) * kCfWarpBytes;
+static_assert(kCfRingBytes + kConfirmTableBudget + 1024u <= 227u * 1024u, "rings and resident tables fit the H100's opt-in shared memory per block");
 
 struct ConfirmCtx {
   const DevRuleset& rs; const ScanWork& w; const uint8_t* bytes;
   const uint8_t* rk; const uint4* slots; const uint32_t* group_entries; const uint32_t* factors; const uint32_t* bytesets;     // shared-memory copies when they fit
   uint2* pring; uint32_t phead, ptail;          // this warp's ring of (gram position, entry) pairs
+  uint2* occ; uint32_t held;                    // this warp's confirmed occurrences not yet in the queue: occ[0, held)
   uint32_t begin, end, n_shapes, passed, lane;
 };
+// the warp's held occurrences -> the queue (warp-uniform; the counter keeps counting past l1_cap, as every queue's does)
+__device__ __forceinline__ void append_occurrences(ConfirmCtx& c) {
+  uint32_t base = 0;
+  if (c.lane == 0) base = atomicAdd(&c.w.counters[kCtrConfirmed], c.held);
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (c.lane < c.held) {
+    const uint2 o = c.occ[c.lane];
+    if (base + c.lane < c.w.l1_cap) { c.w.l1_pos[base + c.lane] = o.x; c.w.l1_fac[base + c.lane] = o.y; } else atomicOr(&c.w.counters[kCtrErrors], ERR_L1_OVERFLOW);
+  }
+  c.held = 0;
+  __syncwarp();
+}
 __device__ __forceinline__ uint32_t byteset_bit(const uint32_t* __restrict__ bytesets, uint32_t sid, uint32_t b) { return (bytesets[(size_t)sid * 8 + (b >> 5)] >> (b & 31)) & 1u; }
 
 // one (gram, entry) pair per lane: does the entry's factor start at the position the gram implies?  First the (up to) four
@@ -463,10 +482,12 @@ __device__ __forceinline__ void confirm_pairs(ConfirmCtx& c, uint2 pr, bool acti
     }
     ok = bits != 0;
   }
-  if (ok) {
-    const uint32_t k = atomicAdd(&c.w.counters[kCtrConfirmed], 1u);
-    if (k < c.w.l1_cap) { c.w.l1_pos[k] = (uint32_t)t0; c.w.l1_fac[k] = f; } else atomicOr(&c.w.counters[kCtrErrors], ERR_L1_OVERFLOW);
-  }
+  const uint32_t m = __ballot_sync(0xffffffffu, ok);
+  if (!m) return;
+  if (c.held + __popc(m) > kCfOcc) append_occurrences(c);
+  if (ok) c.occ[c.held + __popc(m & ((1u << c.lane) - 1u))] = make_uint2((uint32_t)t0, f);
+  c.held += __popc(m);
+  __syncwarp();
 }
 
 // one gram position per lane (active lanes only do loads; everybody takes part in the votes): gram -> recheck map -> one probe
@@ -520,6 +541,7 @@ __device__ __forceinline__ void confirm_gram(ConfirmCtx& c, uint32_t pos, bool a
 // here rather than in scan_kernel, where the block that did it started streaming late and set the kernel's end.  The 3 x
 // n_factors checks are spread over the grid and, inside a block, over its warps (the block's j-th check goes to lane
 // j / wpb of warp j mod wpb), so that no warp pays more than a few of these chains of dependent loads before its queue work.
+// They find an occurrence rarely (only where a factor starts the batch), so each keeps its own atomic (QueueEmit).
 __device__ __noinline__ void head_check(const DevRuleset& rs, const ScanWork& w, const uint8_t* __restrict__ bytes, uint32_t begin, uint32_t end) {
   QueueEmit emit{w};
   const uint32_t wpb = blockDim.x >> 5, t = (threadIdx.x & 31u) * wpb + (threadIdx.x >> 5);
@@ -534,25 +556,29 @@ __device__ __noinline__ void head_check(const DevRuleset& rs, const ScanWork& w,
 template <int NPROBE>
 __global__ void __launch_bounds__(kCfThreads, 1)
 confirm_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, uint32_t cstep) {
-  extern __shared__ __align__(16) uint8_t cf_smem[];          // [pair rings][gram rings][tables, when resident]
+  extern __shared__ __align__(16) uint8_t cf_smem[];          // [pair rings][gram rings][occurrence buffers][tables, when resident]
+  __shared__ uint32_t cta_ctr[3];                             // flagged grams, grams past the recheck map, pairs: one atomic each per CTA
   const uint32_t cstep16 = cstep * 16u;
   const uint32_t nq = (rs.debug_flags & 1u) ? 0u : min(w.counters[kCtrFlagWords + w.q_slot], w.q_cap);
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5, FULL = 0xffffffffu, lt = (1u << lane) - 1u;
   uint2* pring = reinterpret_cast<uint2*>(cf_smem) + warp * kCfRing;
   uint32_t* ring = reinterpret_cast<uint32_t*>(cf_smem + (size_t)wpb * kCfRing * 8) + warp * kCfRing;
+  uint2* occ = reinterpret_cast<uint2*>(cf_smem + (size_t)wpb * kCfRing * 12) + warp * kCfOcc;
+  if (threadIdx.x < 3) cta_ctr[threadIdx.x] = 0u;
   const uint8_t* T = rs.cf_image;
   if (rs.cf_resident) {
-    uint8_t* st = cf_smem + (size_t)wpb * kCfRing * 12;
+    uint8_t* st = cf_smem + (size_t)wpb * kCfWarpBytes;
     if (blockIdx.x * 32u * wpb < nq) {           // (a block without work does not need them)
       for (uint32_t o = threadIdx.x * 16u; o < rs.cf_bytes; o += blockDim.x * 16u) *reinterpret_cast<uint4*>(st + o) = ldg_stream(rs.cf_image + o);
     }
     T = st;
-    __syncthreads();
   }
+  __syncthreads();
   head_check(rs, w, bytes, off[0], off[n]);
   const uint32_t gwarp = blockIdx.x * wpb + warp, nwarps = gridDim.x * wpb;
   ConfirmCtx c{rs, w, bytes, T, reinterpret_cast<const uint4*>(T + rs.cf_slots_off), reinterpret_cast<const uint32_t*>(T + rs.cf_ge_off),
-               reinterpret_cast<const uint32_t*>(T + rs.cf_fac_off), reinterpret_cast<const uint32_t*>(T + rs.cf_bs_off), pring, 0u, 0u, off[0], off[n], rs.n_shapes, 0u, lane};
+               reinterpret_cast<const uint32_t*>(T + rs.cf_fac_off), reinterpret_cast<const uint32_t*>(T + rs.cf_bs_off), pring, 0u, 0u, occ, 0u,
+               off[0], off[n], rs.n_shapes, 0u, lane};
   uint32_t head = 0, tail = 0, flagged = 0;
   for (uint32_t base = gwarp * 32u; base < nq; base += nwarps * 32u) {
     uint2 q = make_uint2(0u, 0u);
@@ -574,8 +600,15 @@ confirm_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ Sc
   }
   if (tail != head) { const bool a = lane < tail - head; const uint32_t pos = a ? ring[(head + lane) & (kCfRing - 1)] : 0u; __syncwarp(); confirm_gram(c, pos, a); }
   if (c.ptail != c.phead) { const bool a = lane < c.ptail - c.phead; const uint2 pr = a ? c.pring[(c.phead + lane) & (kCfRing - 1)] : make_uint2(0u, 0u); confirm_pairs(c, pr, a); }
+  if (c.held) append_occurrences(c);
   const uint32_t passed = __reduce_add_sync(FULL, c.passed);
-  if (lane == 0) { if (flagged) atomicAdd(&w.counters[kCtrFlagged], flagged); if (passed) atomicAdd(&w.counters[kCtrPastRecheck], passed); if (c.ptail) atomicAdd(&w.counters[kCtrPairs + w.q_slot], c.ptail); }
+  if (lane == 0) { if (flagged) atomicAdd(&cta_ctr[0], flagged); if (passed) atomicAdd(&cta_ctr[1], passed); if (c.ptail) atomicAdd(&cta_ctr[2], c.ptail); }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (cta_ctr[0]) atomicAdd(&w.counters[kCtrFlagged], cta_ctr[0]);
+    if (cta_ctr[1]) atomicAdd(&w.counters[kCtrPastRecheck], cta_ctr[1]);
+    if (cta_ctr[2]) atomicAdd(&w.counters[kCtrPairs + w.q_slot], cta_ctr[2]);
+  }
 }
 
 // Which (message, rule) pairs may enter a slot: every pair (the calls without views), or only the rules of the message's
