@@ -166,7 +166,7 @@ CG_HD uint32_t island_start(const DevRuleset& rs, uint32_t rule, const uint8_t* 
 CG_HD int island_test(const DevRuleset& rs, uint32_t f, uint32_t r, const uint8_t* __restrict__ m, uint32_t len, uint32_t t0, uint32_t pre, uint32_t max_steps) {
   const uint64_t* bp = reinterpret_cast<const uint64_t*>(rs.bit_words) + rs.bit_off[r];
   const uint64_t* resume = nullptr; uint32_t s = 0;
-  if (f != 0xffffffffu && rs.factor_skip) {
+  if (f != 0xffffffffu) {
     const uint64_t* sk = reinterpret_cast<const uint64_t*>(rs.factor_skip) + (size_t)f * 3;
     const uint32_t L = (uint32_t)sk[0];
     if (L && t0 + L <= len) { resume = sk + 1; s = t0 + L; }

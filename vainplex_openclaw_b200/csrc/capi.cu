@@ -34,9 +34,7 @@ struct Ctx {
   int device = 0, sm_count = 132;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  cudaEvent_t pev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  cudaEvent_t pev_scan[8] = {};      // profiling: begin / end of scan_kernel for each of the (at most four) pieces of a step
-  uint32_t prof_pieces = 0;
+  cudaEvent_t pev[6] = {};          // profiling: before scan_kernel, after scan_kernel, confirm_kernel, resolve, verify, finalize
   bool profiling = false;
   cg_stats stats{};
   // grow-only staging in HBM
@@ -284,7 +282,6 @@ int ensure_work(cg_ruleset* rs, ScanWork& w, uint32_t n_msgs, uint32_t l1_cap, u
   return CG_OK;
 }
 
-static uint32_t scan_pieces() { static const uint32_t k = [] { const char* e = getenv("CG_PIECES"); const int v = e ? atoi(e) : 1; return (uint32_t)(v >= 1 && v <= 4 ? v : 1); }(); return k; }
 // What a step computes: result words only; a policy step whose per-message scratch a hit list or verdicts read afterwards;
 // or a span step (raw spans for the span resolver, result words in ScanWork::words).
 enum StepKind { kStepWords, kStepPolicy, kStepSpans };
@@ -299,27 +296,16 @@ int run_scan_device(cg_ruleset* rs, const uint8_t* d_bytes, const uint32_t* d_of
   const bool spans = kind == kStepSpans;
   int k = launch_reset(rs->dev, w, n, G.sm_count, st);
   if (G.profiling) cudaEventRecord(G.pev[0], st);
-  // CG_PIECES = 2..4 scans the batch in pieces, each followed by its own lookup + check, so that a flagged gram is read again
-  // while its piece is still in the 50 MB L2.  Every extra launch of the latency-bound kernels costs time the L2 hits have to
-  // win back.  One piece unless asked otherwise.
-  const uint32_t K = scan_pieces();
-  if (G.profiling) G.prof_pieces = K;
-  for (uint32_t piece = 0; piece < K; piece++) {
-    const uint32_t m0 = (uint32_t)((uint64_t)n * piece / K), m1 = (uint32_t)((uint64_t)n * (piece + 1) / K);
-    if (m1 == m0) continue;
-    ScanWork wk = w; wk.q_cap = w.l1_cap / K; wk.q_slot = piece; wk.fq = w.fq + (size_t)piece * wk.q_cap;
-    if (G.profiling) cudaEventRecord(G.pev_scan[2 * piece], st);
-    k += launch_scan(rs->dev, wk, d_bytes, d_off + m0, m1 - m0, d_words + m0, G.sm_count, st);
-    if (G.profiling) cudaEventRecord(G.pev_scan[2 * piece + 1], st);
-    k += launch_confirm(rs->dev, wk, d_bytes, d_off + m0, m1 - m0, G.sm_count, st);
-  }
+  k += launch_scan(rs->dev, w, d_bytes, d_off, n, d_words, G.sm_count, st);
   if (G.profiling) cudaEventRecord(G.pev[1], st);
-  k += launch_resolve(rs->dev, w, d_bytes, d_off, n, spans, G.sm_count, st, views);
+  k += launch_confirm(rs->dev, w, d_bytes, d_off, n, G.sm_count, st);
   if (G.profiling) cudaEventRecord(G.pev[2], st);
-  k += launch_verify(rs->dev, w, d_bytes, d_off, spans, G.sm_count, st, spans ? 4 : rs->verify_ctas);
+  k += launch_resolve(rs->dev, w, d_bytes, d_off, n, spans, G.sm_count, st, views);
   if (G.profiling) cudaEventRecord(G.pev[3], st);
-  k += launch_finalize(rs->dev, w, d_words, n, G.sm_count, st);
+  k += launch_verify(rs->dev, w, d_bytes, d_off, spans, G.sm_count, st, spans ? 4 : rs->verify_ctas);
   if (G.profiling) cudaEventRecord(G.pev[4], st);
+  k += launch_finalize(rs->dev, w, d_words, n, G.sm_count, st);
+  if (G.profiling) cudaEventRecord(G.pev[5], st);
   count_launches(k);
   CU(cudaGetLastError());
   return CG_OK;
@@ -348,12 +334,10 @@ int prepare_step(cg_ruleset* rs, uint32_t n, StepKind kind, cudaStream_t st, uin
   CU(cudaStreamSynchronize(st));
   return ensure_work(rs, rs->work, n, l1, slot, ev, span, res);
 }
-// fq is cut into four equal pieces at most: the fullest piece decides
-static uint32_t queue_need(const uint32_t* hc) { uint32_t m = 0; for (int i = 0; i < 4; i++) m = std::max(m, hc[kCtrFlagWords + i]); return m > 0xffffffffu / scan_pieces() ? 0xffffffffu : scan_pieces() * m; }
 // what an overflowed step teaches about the capacities the next one needs
 void learn_caps(cg_ruleset* rs, const uint32_t* hc) {
   const uint32_t flags = hc[kCtrErrors];
-  if (flags & ERR_L1_OVERFLOW) { const uint32_t need = std::max(hc[kCtrConfirmed], queue_need(hc)); rs->grow_l1 = std::max<uint32_t>(rs->grow_l1, std::max<uint32_t>(2 * need, need + 65536)); }
+  if (flags & ERR_L1_OVERFLOW) { const uint32_t need = std::max(hc[kCtrConfirmed], hc[kCtrFlagWords]); rs->grow_l1 = std::max<uint32_t>(rs->grow_l1, std::max<uint32_t>(2 * need, need + 65536)); }
   if (flags & ERR_SLOT_OVERFLOW) rs->grow_slot = std::max<uint32_t>(rs->grow_slot, std::max<uint32_t>(2 * hc[kCtrSlots], hc[kCtrSlots] + 4096));
   if (flags & ERR_EVENT_OVERFLOW) rs->grow_ev = std::max<uint32_t>(rs->grow_ev, std::max<uint32_t>(2 * hc[kCtrEvents], hc[kCtrEvents] + 4096));
   if (flags & ERR_SPAN_OVERFLOW) rs->grow_span = std::max<uint32_t>(rs->grow_span, std::max<uint32_t>(2 * hc[kCtrRawSpans], hc[kCtrRawSpans] + 4096));
@@ -680,8 +664,7 @@ int cg_init(int device) {
   G.sm_count = prop.multiProcessorCount;
   CU(cudaStreamCreateWithFlags(&G.stream, cudaStreamNonBlocking));
   CU(cudaEventCreate(&G.ev0)); CU(cudaEventCreate(&G.ev1));
-  for (int i = 0; i < 5; i++) CU(cudaEventCreate(&G.pev[i]));
-  for (int i = 0; i < 8; i++) CU(cudaEventCreate(&G.pev_scan[i]));
+  for (cudaEvent_t& e : G.pev) CU(cudaEventCreate(&e));
   CU(cudaEventCreateWithFlags(&G.dig_order.ev, cudaEventDisableTiming));
 
   G.ready = true;
@@ -699,31 +682,32 @@ void cg_shutdown(void) {
   cudaFree(G.d_bytes_raw); cudaFree(G.d_off32); cudaFree(G.d_off64); cudaFree(G.d_words); cudaFree(G.d_dig[0]); cudaFree(G.d_dig[1]);
   free_shard_roots();
   cudaEventDestroy(G.dig_order.ev);
-  cudaEventDestroy(G.ev0); cudaEventDestroy(G.ev1); for (int i = 0; i < 5; i++) cudaEventDestroy(G.pev[i]); for (int i = 0; i < 8; i++) cudaEventDestroy(G.pev_scan[i]); cudaStreamDestroy(G.stream);
+  cudaEventDestroy(G.ev0); cudaEventDestroy(G.ev1); for (cudaEvent_t e : G.pev) cudaEventDestroy(e); cudaStreamDestroy(G.stream);
   G = Ctx();
 }
 
 int cg_set_profiling(int on) { G.profiling = on != 0; return CG_OK; }
 
+// device time between profiling events pev[from] and pev[to] of the most recent completed step
+static int elapsed_ms(int from, int to, float* out) {
+  *out = 0;
+  if (cudaEventElapsedTime(out, G.pev[from], G.pev[to]) == cudaSuccess) return CG_OK;
+  cudaGetLastError();
+  return fail(CG_ERR_CUDA, "profiling events not recorded / not complete");
+}
+
 int cg_last_kernel_ms(float out_ms[4]) {
-  // device time of scan / confirm / verify / finalize of the most recent *completed* scan step
+  // device time of scan_kernel / confirm_kernel + resolve / verify / finalize of the most recent *completed* scan step
   if (!G.ready || !out_ms) return fail(CG_ERR_INVALID_ARG, "not initialised");
-  for (int i = 0; i < 4; i++) { out_ms[i] = 0; if (cudaEventElapsedTime(&out_ms[i], G.pev[i], G.pev[i + 1]) != cudaSuccess) { cudaGetLastError(); return fail(CG_ERR_CUDA, "profiling events not recorded / not complete"); } }
-  // [0] = scan_kernel alone (summed over the pieces of the step), [1] = everything else before the VM (lookup, check, resolve)
-  float scan = 0;
-  for (uint32_t p = 0; p < G.prof_pieces; p++) { float t = 0; if (cudaEventElapsedTime(&t, G.pev_scan[2 * p], G.pev_scan[2 * p + 1]) == cudaSuccess) scan += t; else cudaGetLastError(); }
-  if (G.prof_pieces) { out_ms[1] += out_ms[0] - scan; out_ms[0] = scan; }
+  static const int ev[5] = {0, 1, 3, 4, 5};
+  for (int i = 0; i < 4; i++) if (int rc = elapsed_ms(ev[i], ev[i + 1], &out_ms[i])) return rc;
   return CG_OK;
 }
 
 int cg_last_tail_ms(float out_ms[2]) {
-  // confirm_kernel / resolve_kernel of the most recent completed step in profiling mode (all pieces)
+  // confirm_kernel / resolve_kernel of the most recent completed step in profiling mode
   if (!G.ready || !out_ms) return fail(CG_ERR_INVALID_ARG, "not initialised");
-  float scan = 0, pre = 0;
-  for (uint32_t p = 0; p < G.prof_pieces; p++) { float t = 0; if (cudaEventElapsedTime(&t, G.pev_scan[2 * p], G.pev_scan[2 * p + 1]) == cudaSuccess) scan += t; else cudaGetLastError(); }
-  out_ms[0] = out_ms[1] = 0;
-  if (cudaEventElapsedTime(&pre, G.pev[0], G.pev[1]) != cudaSuccess || cudaEventElapsedTime(&out_ms[1], G.pev[1], G.pev[2]) != cudaSuccess) { cudaGetLastError(); return fail(CG_ERR_CUDA, "profiling events not recorded / not complete"); }
-  out_ms[0] = pre - scan;
+  for (int i = 0; i < 2; i++) if (int rc = elapsed_ms(1 + i, 2 + i, &out_ms[i])) return rc;
   return CG_OK;
 }
 
@@ -734,7 +718,7 @@ int cg_scan_work_counters(const cg_ruleset* rs, uint32_t out16[16]) {
   if (!rs || !out16) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (!rs->work.counters) return fail(CG_ERR_INVALID_ARG, "no scan has run");
   memcpy(out16, rs->last_counters, 64);
-  if (!(rs->dev.debug_flags & 2u)) { out16[7] = rs->last_counters[kCtrPastRecheck]; out16[8] = out16[9] = 0; for (int i = 0; i < 4; i++) { out16[8] += rs->last_counters[kCtrFlagWords + i]; out16[9] += rs->last_counters[kCtrPairs + i]; } }   // grams past the recheck map, flag words, (gram, entry) pairs
+  if (!(rs->dev.debug_flags & 2u)) { out16[7] = rs->last_counters[kCtrPastRecheck]; out16[8] = rs->last_counters[kCtrFlagWords]; out16[9] = rs->last_counters[kCtrPairs]; }   // grams past the recheck map, flag words, (gram, entry) pairs
   return CG_OK;
 }
 
@@ -760,10 +744,7 @@ int cg_ruleset_create(const cg_rule* rules, uint32_t n_rules, uint32_t options, 
   for (uint32_t i = 0; i < n_rules; i++) { src[i] = RuleSrc{rules[i].source, rules[i].source_len, rules[i].flags}; rs->category[i] = rules[i].category; }
   ImageOptions io;
   io.stride = (options & 7u) == CG_OPT_STRIDE2 ? 2 : (options & 7u) == CG_OPT_STRIDE4 ? 4 : 0;
-  if (const char* e = getenv("CG_STRIDE")) io.stride = atoi(e);
-  if (const char* e = getenv("CG_BITMAP_KB")) io.bitmap_kb = (uint32_t)atoi(e);
   if (const char* e = getenv("CG_BLOOM2")) io.bloom2 = atoi(e);
-  if (const char* e = getenv("CG_MAX_KEYS")) io.max_keys = (uint32_t)atoi(e);
   std::string perr;
   if (!build_host_image(src.data(), n_rules, io, &rs->host, &perr)) return fail(CG_ERR_TOO_LARGE, perr);
   HostImage& H = rs->host;
@@ -806,8 +787,7 @@ int cg_ruleset_create(const cg_rule* rules, uint32_t n_rules, uint32_t options, 
     d.cf_fac_off = put(H.factor_words.data(), H.factor_words.size() * 4, 64);
     d.cf_bs_off = put(P.bytesets.data(), P.bytesets.size() * 4, 32);
     d.cf_bytes = (uint32_t)cf.size();
-    static const bool no_smem = getenv("CG_CONFIRM_SMEM") && atoi(getenv("CG_CONFIRM_SMEM")) == 0;
-    d.cf_resident = (!no_smem && d.cf_bytes <= kConfirmTableBudget) ? 1u : 0u;
+    d.cf_resident = d.cf_bytes <= kConfirmTableBudget ? 1u : 0u;
     const uint8_t* dcf = nullptr; if ((rc = upload(rs.get(), cf, &dcf, 16))) return rc;
     d.cf_image = dcf;
   }
@@ -824,8 +804,7 @@ int cg_ruleset_create(const cg_rule* rules, uint32_t n_rules, uint32_t options, 
   if ((rc = upload(rs.get(), H.alpha, &d.rule_alpha, 8))) return rc;
   { const uint64_t* bw = nullptr; if ((rc = upload(rs.get(), H.bit_words, &bw, 8))) return rc; d.bit_words = reinterpret_cast<const unsigned long long*>(bw); }
   if ((rc = upload(rs.get(), H.bit_off, &d.bit_off))) return rc;
-  { const uint64_t* fs = nullptr; if ((rc = upload(rs.get(), H.factor_skip, &fs, 8))) return rc; d.factor_skip = getenv("CG_NO_SKIP") ? nullptr : reinterpret_cast<const unsigned long long*>(fs); }
-  if (getenv("CG_NO_BITPROG")) d.bit_words = nullptr;
+  { const uint64_t* fs = nullptr; if ((rc = upload(rs.get(), H.factor_skip, &fs, 8))) return rc; d.factor_skip = reinterpret_cast<const unsigned long long*>(fs); }
   d.rule_policy = nullptr; d.rule_action = nullptr;
   {
     // the span resolver's tie-break: rank of every rule in (category, rule) order
@@ -869,8 +848,7 @@ int cg_scan_batch(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets,
   std::lock_guard<std::mutex> lk(g_mu);
   int rc;
   // large words-only batches: chunked, copies overlapped with the kernels (the hit list needs the per-batch slot tables)
-  static const bool no_chunks = getenv("CG_NO_CHUNKS") && atoi(getenv("CG_NO_CHUNKS"));
-  if (!no_chunks && !out_hits && out_words && n >= (1u << 16) && G.ready && rs && bytes && offsets) {
+  if (!out_hits && out_words && n >= (1u << 16) && G.ready && rs && bytes && offsets) {
     rc = scan_host_chunked(rs, bytes, offsets, n, out_words);
     if (rc < 0) return rc;
     if (rc == 0) {
@@ -937,8 +915,7 @@ int cg_scan_batch_views(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* of
 namespace {
 // -> CG_OK, an error, or 1 = take the general path (long message, large rule set, a queue overflowed)
 int scan_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* out_word, uint32_t* out_rules, uint32_t rules_cap, uint32_t* out_nrules) {
-  static const bool off_ = getenv("CG_ONE_FAST") && atoi(getenv("CG_ONE_FAST")) == 0;
-  if (off_ || !G.ready || !rs || (len && !bytes) || len > kOneBytes || rs->dev.rw > kOneRw - 2 || G.profiling) return 1;
+  if (!G.ready || !rs || (len && !bytes) || len > kOneBytes || rs->dev.rw > kOneRw - 2 || G.profiling) return 1;
   Staging& s = rs->one.io;
   const uint32_t off[2] = {0, len};
   const int rc = blocking_call(rs, kStepWords, 1, 0, rs->one.graphs, {}, s, [&](uint8_t* h) { return stage_texts(h, 256, bytes, off, 1); }, [&] {
@@ -1240,8 +1217,7 @@ int cg_scan_batch_device(cg_ruleset* rs, const void* d_bytes, const void* d_offs
   if (!d_out_words) return fail(CG_ERR_INVALID_ARG, "null argument");
   cudaStream_t st = stream ? (cudaStream_t)stream : G.stream;
   if (!n) return CG_OK;
-  static const bool use_graph = !(getenv("CG_NO_GRAPH") && atoi(getenv("CG_NO_GRAPH")));
-  return scan_device(rs, d_bytes, d_offsets, n, (uint64_t*)d_out_words, kStepWords, st, [](const ScanWork&) { return 0; }, use_graph && !G.profiling);
+  return scan_device(rs, d_bytes, d_offsets, n, (uint64_t*)d_out_words, kStepWords, st, [](const ScanWork&) { return 0; }, !G.profiling);
 }
 
 int cg_scan_join(cg_ruleset* rs, void* stream) {

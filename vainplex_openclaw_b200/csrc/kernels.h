@@ -44,7 +44,7 @@ struct DevRuleset {
   const uint32_t* sets;          // 6 words per unit set: ascii[4], range_off, n_ranges
   const uint16_t* set_ranges;    // inclusive lo,hi pairs
   const unsigned long long* bit_words; const uint32_t* bit_off;   // bitprog.h: 139 + 64 x rows words per eligible rule, bit_off[rule] = first word or 0xffffffff
-  const unsigned long long* factor_skip;   // 3 words per factor: elements the island matcher may skip | its state behind them (bitprog.h: island_test); nullptr = none
+  const unsigned long long* factor_skip;   // 3 words per factor: elements the island matcher may skip | its state behind them (bitprog.h: island_test)
   const uint32_t* rule_first;    // 8 words per rule: first-byte bitmap
   const uint32_t* rule_alpha;    // 8 words per rule: alphabet bitmap (bytes a match can contain)
   // verdict aggregation (policy-evaluator.ts:44-146, messageContains slice): per rule its policy (index in priority order,
@@ -71,7 +71,6 @@ struct ScanWork {
   uint32_t* event_pre;           // [event_cap]  policy mode: max units of a match before that factor (0xffff = unbounded)
   uint32_t* spans;               // [span_cap * 6] msg, rule, start_byte, end_byte, start16, end16
   uint32_t l1_cap, msg_cap, slot_cap, event_cap, span_cap;
-  uint32_t q_cap, q_slot;        // this launch's piece of fq (a step scans the batch in up to 4 pieces: q_slot 0..3) and its counter [kCtrFlagWords + q_slot]
   // span resolution (span-mode steps) and hit lists: [res_cap + 1] per message, [span_cap] per raw span
   uint64_t* words;               // [res_cap] result words of span-mode steps and of cg_policy_verdict_batch_device
   uint32_t* seg_cnt;             // raw spans per message (counted down again by the scatter)
@@ -114,8 +113,8 @@ enum : uint32_t {
   kCtrDigests = 21,              // spans to digest (redaction; 0 unless every output fits)
   kCtrSplice = 22,               // messages to splice (likewise)
   kCtrHits = 23,                 // (msg, rule) hits of the hit list
-  kCtrFlagWords = 24,            // [24..27] flag words queued, per piece of the batch (q_slot)
-  kCtrPairs = 28,                // [28..31] (gram, entry) pairs compared, per piece
+  kCtrFlagWords = 24,            // flag words queued (fq); 25..27 reserved, always zero
+  kCtrPairs = 28,                // (gram, entry) pairs compared; 29..31 reserved, always zero
 };
 constexpr uint32_t kScanPartials = 1024;         // blocks an exclusive scan uses at most
 constexpr uint32_t kConfirmTableBudget = 176u * 1024u;     // shared memory confirm_kernel may spend on its tables (beside 32 KB of rings)
@@ -126,7 +125,7 @@ constexpr uint64_t kWordIncomplete = ~0ull;      // result word of every message
 // d_bytes must be 16-byte aligned and readable up to 16 bytes past off[n].
 int launch_scan(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n,
                 uint64_t* d_words, int sm_count, cudaStream_t stream);
-// per piece of the batch: flag words -> grams -> recheck map -> table probes -> exact factors (confirm_kernel)
+// behind launch_scan: flag words -> grams -> recheck map -> table probes -> exact factors (confirm_kernel)
 int launch_confirm(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, int sm_count, cudaStream_t stream);
 // Per-message rule subsets (cg_ruleset_set_views): row v is rw words, bit r set = rule r is in view v; ids[m] = the view of
 // message m of the launch (an id >= n_views is the empty view).  Passed by value to resolve_views_kernel only.

@@ -164,8 +164,8 @@ __device__ __forceinline__ void trigger_chunk(const DevRuleset& rs, const ScanWo
   }
 }
 
-template <int NPROBE, int NTRIG, int BLOOM2, int NT>
-__global__ void __launch_bounds__(NT, 1)
+template <int NPROBE, int NTRIG, int BLOOM2>
+__global__ void __launch_bounds__(kScanThreads, 1)
 scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n,
             uint64_t* __restrict__ words) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -180,13 +180,13 @@ scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanW
     }
   }
   // while the image is in flight: result words start at zero (finalize_kernel fills in the messages that hit)
-  for (uint32_t i = blockIdx.x * NT + threadIdx.x; i < n; i += gridDim.x * NT) words[i] = 0ull;
+  for (uint32_t i = blockIdx.x * kScanThreads + threadIdx.x; i < n; i += gridDim.x * kScanThreads) words[i] = 0ull;
   ScanCtx ctx;
   ctx.bytes = bytes; ctx.begin = off[0]; ctx.end = off[n];
   const uint32_t begin = ctx.begin, end = ctx.end;
   mbar_wait(&bar, 0);
 
-  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = NT / 32;
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = kScanThreads / 32;
   uint32_t lt = (1u << lane) - 1u; const uint32_t FULL = 0xffffffffu;
   asm volatile("" : "+r"(lt));                // (loop invariants the compiler would otherwise recompute in every iteration of the hot loop)
   const uint32_t bm = smem_u32(smem);
@@ -287,13 +287,13 @@ scan_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ ScanW
   uint32_t h1 = 0, t1 = 0;       // the ring holds [h1, t1)
   auto append = [&](uint32_t k) {                           // k entries from the ring -> the queue
     uint32_t base = 0;
-    if (lane == 0) base = atomicAdd(&w.counters[kCtrFlagWords + w.q_slot], k);
+    if (lane == 0) base = atomicAdd(&w.counters[kCtrFlagWords], k);
     base = __shfl_sync(FULL, base, 0);
 #pragma unroll 1
     for (uint32_t j = lane; j < k; j += 32u) {
       uint32_t cw, aw;
       asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(cw), "=r"(aw) : "r"(ring1 + (((h1 + j) & (kRing - 1)) << 3)));
-      if (base + j < w.q_cap) w.fq[base + j] = make_uint2(cw, aw); else atomicOr(&w.counters[kCtrErrors], ERR_L1_OVERFLOW);
+      if (base + j < w.l1_cap) w.fq[base + j] = make_uint2(cw, aw); else atomicOr(&w.counters[kCtrErrors], ERR_L1_OVERFLOW);
     }
     h1 += k;
   };
@@ -345,7 +345,7 @@ struct SlotSink {
   __device__ void candidate(uint32_t r, uint32_t t0, uint32_t pre, uint32_t f) {
     // policy mode, rule with a bit-parallel program, ASCII island: RegExp.test around this occurrence is decided right here
     // (bitprog.h) -- no slot for a miss, no VM run for a hit
-    if (!want_spans && text && rs.bit_words) {
+    if (!want_spans && text) {
       const uint32_t bo = rs.bit_off[r];
       if (bo != kBitProgNone) {
         if (slot == 0xffffffffu) { const uint32_t s0 = *reinterpret_cast<volatile uint32_t*>(&w.slot_of_msg[msg]); if (s0 != 0xffffffffu && s0 < w.slot_cap && ((w.hit[(size_t)s0 * rs.rw + (r >> 5)] >> (r & 31)) & 1u)) return; }   // already a hit
@@ -559,7 +559,7 @@ confirm_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ Sc
   extern __shared__ __align__(16) uint8_t cf_smem[];          // [pair rings][gram rings][occurrence buffers][tables, when resident]
   __shared__ uint32_t cta_ctr[3];                             // flagged grams, grams past the recheck map, pairs: one atomic each per CTA
   const uint32_t cstep16 = cstep * 16u;
-  const uint32_t nq = (rs.debug_flags & 1u) ? 0u : min(w.counters[kCtrFlagWords + w.q_slot], w.q_cap);
+  const uint32_t nq = (rs.debug_flags & 1u) ? 0u : min(w.counters[kCtrFlagWords], w.l1_cap);
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5, FULL = 0xffffffffu, lt = (1u << lane) - 1u;
   uint2* pring = reinterpret_cast<uint2*>(cf_smem) + warp * kCfRing;
   uint32_t* ring = reinterpret_cast<uint32_t*>(cf_smem + (size_t)wpb * kCfRing * 8) + warp * kCfRing;
@@ -607,7 +607,7 @@ confirm_kernel(const __grid_constant__ DevRuleset rs, const __grid_constant__ Sc
   if (threadIdx.x == 0) {
     if (cta_ctr[0]) atomicAdd(&w.counters[kCtrFlagged], cta_ctr[0]);
     if (cta_ctr[1]) atomicAdd(&w.counters[kCtrPastRecheck], cta_ctr[1]);
-    if (cta_ctr[2]) atomicAdd(&w.counters[kCtrPairs + w.q_slot], cta_ctr[2]);
+    if (cta_ctr[2]) atomicAdd(&w.counters[kCtrPairs], cta_ctr[2]);
   }
 }
 
@@ -625,13 +625,14 @@ struct InView {
 
 template <class Filter>
 __device__ __forceinline__ void resolve_occurrences(const DevRuleset& rs, const ScanWork& w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off,
-                                                    uint32_t n, int want_spans, uint32_t spread, const Filter& filter) {
+                                                    uint32_t n, int want_spans, const Filter& filter) {
   const uint32_t n1 = min(w.counters[kCtrConfirmed], w.l1_cap);
   const uint32_t stride = gridDim.x * blockDim.x, tid = blockIdx.x * blockDim.x + threadIdx.x;
   // Occurrences take different paths of very different lengths (direct hit, island matcher of 5 .. 96 steps, slot allocation),
   // and a warp executes the union of its lanes' paths one dependent instruction after the other: with 32 occurrences per warp
   // a few warps run long dependent chains while most warp slots stay empty.  So only every `spread`-th lane takes an
-  // occurrence: more warps, each with a short chain.
+  // occurrence: more warps, each with a short chain (4: what fits one wave of resident warps).
+  constexpr uint32_t spread = 4;
   for (uint32_t i = tid / spread; i < n1 && tid % spread == 0; i += stride / spread) {
     const uint32_t pos = w.l1_pos[i], f = w.l1_fac[i];
     const uint32_t msg = message_of(off, n, pos);
@@ -648,16 +649,16 @@ __device__ __forceinline__ void resolve_occurrences(const DevRuleset& rs, const 
 }
 
 __global__ void __launch_bounds__(256, 4)
-resolve_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, int want_spans, uint32_t spread) {
-  resolve_occurrences(rs, w, bytes, off, n, want_spans, spread, AllRules{});
+resolve_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, int want_spans) {
+  resolve_occurrences(rs, w, bytes, off, n, want_spans, AllRules{});
 }
 // the same with the views of cg_*_views: the table is an argument of its own (DevRuleset / ScanWork keep their layout).  Two
-// CTAs per SM, not four: under resolve_kernel's 64-register cap this instantiation spills; at this bound it takes 90
+// CTAs per SM, not four: under resolve_kernel's 64-register cap this instantiation spills; at this bound it takes 92
 // registers and spills nothing
 __global__ void __launch_bounds__(256, 2)
-resolve_views_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, int want_spans, uint32_t spread,
+resolve_views_kernel(DevRuleset rs, ScanWork w, const uint8_t* __restrict__ bytes, const uint32_t* __restrict__ off, uint32_t n, int want_spans,
                      ViewTable views) {
-  resolve_occurrences(rs, w, bytes, off, n, want_spans, spread, InView{views, rs.rw});
+  resolve_occurrences(rs, w, bytes, off, n, want_spans, InView{views, rs.rw});
 }
 
 // ------------------------------------------------------------------------------------------
@@ -899,12 +900,10 @@ __global__ void __launch_bounds__(256) hit_emit_kernel(DevRuleset rs, ScanWork w
 // launchers
 // ------------------------------------------------------------------------------------------
 #define CG_FOR_SCAN_VARIANTS(X) X(1, 0, 0) X(1, 1, 0) X(1, 2, 0) X(2, 0, 0) X(2, 1, 0) X(2, 2, 0) X(1, 0, 1) X(1, 1, 1) X(1, 2, 1) X(2, 0, 1) X(2, 1, 1) X(2, 2, 1)
-static int scan_threads() { static int t = 0; if (!t) { t = kScanThreads; if (const char* e = getenv("CG_SCAN_THREADS")) { int v = atoi(e); if (v == 512 || v == 768 || v == 1024) t = v; } } return t; }
 void prepare_scan_kernels() {
   int dev = 0, optin = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   const int kMaxSmem = (optin > 0 ? optin : 227 * 1024) - 1024;     // leave room for the kernels' static shared memory
-#define CG_PREP(P, T, B) cudaFuncSetAttribute(scan_kernel<P, T, B, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem); \
-  cudaFuncSetAttribute(scan_kernel<P, T, B, 768>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem); cudaFuncSetAttribute(scan_kernel<P, T, B, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+#define CG_PREP(P, T, B) cudaFuncSetAttribute(scan_kernel<P, T, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
   CG_FOR_SCAN_VARIANTS(CG_PREP)
 #undef CG_PREP
   cudaFuncSetAttribute(confirm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kCfRingBytes + kConfirmTableBudget));
@@ -925,11 +924,8 @@ int launch_scan(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes,
   const size_t smem = (size_t)rs.image_bytes + kScanRingBytes;
   // the scanned range is only known on the device (off[0] .. off[n]); a warp tile is 1 KB, messages are rarely shorter than 16
   const uint32_t grid = scan_grid(n, sm_count);
-  const int np = rs.stride == 2 ? 2 : 1, nt = (int)rs.n_trig, bl = rs.bloom2 ? 1 : 0, th = scan_threads();
-#define CG_LAUNCH(P, T, B) if (np == P && nt == T && bl == B) { \
-    if (th == 1024) scan_kernel<P, T, B, 1024><<<grid, 1024, smem, stream>>>(rs, w, d_bytes, d_off, n, d_words); \
-    else if (th == 768) scan_kernel<P, T, B, 768><<<grid, 768, smem, stream>>>(rs, w, d_bytes, d_off, n, d_words); \
-    else scan_kernel<P, T, B, 512><<<grid, 512, smem, stream>>>(rs, w, d_bytes, d_off, n, d_words); }
+  const int np = rs.stride == 2 ? 2 : 1, nt = (int)rs.n_trig, bl = rs.bloom2 ? 1 : 0;
+#define CG_LAUNCH(P, T, B) if (np == P && nt == T && bl == B) scan_kernel<P, T, B><<<grid, kScanThreads, smem, stream>>>(rs, w, d_bytes, d_off, n, d_words);
   CG_FOR_SCAN_VARIANTS(CG_LAUNCH)
 #undef CG_LAUNCH
   return 1;
@@ -937,7 +933,7 @@ int launch_scan(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes,
 
 int launch_confirm(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, int sm_count, cudaStream_t stream) {
   if (n == 0) return 0;
-  const uint32_t cstep = scan_grid(n, sm_count) * (uint32_t)(scan_threads() / 32) * kTileChunks;       // (the queue's chunk numbers are decoded with the scan's grid)
+  const uint32_t cstep = scan_grid(n, sm_count) * (uint32_t)(kScanThreads / 32) * kTileChunks;       // (the queue's chunk numbers are decoded with the scan's grid)
   const size_t smem = (size_t)kCfRingBytes + (rs.cf_resident ? rs.cf_bytes : 0u);
   if (rs.stride == 2) confirm_kernel<2><<<scan_grid(n, sm_count), kCfThreads, smem, stream>>>(rs, w, d_bytes, d_off, n, cstep);
   else confirm_kernel<1><<<scan_grid(n, sm_count), kCfThreads, smem, stream>>>(rs, w, d_bytes, d_off, n, cstep);
@@ -946,17 +942,15 @@ int launch_confirm(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_byt
 int launch_resolve(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off, uint32_t n, bool want_spans, int sm_count, cudaStream_t stream,
                    const ViewTable* views) {
   if (n == 0) return 0;
-  static const uint32_t spread = [] { const char* e = getenv("CG_RESOLVE_SPREAD"); const int v = e ? atoi(e) : 4; return (uint32_t)(v == 1 || v == 2 || v == 4 || v == 8 || v == 16 || v == 32 ? v : 4); }();
-  if (views) resolve_views_kernel<<<sm_count * 8, 256, 0, stream>>>(rs, w, d_bytes, d_off, n, want_spans ? 1 : 0, spread, *views);
-  else resolve_kernel<<<sm_count * 8, 256, 0, stream>>>(rs, w, d_bytes, d_off, n, want_spans ? 1 : 0, spread);
+  if (views) resolve_views_kernel<<<sm_count * 8, 256, 0, stream>>>(rs, w, d_bytes, d_off, n, want_spans ? 1 : 0, *views);
+  else resolve_kernel<<<sm_count * 8, 256, 0, stream>>>(rs, w, d_bytes, d_off, n, want_spans ? 1 : 0);
   return 1;
 }
 
 int launch_verify(const DevRuleset& rs, const ScanWork& w, const uint8_t* d_bytes, const uint32_t* d_off,
                   bool want_spans, int sm_count, cudaStream_t stream, int ctas_per_sm) {
   int k = 1;
-  static const int forced = [] { const char* e = getenv("CG_VERIFY_CTAS"); const int v = e ? atoi(e) : 0; return v >= 1 && v <= kVerifyCtasPerSm ? v : 0; }();       // (experiments)
-  const int ctas = forced ? forced : (ctas_per_sm >= 1 && ctas_per_sm <= kVerifyCtasPerSm ? ctas_per_sm : kVerifyCtasPerSm);
+  const int ctas = ctas_per_sm >= 1 && ctas_per_sm <= kVerifyCtasPerSm ? ctas_per_sm : kVerifyCtasPerSm;
   if (want_spans) {
     verify_small_kernel<true><<<sm_count * ctas, kVerifyBlock, kVerifySmem, stream>>>(rs, w, d_bytes, d_off);
   } else {
