@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libopenclaw_gov.so")
 SOURCES = ["capi.cu", "scan_kernels.cu", "span_resolve.cu", "sha256_kernels.cu", "policy_eval.cu", "policy_eval_one.cu", "rulec.cpp", "ruleset_image.cpp"]
-HEADERS = ["kernels.h", "policy_eval.h", "rulec.h", "pike_vm.h", "gram_filter.h", "ruleset_image.h", os.path.join("..", "..", "include", "openclaw_gov.h")]
+HEADERS = ["dev_buffer.h", "kernels.h", "policy_eval.h", "rulec.h", "pike_vm.h", "gram_filter.h", "ruleset_image.h", os.path.join("..", "..", "include", "openclaw_gov.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared"]
 

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "../../include/openclaw_gov.h"
+#include "dev_buffer.h"
 #include "kernels.h"
 #include "rulec.h"
 #include "ruleset_image.h"
@@ -38,33 +39,29 @@ struct Ctx {
   bool profiling = false;
   cg_stats stats{};
   // grow-only staging in HBM
-  uint8_t* d_bytes = nullptr; size_t cap_bytes = 0; uint8_t* d_bytes_raw = nullptr;   // d_bytes = d_bytes_raw + 256: readable in front (sha_words)
-  uint32_t* d_off32 = nullptr; size_t cap_off32 = 0;
-  uint64_t* d_off64 = nullptr; size_t cap_off64 = 0;
-  uint64_t* d_words = nullptr; size_t cap_words = 0;
-  uint32_t* d_dig[2] = {nullptr, nullptr}; size_t cap_dig[2] = {0, 0};
+  Buf<uint8_t, false, 256> d_bytes;   // message / leaf bytes: 256 zero bytes readable in front (sha_words)
+  DevBuf<uint32_t> d_off32;
+  DevBuf<uint64_t> d_off64, d_words;
+  DevBuf<uint32_t> d_dig[2];
   IssueOrder dig_order;           // the calls that use d_dig, on the library's stream or the caller's
   // chunked host-buffer scans: H2D of chunk c+1 and D2H of chunk c-1 overlap the kernels of chunk c
   static constexpr int kChunks = 8;
-  cudaStream_t s_h2d = nullptr, s_d2h = nullptr; cudaEvent_t e_h2d[kChunks] = {}, e_done[kChunks] = {}; uint32_t* h_chunk_counters = nullptr;
+  cudaStream_t s_h2d = nullptr, s_d2h = nullptr; cudaEvent_t e_h2d[kChunks] = {}, e_done[kChunks] = {}; HostBuf<uint32_t> h_chunk_counters;
   // cg_find_matches_batch / cg_redact_batch / cg_policy_verdict_batch staging (grow-only)
-  cg_span* d_spans = nullptr; size_t cap_spans = 0;
-  uint8_t* d_redact_out = nullptr; size_t cap_redact_out = 0; uint32_t* d_redact_meta = nullptr; size_t cap_redact_meta = 0;
-  uint32_t* d_verdicts = nullptr; size_t cap_verdicts = 0;
-  uint32_t* d_hits = nullptr; size_t cap_hits = 0;          // cg_scan_batch's hit list: [count][(msg, rule) pairs]
-  uint8_t* d_views = nullptr; size_t cap_views = 0;         // the host-buffer *_views calls' view ids, staged beside the offsets
+  DevBuf<cg_span> d_spans;
+  DevBuf<uint8_t> d_redact_out; DevBuf<uint32_t> d_redact_meta;
+  DevBuf<uint32_t> d_verdicts;
+  DevBuf<uint32_t> d_hits;        // cg_scan_batch's hit list: [count][(msg, rule) pairs]
+  DevBuf<uint8_t> d_views;        // the host-buffer *_views calls' view ids, staged beside the offsets
   // cg_policy_eval_batch staging: text roles, context offsets, atom rows, [count][(ctx, rule) pairs]
-  uint8_t* d_proles = nullptr; size_t cap_proles = 0;
-  uint32_t* d_pctx = nullptr; size_t cap_pctx = 0;
-  uint32_t* d_patoms = nullptr; size_t cap_patoms = 0;
-  uint32_t* d_pmatch = nullptr; size_t cap_pmatch = 0;
-} G;
+  DevBuf<uint8_t> d_proles;
+  DevBuf<uint32_t> d_pctx, d_patoms, d_pmatch;
+  DevBuf<uint32_t> d_roots;       // cg_merkle_root_sharded_device: every rank's block roots (cg_comm_destroy frees them)
+};
+// never destroyed: no CUDA call may run from a static destructor at process exit (cg_shutdown frees what G holds)
+Ctx& G = *new Ctx;
 
 int fail(int code, const std::string& msg) { g_err = msg; return code; }
-int cuda_fail(cudaError_t e, const char* what) {
-  g_err = std::string(what) + ": " + cudaGetErrorString(e);
-  return CG_ERR_CUDA;
-}
 #define CU(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) return cuda_fail(_e, #x); } while (0)
 int require_ready() { return G.ready ? CG_OK : fail(CG_ERR_NOT_INITIALIZED, "cg_init has not been called (or no CUDA device)"); }
 void count_launches(int k) { G.stats.kernel_launches += k; }
@@ -94,34 +91,7 @@ struct NcclApi {
   int (*AllGather)(const void*, void*, size_t, int, void*, cudaStream_t) = nullptr;
   int (*CommDestroy)(void*) = nullptr;
   const char* (*GetErrorString)(int) = nullptr;
-  uint32_t* d_roots = nullptr; size_t cap_roots = 0;     // cg_merkle_root_sharded_device: every rank's block roots (grow-only)
 } g_nccl;
-void free_shard_roots() { if (g_nccl.d_roots) cudaFree(g_nccl.d_roots); g_nccl.d_roots = nullptr; g_nccl.cap_roots = 0; }
-
-template <typename T>
-int grow(T** p, size_t* cap, size_t need_elems) {
-  if (need_elems <= *cap && *p) return CG_OK;
-  if (*p) cudaFree(*p);
-  *p = nullptr; *cap = 0;
-  size_t n = need_elems + need_elems / 4 + 64;
-  cudaError_t e = cudaMalloc((void**)p, n * sizeof(T));
-  if (e != cudaSuccess) { *p = nullptr; return cuda_fail(e, "cudaMalloc"); }
-  *cap = n;
-  return CG_OK;
-}
-
-// the staging buffer for message / leaf bytes: 256 readable bytes in front of it and 64 + slack behind what is asked for
-int grow_bytes(size_t need) {
-  if (need <= G.cap_bytes && G.d_bytes) return CG_OK;
-  if (G.d_bytes_raw) cudaFree(G.d_bytes_raw);
-  G.d_bytes_raw = G.d_bytes = nullptr; G.cap_bytes = 0;
-  const size_t n = need + need / 4 + 64;
-  cudaError_t e = cudaMalloc((void**)&G.d_bytes_raw, n + 512);
-  if (e != cudaSuccess) { G.d_bytes_raw = nullptr; return cuda_fail(e, "cudaMalloc"); }
-  cudaMemset(G.d_bytes_raw, 0, 256);
-  G.d_bytes = G.d_bytes_raw + 256; G.cap_bytes = n;
-  return CG_OK;
-}
 
 // The single-message staging block, host (pinned) and device: [offsets, 256 B][message bytes][64 zero bytes] in (kOneIn),
 // [word][counters][hit row] out (kOneOut).  The span calls stage their input in their own block (kFew*) and keep the packed
@@ -147,14 +117,10 @@ static_assert(4 * (kPeOneTexts + 1) <= kPeRolesAt && kPeOneTexts <= 256 && kPeTe
 // by the family's first call
 struct Staging {
   const size_t host_bytes, dev_bytes;
-  uint8_t* h = nullptr; uint8_t* d = nullptr;
-  Staging(size_t host, size_t dev) : host_bytes(host), dev_bytes(dev) {}
-  Staging(const Staging&) = delete;
-  Staging& operator=(const Staging&) = delete;
-  ~Staging() { if (h) cudaFreeHost(h); cudaFree(d); }
+  HostBuf<uint8_t> h{}; DevBuf<uint8_t> d{};
   int ensure() {
-    if (!h) { CU(cudaMallocHost((void**)&h, host_bytes)); memset(h, 0, host_bytes); }
-    if (!d) { CU(cudaMalloc((void**)&d, dev_bytes)); CU(cudaMemset(d, 0, dev_bytes)); }
+    if (!h.get()) { if (int rc = h.alloc(host_bytes)) return rc; memset(h.get(), 0, host_bytes); }
+    if (!d.get()) { if (int rc = d.alloc(dev_bytes)) return rc; CU(cudaMemset(d.get(), 0, dev_bytes)); }
     return CG_OK;
   }
 };
@@ -175,19 +141,42 @@ struct GraphCache {
 
 }  // namespace
 
+int cg::cuda_fail(cudaError_t e, const char* what) {
+  g_err = std::string(what) + ": " + cudaGetErrorString(e);
+  return CG_ERR_CUDA;
+}
 struct cg_ruleset {
   HostImage host;
   std::vector<uint32_t> category;
   DevRuleset dev{};
-  std::vector<void*> allocs;
+  std::vector<DevBuf<uint8_t>> allocs;     // the device tables of dev and work (upload)
+  DevBuf<uint8_t> rule_policy, rule_action;    // dev.rule_policy / dev.rule_action (cg_ruleset_set_policy)
   uint32_t n_sets = 0, program_words = 0;
-  ScanWork work{};
+  // the step scratch: ScanWork's buffers, grouped by the capacity that sizes them (prepare_step)
+  struct {
+    DevBuf<uint32_t> counters, persist;      // allocated once
+    uint32_t msg_cap = 0; DevBuf<uint32_t> slot_of_msg;
+    uint32_t l1_cap = 0; DevBuf<uint32_t> l1_pos, l1_fac; DevBuf<uint2> fq;
+    uint32_t slot_cap = 0; DevBuf<uint32_t> slot_msg, cand, hit;
+    uint32_t event_cap = 0; DevBuf<uint2> events; DevBuf<uint32_t> heavy_idx, event_pos, event_pre;
+    uint32_t span_cap = 0; DevBuf<uint32_t> spans, sp_start, sp_len, sp_cat; DevBuf<uint4> sorted, sort_tmp;
+    uint32_t res_cap = 0; DevBuf<uint64_t> words, out_len, out_off, scan_part; DevBuf<uint32_t> seg_cnt, seg_begin, kept_cnt, kept_begin;
+    void view(ScanWork& w) const {    // (w's rule tables stay as they are)
+      w.counters = counters.get(); w.persist = persist.get(); w.msg_cap = msg_cap; w.slot_of_msg = slot_of_msg.get();
+      w.l1_cap = l1_cap; w.l1_pos = l1_pos.get(); w.l1_fac = l1_fac.get(); w.fq = fq.get(); w.slot_cap = slot_cap; w.slot_msg = slot_msg.get(); w.cand = cand.get(); w.hit = hit.get();
+      w.event_cap = event_cap; w.events = events.get(); w.heavy_idx = heavy_idx.get(); w.event_pos = event_pos.get(); w.event_pre = event_pre.get();
+      w.span_cap = span_cap; w.spans = spans.get(); w.sorted = sorted.get(); w.sort_tmp = sort_tmp.get(); w.sp_start = sp_start.get(); w.sp_len = sp_len.get(); w.sp_cat = sp_cat.get();
+      w.res_cap = res_cap; w.words = words.get(); w.out_len = out_len.get(); w.out_off = out_off.get(); w.seg_cnt = seg_cnt.get(); w.seg_begin = seg_begin.get();
+      w.kept_cnt = kept_cnt.get(); w.kept_begin = kept_begin.get(); w.scan_part = scan_part.get();
+    }
+  } scratch;
+  ScanWork work{};                // scratch as the launchers take it (by value): rebuilt by every prepare_step that grows it
   IssueOrder order;               // the calls that use work and one, on the library's stream or the caller's
   uint64_t seq = 0;               // device-path batches issued so far
   // device path: every batch's counters are mirrored into a ring of pinned slots, so that a queue overflow (results of
   // that batch marked incomplete by finalize_kernel) is seen by the next call / by cg_scan_join and the scratch grows
   static constexpr int kMirror = 16;
-  uint32_t* h_counters = nullptr; cudaEvent_t e_cnt[kMirror] = {}; bool cnt_pending[kMirror] = {};
+  HostBuf<uint32_t> h_counters; cudaEvent_t e_cnt[kMirror] = {}; bool cnt_pending[kMirror] = {};
   uint32_t grow_l1 = 0, grow_slot = 0, grow_ev = 0, grow_span = 0;     // capacities learnt from overflows
   uint32_t sticky_flags = 0;      // error flags of batches since the last cg_scan_join
   uint32_t sticky_status = 0;     // 1 << span resolution status (kResolve*) of batches since the last cg_scan_join
@@ -209,77 +198,37 @@ struct cg_ruleset {
   // cg_policy_eval_one: the step + policy_eval_one_kernel per (text count, prog_gen) (a graph holds PolicyTable by value)
   struct { Staging io{kPeIn + kPeOut, kPeIn + kPeOut}; GraphCache<std::tuple<uint32_t, uint64_t>, 8> graphs; } pone;
   // cg_ruleset_set_views: n_views rows of dev.rw words in HBM (bit r of row v = rule r is in view v); none before the first call
-  uint32_t* view_rows = nullptr; uint32_t n_views = 0;
+  DevBuf<uint32_t> view_rows; uint32_t n_views = 0;
   // cg_ruleset_set_policy_program: the program's words and one rule record per program rule (kernels.h PolicyTable) in HBM;
   // prog_gen advances with every program set (a captured graph holds the tables by value)
-  uint32_t* prog_ops = nullptr; uint4* prog_rules = nullptr; uint32_t prog_n_rules = 0, prog_n_atoms = 0;
+  DevBuf<uint32_t> prog_ops; DevBuf<uint4> prog_rules; uint32_t prog_n_rules = 0, prog_n_atoms = 0;
   uint64_t prog_gen = 0;
-  ~cg_ruleset() {                 // (the graph caches and staging blocks release themselves)
-    cudaFree(view_rows); cudaFree(prog_ops); cudaFree(prog_rules);
-    if (h_counters) cudaFreeHost(h_counters);
+  ~cg_ruleset() {                 // (the buffers, graph caches and staging blocks release themselves)
     for (auto& e : e_cnt) if (e) cudaEventDestroy(e);
     if (order.ev) cudaEventDestroy(order.ev);
-    for (void* p : allocs) cudaFree(p);
-    cudaFree(work.heavy_idx); cudaFree(work.l1_pos); cudaFree(work.l1_fac); cudaFree(work.fq); cudaFree(work.slot_of_msg);
-    cudaFree(work.counters); cudaFree(work.persist); cudaFree(work.slot_msg); cudaFree(work.cand); cudaFree(work.hit); cudaFree(work.events); cudaFree(work.event_pos); cudaFree(work.event_pre); cudaFree(work.spans);
-    cudaFree(work.words); cudaFree(work.seg_cnt); cudaFree(work.seg_begin); cudaFree(work.kept_cnt); cudaFree(work.kept_begin); cudaFree(work.out_len); cudaFree(work.out_off);
-    cudaFree(work.sorted); cudaFree(work.sort_tmp); cudaFree(work.sp_start); cudaFree(work.sp_len); cudaFree(work.sp_cat); cudaFree(work.scan_part);
   }
 };
 
 namespace {
 
+// v and pad_elems zero elements behind it into one more of the rule set's tables, or into *into (allocated anew) -> *out
 template <typename T>
-int upload(cg_ruleset* rs, const std::vector<T>& v, const T** out, size_t pad_elems = 4) {
-  void* d = nullptr;
-  size_t bytes = (v.size() + pad_elems) * sizeof(T);
-  CU(cudaMalloc(&d, bytes));
-  rs->allocs.push_back(d);
-  CU(cudaMemset(d, 0, bytes));
-  if (!v.empty()) CU(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-  *out = reinterpret_cast<const T*>(d);
+int upload(cg_ruleset* rs, const std::vector<T>& v, const T** out, size_t pad_elems = 4, DevBuf<uint8_t>* into = nullptr) {
+  DevBuf<uint8_t>& d = into ? *into : rs->allocs.emplace_back();
+  const size_t bytes = (v.size() + pad_elems) * sizeof(T);
+  if (int rc = d.alloc(bytes)) return rc;
+  CU(cudaMemset(d.get(), 0, bytes));
+  if (!v.empty()) CU(cudaMemcpy(d.get(), v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+  *out = reinterpret_cast<const T*>(d.get());
   return CG_OK;
 }
-
-// (res_msgs: messages the span resolver must have room for; 0 for a step without spans)
-int ensure_work(cg_ruleset* rs, ScanWork& w, uint32_t n_msgs, uint32_t l1_cap, uint32_t slot_cap, uint32_t event_cap, uint32_t span_cap, uint32_t res_msgs) {
-  rs->scratch_gen++;                                        // (prepare_step calls this only when some buffer must grow)
-  if (!w.counters) { CU(cudaMalloc((void**)&w.counters, kCounterWords * sizeof(uint32_t))); CU(cudaMalloc((void**)&w.persist, 16)); CU(cudaMemset(w.persist, 0, 16)); CU(cudaDeviceSynchronize()); }
-  if (n_msgs > w.msg_cap) { cudaFree(w.slot_of_msg); w.slot_of_msg = nullptr; w.msg_cap = 0; CU(cudaMalloc((void**)&w.slot_of_msg, (size_t)n_msgs * 4)); w.msg_cap = n_msgs; }
-  if (l1_cap > w.l1_cap) {
-    cudaFree(w.l1_pos); cudaFree(w.l1_fac); cudaFree(w.fq); w.l1_pos = w.l1_fac = nullptr; w.fq = nullptr; w.l1_cap = 0;
-    CU(cudaMalloc((void**)&w.l1_pos, (size_t)l1_cap * 4)); CU(cudaMalloc((void**)&w.l1_fac, (size_t)l1_cap * 4)); CU(cudaMalloc((void**)&w.fq, (size_t)l1_cap * 8));
-    w.l1_cap = l1_cap;
-  }
-  if (slot_cap > w.slot_cap) {
-    cudaFree(w.slot_msg); cudaFree(w.cand); cudaFree(w.hit); w.slot_msg = w.cand = w.hit = nullptr; w.slot_cap = 0;
-    size_t rw = rs->dev.rw ? rs->dev.rw : 1;
-    CU(cudaMalloc((void**)&w.slot_msg, (size_t)slot_cap * 4));
-    CU(cudaMalloc((void**)&w.cand, (size_t)slot_cap * rw * 4));
-    CU(cudaMalloc((void**)&w.hit, (size_t)slot_cap * rw * 4));
-    // rows start out zero and every step clears the ones it used (reset_kernel)
-    CU(cudaMemset(w.cand, 0, (size_t)slot_cap * rw * 4)); CU(cudaMemset(w.hit, 0, (size_t)slot_cap * rw * 4)); CU(cudaMemset(w.persist, 0, 16)); CU(cudaDeviceSynchronize());
-    w.slot_cap = slot_cap;
-  }
-  if (event_cap > w.event_cap) { cudaFree(w.events); cudaFree(w.event_pos); cudaFree(w.event_pre); cudaFree(w.heavy_idx); w.events = nullptr; w.event_pos = w.event_pre = w.heavy_idx = nullptr; w.event_cap = 0; CU(cudaMalloc((void**)&w.events, (size_t)event_cap * sizeof(uint2))); CU(cudaMalloc((void**)&w.heavy_idx, (size_t)event_cap * 4)); CU(cudaMalloc((void**)&w.event_pos, (size_t)event_cap * 4)); CU(cudaMalloc((void**)&w.event_pre, (size_t)event_cap * 4)); w.event_cap = event_cap; }
-  if (span_cap > w.span_cap) {
-    cudaFree(w.spans); cudaFree(w.sorted); cudaFree(w.sort_tmp); cudaFree(w.sp_start); cudaFree(w.sp_len); cudaFree(w.sp_cat);
-    w.spans = w.sp_start = w.sp_len = w.sp_cat = nullptr; w.sorted = w.sort_tmp = nullptr; w.span_cap = 0;
-    CU(cudaMalloc((void**)&w.spans, (size_t)span_cap * 24));
-    CU(cudaMalloc((void**)&w.sorted, (size_t)span_cap * 16)); CU(cudaMalloc((void**)&w.sort_tmp, (size_t)span_cap * 16));
-    CU(cudaMalloc((void**)&w.sp_start, (size_t)span_cap * 4)); CU(cudaMalloc((void**)&w.sp_len, (size_t)span_cap * 4)); CU(cudaMalloc((void**)&w.sp_cat, (size_t)span_cap * 4));
-    w.span_cap = span_cap;
-  }
-  if (res_msgs > w.res_cap || (res_msgs && !w.scan_part)) {
-    cudaFree(w.words); cudaFree(w.seg_cnt); cudaFree(w.seg_begin); cudaFree(w.kept_cnt); cudaFree(w.kept_begin); cudaFree(w.out_len); cudaFree(w.out_off);
-    w.words = w.out_len = w.out_off = nullptr; w.seg_cnt = w.seg_begin = w.kept_cnt = w.kept_begin = nullptr; w.res_cap = 0;
-    const size_t m = (size_t)res_msgs + 1;
-    CU(cudaMalloc((void**)&w.words, m * 8)); CU(cudaMalloc((void**)&w.out_len, m * 8)); CU(cudaMalloc((void**)&w.out_off, m * 8));
-    CU(cudaMalloc((void**)&w.seg_cnt, m * 4)); CU(cudaMalloc((void**)&w.seg_begin, m * 4)); CU(cudaMalloc((void**)&w.kept_cnt, m * 4)); CU(cudaMalloc((void**)&w.kept_begin, m * 4));
-    if (!w.scan_part) CU(cudaMalloc((void**)&w.scan_part, (size_t)kScanPartials * 8));
-    w.res_cap = res_msgs;
-  }
-  return CG_OK;
+// one group of scratch buffers at n elements each: all of them freed, then each allocated
+template <typename... B>
+int regrow(size_t n, B&... b) {
+  (b.reset(), ...);
+  int rc = CG_OK;
+  ((rc = rc ? rc : b.alloc(n)), ...);
+  return rc;
 }
 
 // What a step computes: result words only; a policy step whose per-message scratch a hit list or verdicts read afterwards;
@@ -332,7 +281,34 @@ int prepare_step(cg_ruleset* rs, uint32_t n, StepKind kind, cudaStream_t st, uin
   const uint32_t res = kind != kStepWords ? std::max(n, res_min) : 0;
   if (n <= w.msg_cap && l1 <= w.l1_cap && slot <= w.slot_cap && ev <= w.event_cap && span <= w.span_cap && res <= w.res_cap) return CG_OK;
   CU(cudaStreamSynchronize(st));
-  return ensure_work(rs, rs->work, n, l1, slot, ev, span, res);
+  rs->scratch_gen++;
+  // a group's capacity is recorded once all its buffers are there; rs->work is rebuilt on every return (no freed buffer in it)
+  auto& s = rs->scratch; int rc;
+  struct View { cg_ruleset* rs; ~View() { rs->scratch.view(rs->work); } } view{rs};
+  if (!s.counters.get()) { if ((rc = s.counters.alloc(kCounterWords)) || (rc = s.persist.alloc(4))) return rc; CU(cudaMemset(s.persist.get(), 0, 16)); CU(cudaDeviceSynchronize()); }
+  if (n > s.msg_cap) { s.msg_cap = 0; if ((rc = regrow(n, s.slot_of_msg))) return rc; s.msg_cap = n; }
+  if (l1 > s.l1_cap) { s.l1_cap = 0; if ((rc = regrow(l1, s.l1_pos, s.l1_fac, s.fq))) return rc; s.l1_cap = l1; }
+  if (slot > s.slot_cap) {
+    const size_t rows = (size_t)slot * (rs->dev.rw ? rs->dev.rw : 1);
+    s.slot_cap = 0; s.slot_msg.reset();
+    if ((rc = regrow(rows, s.cand, s.hit)) || (rc = s.slot_msg.alloc(slot))) return rc;
+    // rows start out zero and every step clears the ones it used (reset_kernel)
+    CU(cudaMemset(s.cand.get(), 0, rows * 4)); CU(cudaMemset(s.hit.get(), 0, rows * 4)); CU(cudaMemset(s.persist.get(), 0, 16)); CU(cudaDeviceSynchronize());
+    s.slot_cap = slot;
+  }
+  if (ev > s.event_cap) { s.event_cap = 0; if ((rc = regrow(ev, s.events, s.heavy_idx, s.event_pos, s.event_pre))) return rc; s.event_cap = ev; }
+  if (span > s.span_cap) {
+    s.span_cap = 0; s.spans.reset();
+    if ((rc = regrow(span, s.sorted, s.sort_tmp, s.sp_start, s.sp_len, s.sp_cat)) || (rc = s.spans.alloc((size_t)span * 6))) return rc;
+    s.span_cap = span;
+  }
+  if (res > s.res_cap || (res && !s.scan_part.get())) {
+    s.res_cap = 0;
+    if ((rc = regrow((size_t)res + 1, s.words, s.out_len, s.out_off, s.seg_cnt, s.seg_begin, s.kept_cnt, s.kept_begin))) return rc;
+    if (!s.scan_part.get() && (rc = s.scan_part.alloc(kScanPartials))) return rc;
+    s.res_cap = res;
+  }
+  return CG_OK;
 }
 // what an overflowed step teaches about the capacities the next one needs
 void learn_caps(cg_ruleset* rs, const uint32_t* hc) {
@@ -425,24 +401,24 @@ int scan_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, uin
   int rc;
   if (n && (rc = check_offsets(offsets, n))) return rc;
   const size_t first = n ? offsets[0] : 0, total = n ? offsets[n] : 0;
-  if ((rc = grow_bytes(total + 64))) return rc;
-  if ((rc = grow(&G.d_off32, &G.cap_off32, (size_t)n + 1))) return rc;
-  if ((rc = grow(&G.d_words, &G.cap_words, (size_t)n + 1))) return rc;
-  if (views && (rc = grow(&G.d_views, &G.cap_views, (size_t)n + 1))) return rc;
+  if ((rc = G.d_bytes.grow(total + 64))) return rc;
+  if ((rc = G.d_off32.grow((size_t)n + 1))) return rc;
+  if ((rc = G.d_words.grow((size_t)n + 1))) return rc;
+  if (views && (rc = G.d_views.grow((size_t)n + 1))) return rc;
   cudaStream_t st = G.stream;
   if (n) {
-    if (total > first) CU(cudaMemcpyAsync(G.d_bytes + first, bytes + first, total - first, cudaMemcpyHostToDevice, st));
-    CU(cudaMemsetAsync(G.d_bytes + total, 0, 64, st));
-    CU(cudaMemcpyAsync(G.d_off32, offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (views) CU(cudaMemcpyAsync(G.d_views, views, n, cudaMemcpyHostToDevice, st));
+    if (total > first) CU(cudaMemcpyAsync(G.d_bytes.get() + first, bytes + first, total - first, cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(G.d_bytes.get() + total, 0, 64, st));
+    CU(cudaMemcpyAsync(G.d_off32.get(), offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (views) CU(cudaMemcpyAsync(G.d_views.get(), views, n, cudaMemcpyHostToDevice, st));
   }
-  const ViewTable vt{rs->view_rows, G.d_views, rs->n_views};
+  const ViewTable vt{rs->view_rows.get(), G.d_views.get(), rs->n_views};
   uint32_t hc[kCounterWords] = {};
   for (int attempt = 0; attempt < 10; attempt++) {
     if ((rc = prepare_step(rs, n, kind, st, res_min))) return rc;
     const ScanWork& w = rs->work;
     CU(cudaEventRecord(G.ev0, st));
-    if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32, n, kind == kStepSpans ? w.words : G.d_words, kind, st, views ? &vt : nullptr))) return rc;
+    if ((rc = run_scan_device(rs, G.d_bytes.get(), G.d_off32.get(), n, kind == kStepSpans ? w.words : G.d_words.get(), kind, st, views ? &vt : nullptr))) return rc;
     CU(cudaEventRecord(G.ev1, st));
     if ((rc = after(w))) return rc;
     CU(cudaMemcpyAsync(hc, w.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
@@ -461,8 +437,7 @@ int ensure_copy_streams() {
   const int C = Ctx::kChunks;
   CU(cudaStreamCreateWithFlags(&G.s_h2d, cudaStreamNonBlocking)); CU(cudaStreamCreateWithFlags(&G.s_d2h, cudaStreamNonBlocking));
   for (int c = 0; c < C; c++) { CU(cudaEventCreateWithFlags(&G.e_h2d[c], cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&G.e_done[c], cudaEventDisableTiming)); }
-  CU(cudaMallocHost((void**)&G.h_chunk_counters, (size_t)C * kCounterWords * 4));
-  return CG_OK;
+  return G.h_chunk_counters.alloc((size_t)C * kCounterWords);
 }
 
 // Words-only scan of a large host batch in kChunks pieces: the H2D copy of piece c+1 and the D2H copy of piece c-1 run
@@ -473,9 +448,9 @@ int scan_host_chunked(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offs
   int rc;
   if ((rc = check_offsets(offsets, n))) return rc;
   const size_t total = offsets[n];
-  if ((rc = grow_bytes(total + 64))) return rc;
-  if ((rc = grow(&G.d_off32, &G.cap_off32, (size_t)n + 1))) return rc;
-  if ((rc = grow(&G.d_words, &G.cap_words, (size_t)n + 1))) return rc;
+  if ((rc = G.d_bytes.grow(total + 64))) return rc;
+  if ((rc = G.d_off32.grow((size_t)n + 1))) return rc;
+  if ((rc = G.d_words.grow((size_t)n + 1))) return rc;
   if ((rc = ensure_copy_streams())) return rc;
   cudaStream_t st = G.stream;
   InOrder turn(&rs->order, st);
@@ -483,8 +458,8 @@ int scan_host_chunked(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offs
   const uint32_t per = (n + C - 1) / C;
   CU(cudaStreamSynchronize(st));                            // (whatever still read the staging buffers is done: s_h2d does not wait for st)
   if ((rc = prepare_step(rs, per, kStepWords, st))) return rc;
-  CU(cudaMemcpyAsync(G.d_off32, offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, G.s_h2d));
-  CU(cudaMemsetAsync(G.d_bytes + total, 0, 64, G.s_h2d));
+  CU(cudaMemcpyAsync(G.d_off32.get(), offsets, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, G.s_h2d));
+  CU(cudaMemsetAsync(G.d_bytes.get() + total, 0, 64, G.s_h2d));
   CU(cudaEventRecord(G.ev0, st));
   int used = 0;
   for (int c = 0; c < C; c++) {
@@ -492,29 +467,29 @@ int scan_host_chunked(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offs
     if (m1 <= m0) break;
     used = c + 1;
     const size_t b0 = offsets[m0], b1 = offsets[m1];
-    if (b1 > b0) CU(cudaMemcpyAsync(G.d_bytes + b0, bytes + b0, b1 - b0, cudaMemcpyHostToDevice, G.s_h2d));
+    if (b1 > b0) CU(cudaMemcpyAsync(G.d_bytes.get() + b0, bytes + b0, b1 - b0, cudaMemcpyHostToDevice, G.s_h2d));
     CU(cudaEventRecord(G.e_h2d[c], G.s_h2d));
     CU(cudaStreamWaitEvent(st, G.e_h2d[c], 0));
     // (a piece reads up to 16 bytes past its last message -- bytes of the next piece that may still be in flight; whatever
     // it sees there cannot produce an occurrence inside its own range)
-    if ((rc = run_scan_device(rs, G.d_bytes, G.d_off32 + m0, m1 - m0, G.d_words + m0, kStepWords, st))) return rc;
-    CU(cudaMemcpyAsync(G.h_chunk_counters + (size_t)c * kCounterWords, rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
+    if ((rc = run_scan_device(rs, G.d_bytes.get(), G.d_off32.get() + m0, m1 - m0, G.d_words.get() + m0, kStepWords, st))) return rc;
+    CU(cudaMemcpyAsync(G.h_chunk_counters.get() + (size_t)c * kCounterWords, rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(G.e_done[c], st));
     CU(cudaStreamWaitEvent(G.s_d2h, G.e_done[c], 0));
-    if (out_words) CU(cudaMemcpyAsync(out_words + m0, G.d_words + m0, (size_t)(m1 - m0) * 8, cudaMemcpyDeviceToHost, G.s_d2h));
+    if (out_words) CU(cudaMemcpyAsync(out_words + m0, G.d_words.get() + m0, (size_t)(m1 - m0) * 8, cudaMemcpyDeviceToHost, G.s_d2h));
   }
   CU(cudaEventRecord(G.ev1, st));
   CU(cudaStreamSynchronize(st)); CU(cudaStreamSynchronize(G.s_d2h)); CU(cudaStreamSynchronize(G.s_h2d));
   float ms = 0; cudaEventElapsedTime(&ms, G.ev0, G.ev1); G.stats.last_scan_ms = ms;
   bool overflow = false;
   for (int c = 0; c < used; c++) {
-    if ((rc = absorb_counters(rs, G.h_chunk_counters + (size_t)c * kCounterWords)) < 0) return rc;
+    if ((rc = absorb_counters(rs, G.h_chunk_counters.get() + (size_t)c * kCounterWords)) < 0) return rc;
     overflow |= rc == 1;
   }
   if (overflow) return 1;
   for (int c = 0; c < used; c++) {
     const uint32_t m0 = c * per, m1 = std::min<uint64_t>((uint64_t)(c + 1) * per, n);
-    count_step(m1 - m0, offsets[m1] - offsets[m0], G.h_chunk_counters + (size_t)c * kCounterWords);
+    count_step(m1 - m0, offsets[m1] - offsets[m0], G.h_chunk_counters.get() + (size_t)c * kCounterWords);
   }
   return CG_OK;
 }
@@ -526,7 +501,7 @@ void poll_mirrors(cg_ruleset* rs, bool wait) {
     if (wait) cudaEventSynchronize(rs->e_cnt[i]);
     else if (cudaEventQuery(rs->e_cnt[i]) != cudaSuccess) { cudaGetLastError(); continue; }
     rs->cnt_pending[i] = false;
-    const uint32_t* hc = rs->h_counters + (size_t)i * kCounterWords;
+    const uint32_t* hc = rs->h_counters.get() + (size_t)i * kCounterWords;
     rs->sticky_flags |= hc[kCtrErrors];
     if (!hc[kCtrErrors]) rs->sticky_status |= hc[kCtrResolveStatus] ? 1u << hc[kCtrResolveStatus] : 0u;
     G.stats.spans += hc[kCtrResolved]; G.stats.sha256_items += hc[kCtrDigests]; G.stats.hits += hc[kCtrHits];     // (zero for steps without them)
@@ -536,8 +511,8 @@ void poll_mirrors(cg_ruleset* rs, bool wait) {
 
 // device path: the pinned counter mirror ring (allocated by the first device-path call)
 int ensure_mirrors(cg_ruleset* rs) {
-  if (rs->h_counters) return CG_OK;
-  CU(cudaMallocHost((void**)&rs->h_counters, (size_t)cg_ruleset::kMirror * kCounterWords * 4));
+  if (rs->h_counters.get()) return CG_OK;
+  if (int rc = rs->h_counters.alloc((size_t)cg_ruleset::kMirror * kCounterWords)) return rc;
   for (auto& e : rs->e_cnt) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   return CG_OK;
 }
@@ -545,7 +520,7 @@ int ensure_mirrors(cg_ruleset* rs) {
 int mirror_counters(cg_ruleset* rs, cudaStream_t st) {
   const int slot = (int)(rs->seq % cg_ruleset::kMirror);
   if (rs->cnt_pending[slot]) { cudaEventSynchronize(rs->e_cnt[slot]); poll_mirrors(rs, false); }
-  CU(cudaMemcpyAsync(rs->h_counters + (size_t)slot * kCounterWords, rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(rs->h_counters.get() + (size_t)slot * kCounterWords, rs->work.counters, kCounterWords * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaEventRecord(rs->e_cnt[slot], st));
   rs->cnt_pending[slot] = true; rs->seq++;
   return CG_OK;
@@ -578,12 +553,12 @@ int blocking_call(cg_ruleset* rs, StepKind kind, uint32_t n, uint32_t res_min, G
   if ((rc = prepare_step(rs, n, kind, st, res_min))) return rc;
   typename GraphCache<Key, Cap>::Entry* g = nullptr;
   if ((rc = cached_graph(rs, cache, key, st, enqueue, &g))) return rc;
-  CU(cudaMemcpyAsync(in.d, in.h, stage(in.h), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(in.d.get(), in.h.get(), stage(in.h.get()), cudaMemcpyHostToDevice, st));
   CU(cudaGraphLaunch(g->exec, st));
-  CU(cudaMemcpyAsync(out.h + at, out.d + at, bytes, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(out.h.get() + at, out.d.get() + at, bytes, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   count_launches(g->kernels);
-  return absorb_counters(rs, reinterpret_cast<const uint32_t*>(out.h + counters));
+  return absorb_counters(rs, reinterpret_cast<const uint32_t*>(out.h.get() + counters));
 }
 
 // cg_scan_batch_device's step replayed as one CUDA graph -- one launch per step instead of six, so the host never becomes
@@ -675,15 +650,10 @@ void cg_shutdown(void) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (!G.ready) return;
   cudaDeviceSynchronize();
-  cudaFree(G.d_spans); cudaFree(G.d_redact_out); cudaFree(G.d_redact_meta); cudaFree(G.d_verdicts); cudaFree(G.d_hits); cudaFree(G.d_views);
-  cudaFree(G.d_proles); cudaFree(G.d_pctx); cudaFree(G.d_patoms); cudaFree(G.d_pmatch);
-  if (G.h_chunk_counters) cudaFreeHost(G.h_chunk_counters);
   if (G.s_h2d) { cudaStreamDestroy(G.s_h2d); cudaStreamDestroy(G.s_d2h); for (int c = 0; c < Ctx::kChunks; c++) { cudaEventDestroy(G.e_h2d[c]); cudaEventDestroy(G.e_done[c]); } }
-  cudaFree(G.d_bytes_raw); cudaFree(G.d_off32); cudaFree(G.d_off64); cudaFree(G.d_words); cudaFree(G.d_dig[0]); cudaFree(G.d_dig[1]);
-  free_shard_roots();
   cudaEventDestroy(G.dig_order.ev);
   cudaEventDestroy(G.ev0); cudaEventDestroy(G.ev1); for (cudaEvent_t e : G.pev) cudaEventDestroy(e); cudaStreamDestroy(G.stream);
-  G = Ctx();
+  G = Ctx();                      // (frees every buffer G held)
 }
 
 int cg_set_profiling(int on) { G.profiling = on != 0; return CG_OK; }
@@ -873,19 +843,19 @@ int scan_batch_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offset
   uint64_t total = 0;
   int rc = scan_host(rs, bytes, offsets, n, want_hits ? kStepPolicy : kStepWords, [&](const ScanWork& w) {
     if (!want_hits || !n) return CG_OK;
-    count_launches(launch_hit_count(w, G.d_words, n, G.sm_count, st));
+    count_launches(launch_hit_count(w, G.d_words.get(), n, G.sm_count, st));
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(&total, w.out_off + n, 8, cudaMemcpyDeviceToHost, st));
     return CG_OK;
   }, views);
   if (rc) return rc;
   const uint32_t nh = (uint32_t)total, k = out_hits && !(total >> 32) ? std::min(nh, hits_cap) : 0u;
-  if (out_words && n) CU(cudaMemcpyAsync(out_words, G.d_words, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+  if (out_words && n) CU(cudaMemcpyAsync(out_words, G.d_words.get(), (size_t)n * 8, cudaMemcpyDeviceToHost, st));
   if (k) {
-    if ((rc = grow(&G.d_hits, &G.cap_hits, 2 * (size_t)k + 1))) return rc;      // [count][pairs]
-    count_launches(launch_hit_emit(rs->dev, rs->work, n, G.d_hits + 1, k, G.d_hits, G.sm_count, st));
+    if ((rc = G.d_hits.grow(2 * (size_t)k + 1))) return rc;      // [count][pairs]
+    count_launches(launch_hit_emit(rs->dev, rs->work, n, G.d_hits.get() + 1, k, G.d_hits.get(), G.sm_count, st));
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(out_hits, G.d_hits + 1, (size_t)k * sizeof(cg_hit), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out_hits, G.d_hits.get() + 1, (size_t)k * sizeof(cg_hit), cudaMemcpyDeviceToHost, st));
   }
   CU(cudaStreamSynchronize(st));
   if (total >> 32) { if (out_nhits) *out_nhits = 0xffffffffu; return fail(CG_ERR_TOO_LARGE, "2^32 hits or more in one batch"); }
@@ -919,14 +889,14 @@ int scan_one_fast(cg_ruleset* rs, const uint8_t* bytes, uint32_t len, uint64_t* 
   Staging& s = rs->one.io;
   const uint32_t off[2] = {0, len};
   const int rc = blocking_call(rs, kStepWords, 1, 0, rs->one.graphs, {}, s, [&](uint8_t* h) { return stage_texts(h, 256, bytes, off, 1); }, [&] {
-        const uint32_t* d_off = reinterpret_cast<const uint32_t*>(s.d);
-        uint32_t* d_out = reinterpret_cast<uint32_t*>(s.d + kOneIn); uint64_t* d_word = reinterpret_cast<uint64_t*>(s.d + kOneIn + kOneOut - 8);   // (the word lands behind the hit row, then is packed to the front)
-        const int r = run_scan_device(rs, s.d, d_off, 1, d_word, kStepWords, G.stream);
+        const uint32_t* d_off = reinterpret_cast<const uint32_t*>(s.d.get());
+        uint32_t* d_out = reinterpret_cast<uint32_t*>(s.d.get() + kOneIn); uint64_t* d_word = reinterpret_cast<uint64_t*>(s.d.get() + kOneIn + kOneOut - 8);   // (the word lands behind the hit row, then is packed to the front)
+        const int r = run_scan_device(rs, s.d.get(), d_off, 1, d_word, kStepWords, G.stream);
         if (r == CG_OK) count_launches(launch_pack_one(rs->dev, rs->work, d_word, d_out, kOneRw - 2, G.stream));
         return r;
       }, s, kOneIn, (kOneHitRow + rs->dev.rw) * 4, kOneIn + 4 * kOneCounters);
   if (rc) return rc;                                             // 1: a queue overflowed, the general path retries with larger scratch
-  const uint32_t* ho = reinterpret_cast<const uint32_t*>(s.h + kOneIn);
+  const uint32_t* ho = reinterpret_cast<const uint32_t*>(s.h.get() + kOneIn);
   const uint32_t* hc = ho + kOneCounters;
   count_step(1, len, hc);
   if (out_word) *out_word = (uint64_t)ho[0] | ((uint64_t)ho[1] << 32);
@@ -957,13 +927,13 @@ namespace {
 int resolve_staged(const ScanWork& w, uint32_t n, bool redact, uint64_t sizes[2], uint32_t** d_digests) {
   const size_t dig_at = ((size_t)n + 1 + 4 + 3) & ~(size_t)3;
   int rc;
-  if ((rc = grow(&G.d_spans, &G.cap_spans, (size_t)w.span_cap))) return rc;
-  if ((rc = grow(&G.d_redact_meta, &G.cap_redact_meta, dig_at + (redact ? (size_t)w.span_cap * 8 : 0)))) return rc;
-  *d_digests = G.d_redact_meta + dig_at;
-  const SpanOutputs o{reinterpret_cast<uint32_t*>(G.d_spans), w.span_cap, G.d_redact_meta + 4, ~0ull, G.d_redact_meta, redact};
-  count_launches(launch_span_resolve(w, G.d_off32, n, o, G.sm_count, G.stream));
+  if ((rc = G.d_spans.grow((size_t)w.span_cap))) return rc;
+  if ((rc = G.d_redact_meta.grow(dig_at + (redact ? (size_t)w.span_cap * 8 : 0)))) return rc;
+  *d_digests = G.d_redact_meta.get() + dig_at;
+  const SpanOutputs o{reinterpret_cast<uint32_t*>(G.d_spans.get()), w.span_cap, G.d_redact_meta.get() + 4, ~0ull, G.d_redact_meta.get(), redact};
+  count_launches(launch_span_resolve(w, G.d_off32.get(), n, o, G.sm_count, G.stream));
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(sizes, G.d_redact_meta, redact ? 16 : 4, cudaMemcpyDeviceToHost, G.stream));
+  CU(cudaMemcpyAsync(sizes, G.d_redact_meta.get(), redact ? 16 : 4, cudaMemcpyDeviceToHost, G.stream));
   return CG_OK;
 }
 
@@ -976,7 +946,7 @@ int find_matches_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offs
   if (rc) return rc;
   const uint32_t outn = (uint32_t)sizes[0], k = std::min(outn, spans_cap);
   G.stats.spans += outn;
-  if (out_spans && k) { CU(cudaMemcpyAsync(out_spans, G.d_spans, (size_t)k * sizeof(cg_span), cudaMemcpyDeviceToHost, G.stream)); CU(cudaStreamSynchronize(G.stream)); }
+  if (out_spans && k) { CU(cudaMemcpyAsync(out_spans, G.d_spans.get(), (size_t)k * sizeof(cg_span), cudaMemcpyDeviceToHost, G.stream)); CU(cudaStreamSynchronize(G.stream)); }
   if (out_nspans) *out_nspans = outn;
   if (out_spans && outn > spans_cap) return fail(CG_ERR_CAPACITY, "out_spans too small");
   return CG_OK;
@@ -1006,9 +976,10 @@ int cg_ruleset_set_policy(cg_ruleset* rs, const uint32_t* rule_policy, const uin
     act[i] = rule_action[i];
   }
   CU(cudaStreamSynchronize(G.stream));
-  int rc;
-  if ((rc = upload(rs, pol, &rs->dev.rule_policy))) return rc;
-  if ((rc = upload(rs, act, &rs->dev.rule_action))) return rc;
+  DevBuf<uint8_t> d_pol, d_act; const uint32_t *p, *a; int rc;     // (they replace the old tables once both are there)
+  if ((rc = upload(rs, pol, &p, 4, &d_pol)) || (rc = upload(rs, act, &a, 4, &d_act))) return rc;
+  rs->rule_policy = std::move(d_pol); rs->rule_action = std::move(d_act);
+  rs->dev.rule_policy = p; rs->dev.rule_action = a;
   rs->scratch_gen++;                                        // DevRuleset is captured by value
   return CG_OK;
 }
@@ -1025,9 +996,9 @@ int cg_ruleset_set_views(cg_ruleset* rs, const uint32_t* rows, uint32_t n_views)
       if (rows[(size_t)v * rw + k] & ~valid) return fail(CG_ERR_INVALID_ARG, "view " + std::to_string(v) + " has a bit at or past n_rules");
     }
   CU(cudaStreamSynchronize(G.stream));
-  cudaFree(rs->view_rows); rs->view_rows = nullptr; rs->n_views = 0;
-  CU(cudaMalloc((void**)&rs->view_rows, (size_t)n_views * rw * 4));
-  CU(cudaMemcpy(rs->view_rows, rows, (size_t)n_views * rw * 4, cudaMemcpyHostToDevice));
+  rs->view_rows.reset(); rs->n_views = 0;
+  if (int rc = rs->view_rows.alloc((size_t)n_views * rw)) return rc;
+  CU(cudaMemcpy(rs->view_rows.get(), rows, (size_t)n_views * rw * 4, cudaMemcpyHostToDevice));
   rs->n_views = n_views;
   rs->scratch_gen++;
   return CG_OK;
@@ -1041,14 +1012,14 @@ int verdict_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, 
   int rc = scan_host(rs, bytes, offsets, n, kStepWords, [&](const ScanWork& w) {
     if (!n) return CG_OK;
     int r;
-    if ((r = grow(&G.d_verdicts, &G.cap_verdicts, (size_t)n))) return r;
-    CU(cudaMemsetAsync(G.d_verdicts, 0, (size_t)n * 4, st));  // (verdict_kernel writes the messages that hit)
-    count_launches(launch_verdicts(rs->dev, w, G.d_verdicts, n, G.sm_count, st));
+    if ((r = G.d_verdicts.grow((size_t)n))) return r;
+    CU(cudaMemsetAsync(G.d_verdicts.get(), 0, (size_t)n * 4, st));  // (verdict_kernel writes the messages that hit)
+    count_launches(launch_verdicts(rs->dev, w, G.d_verdicts.get(), n, G.sm_count, st));
     CU(cudaGetLastError());
     return CG_OK;
   }, views);
   if (rc || !n) return rc;
-  CU(cudaMemcpyAsync(out_verdicts, G.d_verdicts, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(out_verdicts, G.d_verdicts.get(), (size_t)n * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
 }
@@ -1085,14 +1056,14 @@ int redact_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, u
   if (out_nspans) *out_nspans = ns;
   const bool too_large = pos >> 32, fits = !too_large && !(out_spans && ns > spans_cap) && pos <= out_cap && out_bytes;
   cudaStream_t st = G.stream;
-  if (fits && (rc = grow(&G.d_redact_out, &G.cap_redact_out, (size_t)pos + 64))) return rc;
-  CU(cudaMemcpyAsync(out_offsets, G.d_redact_meta + 4, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, st));
+  if (fits && (rc = G.d_redact_out.grow((size_t)pos + 64))) return rc;
+  CU(cudaMemcpyAsync(out_offsets, G.d_redact_meta.get() + 4, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, st));
   if (fits) {
-    count_launches(enqueue_redact_tail(rs->work, G.d_bytes, G.d_off32, G.d_redact_meta + 4, d_dig, G.d_redact_out, n, st));
+    count_launches(enqueue_redact_tail(rs->work, G.d_bytes.get(), G.d_off32.get(), G.d_redact_meta.get() + 4, d_dig, G.d_redact_out.get(), n, st));
     G.stats.sha256_items += ns;
     CU(cudaGetLastError());
-    if (pos) CU(cudaMemcpyAsync(out_bytes, G.d_redact_out, (size_t)pos, cudaMemcpyDeviceToHost, st));
-    if (ns && out_spans) CU(cudaMemcpyAsync(out_spans, G.d_spans, (size_t)ns * sizeof(cg_span), cudaMemcpyDeviceToHost, st));
+    if (pos) CU(cudaMemcpyAsync(out_bytes, G.d_redact_out.get(), (size_t)pos, cudaMemcpyDeviceToHost, st));
+    if (ns && out_spans) CU(cudaMemcpyAsync(out_spans, G.d_spans.get(), (size_t)ns * sizeof(cg_span), cudaMemcpyDeviceToHost, st));
     if (ns && out_digests32) CU(cudaMemcpyAsync(out_digests32, d_dig, (size_t)ns * 32, cudaMemcpyDeviceToHost, st));
   }
   CU(cudaStreamSynchronize(st));
@@ -1137,29 +1108,29 @@ int span_few_fast(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets,
   const uint32_t window = std::min<uint32_t>(kOnePack, at + 1024 + (redact ? 2 * len : len / 2));
   const int rc = blocking_call(rs, kStepSpans, n, 0, rs->span.graphs, {redact, n}, in, [&](uint8_t* h) { return stage_texts(h, kFewTextAt, bytes, offsets, n); }, [&] {
         const ScanWork& w = rs->work;
-        const uint32_t* d_off = reinterpret_cast<const uint32_t*>(in.d);
-        uint32_t* d_pack = reinterpret_cast<uint32_t*>(pk.d); uint32_t* d_dig = reinterpret_cast<uint32_t*>(pk.d + kOnePack); uint8_t* d_out = pk.d + 2 * kOnePack;
-        const int r = run_scan_device(rs, in.d, d_off, n, w.words, kStepSpans, G.stream);
+        const uint32_t* d_off = reinterpret_cast<const uint32_t*>(in.d.get());
+        uint32_t* d_pack = reinterpret_cast<uint32_t*>(pk.d.get()); uint32_t* d_dig = reinterpret_cast<uint32_t*>(pk.d.get() + kOnePack); uint8_t* d_out = pk.d.get() + 2 * kOnePack;
+        const int r = run_scan_device(rs, in.d.get(), d_off, n, w.words, kStepSpans, G.stream);
         if (r != CG_OK) return r;
         const SpanOutputs so{d_pack + at / 4, room / (redact ? 56u : 24u), d_pack + kPackOffsets, redact ? (uint64_t)room : 0ull, d_pack + kPackSizes, redact};
         int k = launch_span_resolve_few(w, d_off, n, so, G.stream);
-        if (redact) k += enqueue_redact_tail(w, in.d, d_off, d_pack + kPackOffsets, d_dig, d_out, n, G.stream);
+        if (redact) k += enqueue_redact_tail(w, in.d.get(), d_off, d_pack + kPackOffsets, d_dig, d_out, n, G.stream);
         k += launch_span_pack_few(w, d_dig, d_out, d_pack, kOnePack, n, redact, G.stream);
         count_launches(k);
         CU(cudaGetLastError());
         return CG_OK;
       }, pk, 0, window, 4 * kPackCounters);
   if (rc) return rc;                                             // 1: a queue overflowed, the batch call retries with larger scratch
-  const uint32_t* hp = reinterpret_cast<const uint32_t*>(pk.h);
+  const uint32_t* hp = reinterpret_cast<const uint32_t*>(pk.h.get());
   const uint32_t* hc = hp + kPackCounters;
   const uint32_t packed = hp[0];
   if (!packed) return 1;                                         // longer than the packed region: the batch call has room
   if (packed > window) {
-    CU(cudaMemcpyAsync(pk.h + window, pk.d + window, packed - window, cudaMemcpyDeviceToHost, G.stream));
+    CU(cudaMemcpyAsync(pk.h.get() + window, pk.d.get() + window, packed - window, cudaMemcpyDeviceToHost, G.stream));
     CU(cudaStreamSynchronize(G.stream));
   }
   count_step(n, len, hc);
-  const uint8_t* body = pk.h + at;
+  const uint8_t* body = pk.h.get() + at;
   if (!redact) {
     const uint32_t ns = hp[kPackSizes];
     G.stats.spans += ns;
@@ -1240,7 +1211,7 @@ namespace {
 int device_views(const cg_ruleset* rs, const void* d_views, ViewTable* vt) {
   if (!rs->n_views) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_views has not been called");
   if (!d_views) return fail(CG_ERR_INVALID_ARG, "null argument");
-  *vt = ViewTable{rs->view_rows, (const uint8_t*)d_views, rs->n_views};
+  *vt = ViewTable{rs->view_rows.get(), (const uint8_t*)d_views, rs->n_views};
   return CG_OK;
 }
 
@@ -1410,24 +1381,24 @@ int cg_ruleset_set_policy_program(cg_ruleset* rs, const uint32_t* program, uint3
   }
   if (at != words) return bad("words past the last policy");
   CU(cudaStreamSynchronize(G.stream));
-  cudaFree(rs->prog_ops); cudaFree(rs->prog_rules); rs->prog_ops = nullptr; rs->prog_rules = nullptr; rs->prog_n_rules = rs->prog_n_atoms = 0;
+  rs->prog_ops.reset(); rs->prog_rules.reset(); rs->prog_n_rules = rs->prog_n_atoms = 0;
   rs->prog_gen++;                                           // (cg_policy_eval_one's graphs hold the old tables)
-  CU(cudaMalloc((void**)&rs->prog_ops, (size_t)words * 4));
-  CU(cudaMalloc((void**)&rs->prog_rules, std::max<size_t>(rules.size(), 1) * sizeof(uint4)));
-  CU(cudaMemcpy(rs->prog_ops, program, (size_t)words * 4, cudaMemcpyHostToDevice));
-  if (!rules.empty()) CU(cudaMemcpy(rs->prog_rules, rules.data(), rules.size() * sizeof(uint4), cudaMemcpyHostToDevice));
+  int rc;
+  if ((rc = rs->prog_ops.alloc(words)) || (rc = rs->prog_rules.alloc(std::max<size_t>(rules.size(), 1)))) return rc;
+  CU(cudaMemcpy(rs->prog_ops.get(), program, (size_t)words * 4, cudaMemcpyHostToDevice));
+  if (!rules.empty()) CU(cudaMemcpy(rs->prog_rules.get(), rules.data(), rules.size() * sizeof(uint4), cudaMemcpyHostToDevice));
   rs->prog_n_rules = (uint32_t)rules.size(); rs->prog_n_atoms = n_atoms;
   return CG_OK;
 }
 
 namespace {
-PolicyTable policy_table(const cg_ruleset* rs) { return PolicyTable{rs->prog_ops, rs->prog_rules, rs->prog_n_rules, (rs->prog_n_atoms + 31) / 32}; }
+PolicyTable policy_table(const cg_ruleset* rs) { return PolicyTable{rs->prog_ops.get(), rs->prog_rules.get(), rs->prog_n_rules, (rs->prog_n_atoms + 31) / 32}; }
 
 int policy_eval_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, const uint8_t* roles, uint32_t n_texts, const uint32_t* ctx_offsets,
                      const uint32_t* atoms, uint32_t n_ctx, uint32_t* out_verdicts, cg_policy_match* out_matches, uint32_t matches_cap, uint32_t* out_nmatches) {
   if (int rc = require_ready()) return rc;
   if (!rs) return fail(CG_ERR_INVALID_ARG, "null argument");
-  if (!rs->prog_ops) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy_program has not been called");
+  if (!rs->prog_ops.get()) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy_program has not been called");
   const PolicyTable pt = policy_table(rs);
   if (!ctx_offsets || (n_texts && !roles) || (n_ctx && (!out_verdicts || (pt.aw && !atoms)))) return fail(CG_ERR_INVALID_ARG, "null argument");
   for (uint32_t c = 0; c < n_ctx; c++)
@@ -1438,29 +1409,29 @@ int policy_eval_host(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offse
   InOrder turn(&rs->order, st);
   if (turn.rc) return turn.rc;
   int rc;
-  if ((rc = grow(&G.d_proles, &G.cap_proles, (size_t)n_texts + 1))) return rc;
-  if ((rc = grow(&G.d_pctx, &G.cap_pctx, (size_t)n_ctx + 1))) return rc;
-  if ((rc = grow(&G.d_patoms, &G.cap_patoms, (size_t)n_ctx * pt.aw + 1))) return rc;
-  if ((rc = grow(&G.d_verdicts, &G.cap_verdicts, (size_t)n_ctx))) return rc;
-  if (n_texts) CU(cudaMemcpyAsync(G.d_proles, roles, n_texts, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(G.d_pctx, ctx_offsets, ((size_t)n_ctx + 1) * 4, cudaMemcpyHostToDevice, st));
-  if (pt.aw) CU(cudaMemcpyAsync(G.d_patoms, atoms, (size_t)n_ctx * pt.aw * 4, cudaMemcpyHostToDevice, st));
-  const PolicyBatch b{G.d_proles, n_texts, G.d_pctx, G.d_patoms, n_ctx};
+  if ((rc = G.d_proles.grow((size_t)n_texts + 1))) return rc;
+  if ((rc = G.d_pctx.grow((size_t)n_ctx + 1))) return rc;
+  if ((rc = G.d_patoms.grow((size_t)n_ctx * pt.aw + 1))) return rc;
+  if ((rc = G.d_verdicts.grow((size_t)n_ctx))) return rc;
+  if (n_texts) CU(cudaMemcpyAsync(G.d_proles.get(), roles, n_texts, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(G.d_pctx.get(), ctx_offsets, ((size_t)n_ctx + 1) * 4, cudaMemcpyHostToDevice, st));
+  if (pt.aw) CU(cudaMemcpyAsync(G.d_patoms.get(), atoms, (size_t)n_ctx * pt.aw * 4, cudaMemcpyHostToDevice, st));
+  const PolicyBatch b{G.d_proles.get(), n_texts, G.d_pctx.get(), G.d_patoms.get(), n_ctx};
   uint64_t total = 0;
   rc = scan_host(rs, bytes, offsets, n_texts, kStepPolicy, [&](const ScanWork& w) {
-    count_launches(launch_policy_eval(pt, w, rs->dev.rw, b, G.d_verdicts, want, G.sm_count, st));
+    count_launches(launch_policy_eval(pt, w, rs->dev.rw, b, G.d_verdicts.get(), want, G.sm_count, st));
     CU(cudaGetLastError());
     if (want) CU(cudaMemcpyAsync(&total, w.out_off + n_ctx, 8, cudaMemcpyDeviceToHost, st));
     return CG_OK;
   }, nullptr, n_ctx);
   if (rc) return rc;
-  CU(cudaMemcpyAsync(out_verdicts, G.d_verdicts, (size_t)n_ctx * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(out_verdicts, G.d_verdicts.get(), (size_t)n_ctx * 4, cudaMemcpyDeviceToHost, st));
   const uint32_t k = out_matches && !(total >> 32) ? (uint32_t)std::min<uint64_t>(total, matches_cap) : 0u;
   if (want) {                                                // (emit runs whatever the count: launches do not depend on it)
-    if ((rc = grow(&G.d_pmatch, &G.cap_pmatch, 2 * (size_t)k + 1))) return rc;      // [count][pairs]
-    count_launches(launch_policy_emit(pt, rs->work, rs->dev.rw, b, G.d_pmatch + 1, k, G.d_pmatch, G.sm_count, st));
+    if ((rc = G.d_pmatch.grow(2 * (size_t)k + 1))) return rc;      // [count][pairs]
+    count_launches(launch_policy_emit(pt, rs->work, rs->dev.rw, b, G.d_pmatch.get() + 1, k, G.d_pmatch.get(), G.sm_count, st));
     CU(cudaGetLastError());
-    if (k) CU(cudaMemcpyAsync(out_matches, G.d_pmatch + 1, (size_t)k * sizeof(cg_policy_match), cudaMemcpyDeviceToHost, st));
+    if (k) CU(cudaMemcpyAsync(out_matches, G.d_pmatch.get() + 1, (size_t)k * sizeof(cg_policy_match), cudaMemcpyDeviceToHost, st));
   }
   CU(cudaStreamSynchronize(st));
   if (total >> 32) { if (out_nmatches) *out_nmatches = 0xffffffffu; return fail(CG_ERR_TOO_LARGE, "2^32 matches or more in one batch"); }
@@ -1474,7 +1445,7 @@ int policy_eval_device(cg_ruleset* rs, const void* d_bytes, const void* d_offset
                        void* stream) {
   if (int rc = require_ready()) return rc;
   if (!rs) return fail(CG_ERR_INVALID_ARG, "null argument");
-  if (!rs->prog_ops) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy_program has not been called");
+  if (!rs->prog_ops.get()) return fail(CG_ERR_INVALID_ARG, "cg_ruleset_set_policy_program has not been called");
   const PolicyTable pt = policy_table(rs);
   if ((n_texts && (!d_bytes || !d_offsets || !d_roles)) || !d_ctx_offsets || (n_ctx && (!d_out_verdicts || (pt.aw && !d_atoms))) ||
       (matches_cap && !d_out_matches) || (d_out_matches && !d_out_nmatches))
@@ -1516,7 +1487,7 @@ namespace {
 // holds, more matches than it holds and the caller wants, a queue overflowed)
 int policy_one_fast(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offsets, const uint8_t* roles, uint32_t n_texts, const uint32_t* atoms,
                     uint32_t* out_verdict, uint32_t* out_rules, uint32_t rules_cap, uint32_t* out_nrules) {
-  if (!G.ready || !rs || !rs->prog_ops || !out_verdict || G.profiling || n_texts > kPeOneTexts) return 1;
+  if (!G.ready || !rs || !rs->prog_ops.get() || !out_verdict || G.profiling || n_texts > kPeOneTexts) return 1;
   if (n_texts && (!bytes || !offsets || !roles)) return 1;
   const PolicyTable pt = policy_table(rs);
   if (pt.aw > kPeOneAtomWords || (pt.aw && !atoms)) return 1;
@@ -1532,15 +1503,15 @@ int policy_one_fast(cg_ruleset* rs, const uint8_t* bytes, const uint32_t* offset
         return stage_texts(h, kPeTextAt, bytes, offsets, n_texts);
       }, [&] {
         const ScanWork& w = rs->work;
-        const PolicyBatch b{s.d + kPeRolesAt, n_texts, nullptr, reinterpret_cast<const uint32_t*>(s.d + kPeAtomsAt), 1};
-        const int r = run_scan_device(rs, s.d, reinterpret_cast<const uint32_t*>(s.d), n_texts, w.words, kStepPolicy, G.stream);
+        const PolicyBatch b{s.d.get() + kPeRolesAt, n_texts, nullptr, reinterpret_cast<const uint32_t*>(s.d.get() + kPeAtomsAt), 1};
+        const int r = run_scan_device(rs, s.d.get(), reinterpret_cast<const uint32_t*>(s.d.get()), n_texts, w.words, kStepPolicy, G.stream);
         if (r != CG_OK) return r;
-        count_launches(launch_policy_eval_one(pt, w, rs->dev.rw, b, reinterpret_cast<uint32_t*>(s.d + kPeIn), kPeOneRulesCap, G.stream));
+        count_launches(launch_policy_eval_one(pt, w, rs->dev.rw, b, reinterpret_cast<uint32_t*>(s.d.get() + kPeIn), kPeOneRulesCap, G.stream));
         CU(cudaGetLastError());
         return CG_OK;
       }, s, kPeIn, 4 * ((size_t)kPeOneRules + want), kPeIn + 4 * kPeOneCounters);
   if (rc) return rc;                                             // 1: a queue overflowed, the batch call retries with larger scratch
-  const uint32_t* ho = reinterpret_cast<const uint32_t*>(s.h + kPeIn);
+  const uint32_t* ho = reinterpret_cast<const uint32_t*>(s.h.get() + kPeIn);
   const uint32_t* hc = ho + kPeOneCounters;
   const uint32_t nm = ho[1];
   if (out_rules && nm > kPeOneRulesCap && rules_cap > kPeOneRulesCap) return 1;
@@ -1583,15 +1554,15 @@ int cg_sha256_batch(const uint8_t* bytes, const uint64_t* offsets, uint32_t n, u
   InOrder turn(&G.dig_order, st);
   size_t total = offsets[n]; int rc;
   if ((rc = turn.rc)) return rc;
-  if ((rc = grow_bytes(total + 64))) return rc;
-  if ((rc = grow(&G.d_off64, &G.cap_off64, (size_t)n + 1))) return rc;
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)n * 8))) return rc;
-  if (total) CU(cudaMemcpyAsync(G.d_bytes, bytes, total, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(G.d_off64, offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
-  int k = launch_sha256_batch(G.d_bytes, G.d_off64, n, (uint8_t*)G.d_dig[0], st);
+  if ((rc = G.d_bytes.grow(total + 64))) return rc;
+  if ((rc = G.d_off64.grow((size_t)n + 1))) return rc;
+  if ((rc = G.d_dig[0].grow((size_t)n * 8))) return rc;
+  if (total) CU(cudaMemcpyAsync(G.d_bytes.get(), bytes, total, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(G.d_off64.get(), offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
+  int k = launch_sha256_batch(G.d_bytes.get(), G.d_off64.get(), n, (uint8_t*)G.d_dig[0].get(), st);
   count_launches(k); G.stats.sha256_items += n;
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(out, G.d_dig[0], (size_t)n * 32, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(out, G.d_dig[0].get(), (size_t)n * 32, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
 }
@@ -1602,13 +1573,13 @@ int empty_root(uint8_t out[32]) {
   InOrder turn(&G.dig_order, G.stream);
   int rc;
   if ((rc = turn.rc)) return rc;
-  if ((rc = grow(&G.d_off64, &G.cap_off64, 2))) return rc;
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], 8))) return rc;
-  if ((rc = grow_bytes(64))) return rc;
-  CU(cudaMemsetAsync(G.d_off64, 0, 16, G.stream));
-  int k = launch_sha256_batch(G.d_bytes, G.d_off64, 1, (uint8_t*)G.d_dig[0], G.stream);
+  if ((rc = G.d_off64.grow(2))) return rc;
+  if ((rc = G.d_dig[0].grow(8))) return rc;
+  if ((rc = G.d_bytes.grow(64))) return rc;
+  CU(cudaMemsetAsync(G.d_off64.get(), 0, 16, G.stream));
+  int k = launch_sha256_batch(G.d_bytes.get(), G.d_off64.get(), 1, (uint8_t*)G.d_dig[0].get(), G.stream);
   count_launches(k);
-  CU(cudaMemcpyAsync(out, G.d_dig[0], 32, cudaMemcpyDeviceToHost, G.stream));
+  CU(cudaMemcpyAsync(out, G.d_dig[0].get(), 32, cudaMemcpyDeviceToHost, G.stream));
   CU(cudaStreamSynchronize(G.stream));
   return CG_OK;
 }
@@ -1616,11 +1587,11 @@ int empty_root(uint8_t out[32]) {
 // One-shot trees: size_dig(n) makes room for n staged nodes in G.d_dig[0]; fold_dig folds n nodes at d_nodes (read in place,
 // may be G.d_dig[0]) by at most max_levels levels, ping-ponging between G.d_dig[1] and G.d_dig[0]; *out = the folded nodes
 int size_dig(uint64_t n) {
-  int rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)n * 8);
-  return rc ? rc : grow(&G.d_dig[1], &G.cap_dig[1], (size_t)(n + 1) / 2 * 8 + 8);
+  int rc = G.d_dig[0].grow((size_t)n * 8);
+  return rc ? rc : G.d_dig[1].grow((size_t)(n + 1) / 2 * 8 + 8);
 }
 int fold_dig(const uint32_t* d_nodes, uint64_t n, uint32_t max_levels, cudaStream_t st, const uint32_t** out) {
-  count_launches(launch_merkle_fold(d_nodes, n, max_levels, G.d_dig[1], G.d_dig[0], st, out));
+  count_launches(launch_merkle_fold(d_nodes, n, max_levels, G.d_dig[1].get(), G.d_dig[0].get(), st, out));
   CU(cudaGetLastError());
   return CG_OK;
 }
@@ -1632,9 +1603,9 @@ int staged_root(uint64_t n, const uint64_t* d_off, uint64_t leaf_len, uint8_t ou
   if ((rc = turn.rc)) return rc;
   if ((rc = size_dig(n))) return rc;
   CU(cudaEventRecord(G.ev0, st));
-  count_launches(d_off ? launch_merkle_leaves_var(G.d_bytes, d_off, n, G.d_dig[0], st) : launch_merkle_leaves_fixed(G.d_bytes, leaf_len, n, G.d_dig[0], st));
+  count_launches(d_off ? launch_merkle_leaves_var(G.d_bytes.get(), d_off, n, G.d_dig[0].get(), st) : launch_merkle_leaves_fixed(G.d_bytes.get(), leaf_len, n, G.d_dig[0].get(), st));
   G.stats.merkle_leaves += n;
-  if ((rc = fold_dig(G.d_dig[0], n, 64, st, &d_root))) return rc;
+  if ((rc = fold_dig(G.d_dig[0].get(), n, 64, st, &d_root))) return rc;
   CU(cudaEventRecord(G.ev1, st));
   CU(cudaMemcpyAsync(out_root, d_root, 32, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
@@ -1648,8 +1619,8 @@ int block_roots(const void* d_bytes, uint64_t leaf_len, uint64_t n, uint32_t blo
   InOrder turn(&G.dig_order, st);
   if ((rc = turn.rc)) return rc;
   if ((rc = size_dig(n))) return rc;
-  count_launches(launch_merkle_leaves_fixed((const uint8_t*)d_bytes, leaf_len, n, G.d_dig[0], st)); G.stats.merkle_leaves += n;
-  if ((rc = fold_dig(G.d_dig[0], n, block_log2, st, &d_res))) return rc;
+  count_launches(launch_merkle_leaves_fixed((const uint8_t*)d_bytes, leaf_len, n, G.d_dig[0].get(), st)); G.stats.merkle_leaves += n;
+  if ((rc = fold_dig(G.d_dig[0].get(), n, block_log2, st, &d_res))) return rc;
   CU(cudaMemcpyAsync(d_roots, d_res, ((n + (1ull << block_log2) - 1) >> block_log2) * 32, cudaMemcpyDeviceToDevice, st));
   return CG_OK;
 }
@@ -1662,11 +1633,11 @@ int cg_merkle_root(const uint8_t* bytes, const uint64_t* offsets, uint64_t n, ui
   if (n == 0) return empty_root(out_root);
   if (!offsets) return fail(CG_ERR_INVALID_ARG, "null argument");
   size_t total = offsets[n]; int rc;
-  if ((rc = grow_bytes(total + 64))) return rc;
-  if ((rc = grow(&G.d_off64, &G.cap_off64, (size_t)n + 1))) return rc;
-  if (total) CU(cudaMemcpyAsync(G.d_bytes, bytes, total, cudaMemcpyHostToDevice, G.stream));
-  CU(cudaMemcpyAsync(G.d_off64, offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, G.stream));
-  return staged_root(n, G.d_off64, 0, out_root);
+  if ((rc = G.d_bytes.grow(total + 64))) return rc;
+  if ((rc = G.d_off64.grow((size_t)n + 1))) return rc;
+  if (total) CU(cudaMemcpyAsync(G.d_bytes.get(), bytes, total, cudaMemcpyHostToDevice, G.stream));
+  CU(cudaMemcpyAsync(G.d_off64.get(), offsets, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, G.stream));
+  return staged_root(n, G.d_off64.get(), 0, out_root);
 }
 
 int cg_merkle_root_fixed(const uint8_t* bytes, uint64_t leaf_len, uint64_t n, uint8_t out_root[32]) {
@@ -1675,8 +1646,8 @@ int cg_merkle_root_fixed(const uint8_t* bytes, uint64_t leaf_len, uint64_t n, ui
   if (!out_root) return fail(CG_ERR_INVALID_ARG, "null argument");
   if (n == 0) return empty_root(out_root);
   size_t total = (size_t)leaf_len * n; int rc;
-  if ((rc = grow_bytes(total + 64))) return rc;
-  if (total) CU(cudaMemcpyAsync(G.d_bytes, bytes, total, cudaMemcpyHostToDevice, G.stream));
+  if ((rc = G.d_bytes.grow(total + 64))) return rc;
+  if (total) CU(cudaMemcpyAsync(G.d_bytes.get(), bytes, total, cudaMemcpyHostToDevice, G.stream));
   return staged_root(n, nullptr, leaf_len, out_root);
 }
 
@@ -1700,8 +1671,8 @@ int cg_merkle_fold(const uint8_t* nodes32, uint64_t m, uint8_t out_root[32]) {
   InOrder turn(&G.dig_order, st);
   if ((rc = turn.rc)) return rc;
   if ((rc = size_dig(m))) return rc;
-  CU(cudaMemcpyAsync(G.d_dig[0], nodes32, m * 32, cudaMemcpyHostToDevice, st));
-  if ((rc = fold_dig(G.d_dig[0], m, 64, st, &d_root))) return rc;
+  CU(cudaMemcpyAsync(G.d_dig[0].get(), nodes32, m * 32, cudaMemcpyHostToDevice, st));
+  if ((rc = fold_dig(G.d_dig[0].get(), m, 64, st, &d_root))) return rc;
   CU(cudaMemcpyAsync(out_root, d_root, 32, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
@@ -1717,7 +1688,7 @@ int cg_merkle_fold_device(const void* d_nodes32, uint64_t m, void* d_out_root32,
   if ((rc = size_dig(m))) return rc;
   // the fold reads the nodes in place, unless they are off the 16-byte alignment of the kernels' loads: then from a copy
   const uint32_t* d_nodes = (const uint32_t*)d_nodes32;
-  if ((uintptr_t)d_nodes32 & 15) { CU(cudaMemcpyAsync(G.d_dig[0], d_nodes32, m * 32, cudaMemcpyDeviceToDevice, st)); d_nodes = G.d_dig[0]; }
+  if ((uintptr_t)d_nodes32 & 15) { CU(cudaMemcpyAsync(G.d_dig[0].get(), d_nodes32, m * 32, cudaMemcpyDeviceToDevice, st)); d_nodes = G.d_dig[0].get(); }
   if ((rc = fold_dig(d_nodes, m, 64, st, &d_root))) return rc;
   CU(cudaMemcpyAsync(d_out_root32, d_root, 32, cudaMemcpyDeviceToDevice, st));
   return CG_OK;
@@ -1727,34 +1698,29 @@ int cg_merkle_fold_device(const void* d_nodes32, uint64_t m, void* d_out_root32,
 struct cg_merkle_log {
   uint64_t n = 0;                 // leaves so far; bit h of n set <=> slot h holds the root of a perfect 2^h subtree
   bool keep = false;              // keep every leaf digest in HBM (needed for inclusion proofs)
-  uint32_t* d_slots = nullptr;    // 64 x 8 words
-  uint32_t* d_tmp = nullptr;      // 65 x 8 words: [0..63] a proof folded from the leaf digests, [64] the root
-  uint32_t* d_leaves = nullptr; uint64_t cap_leaves = 0;     // keep: n leaf digests
-  uint32_t* d_new = nullptr; size_t cap_new = 0;             // !keep: the current batch's leaf digests
-  uint32_t* d_a = nullptr; size_t cap_a = 0; uint32_t* d_b = nullptr; size_t cap_b = 0;   // level ping-pong
-  // tree (cg_merkle_log_create_tree): every complete aligned node as well -- level h >= 1 holds floor(n / 2^h) nodes at
-  // d_lvl[h] (node j covers leaves [j 2^h, (j + 1) 2^h)), each level sized cap_leaves >> h, so the store is smaller than the
-  // leaf digests; d_spine: 64 x 8 words, the suffix roots of the tree size of the last proof call (log_spine)
+  DevBuf<uint32_t> d_slots;       // 64 x 8 words
+  DevBuf<uint32_t> d_tmp;         // 65 x 8 words: [0..63] a proof folded from the leaf digests, [64] the root
+  DevBuf<uint32_t> d_new;         // !keep: the current batch's leaf digests
+  DevBuf<uint32_t> d_a, d_b;      // level ping-pong
+  // keep: d_lvl[0] holds the n leaf digests.  tree (cg_merkle_log_create_tree): level h >= 1 holds floor(n / 2^h) nodes at d_lvl[h]
+  // (node j covers leaves [j 2^h, (j + 1) 2^h)), each level sized for (leaf digest room) >> h nodes, so the store is smaller than
+  // the leaf digests; d_spine: 64 x 8 words, the suffix roots of the tree size of the last proof call (log_spine)
   bool tree = false;
-  uint32_t* d_lvl[64] = {}; uint64_t cap_lvl[64] = {};
-  uint32_t* d_spine = nullptr;
+  DevBuf<uint32_t> d_lvl[64];
+  DevBuf<uint32_t> d_spine;
   IssueOrder order;               // every call on the log, host-buffer or device-resident, on the library's stream or the caller's
   // set by the device when an append read a decreasing offset pair (that leaf went in as the empty leaf); cg_merkle_log_join
   // reports it once and from then on the log refuses every call (failed)
-  uint32_t* d_err = nullptr;
+  DevBuf<uint32_t> d_err;
   bool failed = false;
-  ~cg_merkle_log() {
-    cudaFree(d_slots); cudaFree(d_tmp); cudaFree(d_leaves); cudaFree(d_new); cudaFree(d_a); cudaFree(d_b); cudaFree(d_spine); cudaFree(d_err);
-    for (uint32_t* p : d_lvl) cudaFree(p);
-    if (order.ev) cudaEventDestroy(order.ev);
-  }
+  ~cg_merkle_log() { if (order.ev) cudaEventDestroy(order.ev); }     // (the buffers release themselves)
 };
 
 namespace {
 // room in the level ping-pong for a fold of cnt > 1 nodes
 int log_fold_room(cg_merkle_log* L, uint64_t cnt) {
-  int rc = grow(&L->d_a, &L->cap_a, (size_t)(cnt + 1) / 2 * 8 + 8);
-  return rc ? rc : grow(&L->d_b, &L->cap_b, (size_t)(cnt + 3) / 4 * 8 + 8);
+  int rc = L->d_a.grow((size_t)(cnt + 1) / 2 * 8 + 8);
+  return rc ? rc : L->d_b.grow((size_t)(cnt + 3) / 4 * 8 + 8);
 }
 // MTH of `cnt` consecutive leaf digests starting at d_in (level-wise, unpaired node promoted) -> d_out (32 bytes)
 int log_range_root(cg_merkle_log* L, const uint32_t* d_in, uint64_t cnt, uint32_t* d_out, cudaStream_t st) {
@@ -1762,7 +1728,7 @@ int log_range_root(cg_merkle_log* L, const uint32_t* d_in, uint64_t cnt, uint32_
   if (cnt == 1) { CU(cudaMemcpyAsync(d_out, d_in, 32, cudaMemcpyDeviceToDevice, st)); return CG_OK; }
   if ((rc = log_fold_room(L, cnt))) return rc;
   const uint32_t* d_root;
-  count_launches(launch_merkle_fold(d_in, cnt, 64, L->d_a, L->d_b, st, &d_root));
+  count_launches(launch_merkle_fold(d_in, cnt, 64, L->d_a.get(), L->d_b.get(), st, &d_root));
   CU(cudaMemcpyAsync(d_out, d_root, 32, cudaMemcpyDeviceToDevice, st));
   return CG_OK;
 }
@@ -1777,22 +1743,22 @@ int log_root_device(cg_merkle_log* L, cudaStream_t st) {
   // fold the frontier from the smallest subtree upwards: r = slot[lowest]; r = node(slot[h], r) for every higher set bit
   const int lowest = __builtin_ctzll(L->n);
   ChainOperands ops{}; uint32_t nl = 0;
-  for (int h = lowest + 1; h < 64; h++) if ((L->n >> h) & 1ull) ops.left[nl++] = L->d_slots + 8 * h;
-  count_launches(launch_merkle_chain_keep(ops, nl, L->d_slots + 8 * lowest, L->d_tmp + 8 * 64, st));
+  for (int h = lowest + 1; h < 64; h++) if ((L->n >> h) & 1ull) ops.left[nl++] = L->d_slots.get() + 8 * h;
+  count_launches(launch_merkle_chain_keep(ops, nl, L->d_slots.get() + 8 * lowest, L->d_tmp.get() + 8 * 64, st));
   return CG_OK;
 }
 // node j of level h of a tree log (level 0: leaf digest j)
-uint32_t* log_node(cg_merkle_log* L, uint32_t h, uint64_t j) { return (h ? L->d_lvl[h] : L->d_leaves) + 8 * (size_t)j; }
+uint32_t* log_node(cg_merkle_log* L, uint32_t h, uint64_t j) { return L->d_lvl[h].get() + 8 * (size_t)j; }
 
 int log_new(cg_merkle_log** out, bool keep, bool tree) {
   if (int rc = require_ready()) return rc;
   if (!out) return fail(CG_ERR_INVALID_ARG, "null argument");
   std::unique_ptr<cg_merkle_log> L(new cg_merkle_log());
-  L->keep = keep; L->tree = tree;
-  CU(cudaMalloc((void**)&L->d_slots, 64 * 32)); CU(cudaMalloc((void**)&L->d_tmp, 65 * 32)); CU(cudaMalloc((void**)&L->d_err, 4));
-  CU(cudaMemset(L->d_slots, 0, 64 * 32)); CU(cudaMemset(L->d_err, 0, 4));
+  L->keep = keep; L->tree = tree; int rc;
+  if ((rc = L->d_slots.alloc(64 * 8)) || (rc = L->d_tmp.alloc(65 * 8)) || (rc = L->d_err.alloc(1))) return rc;
+  CU(cudaMemset(L->d_slots.get(), 0, 64 * 32)); CU(cudaMemset(L->d_err.get(), 0, 4));
   CU(cudaEventCreateWithFlags(&L->order.ev, cudaEventDisableTiming));
-  if (tree) CU(cudaMalloc((void**)&L->d_spine, 64 * 32));
+  if (tree && (rc = L->d_spine.alloc(64 * 8))) return rc;
   *out = L.release();
   return CG_OK;
 }
@@ -1815,12 +1781,13 @@ int cg_merkle_log_size(const cg_merkle_log* L, uint64_t* out_n) { if (!L || !out
 
 int cg_merkle_log_restore(cg_merkle_log** out, uint64_t n, const uint8_t* frontier32, uint32_t count) {
   if (!out || (count && !frontier32) || count != (uint32_t)__builtin_popcountll(n)) return fail(CG_ERR_INVALID_ARG, "frontier must hold one digest per set bit of n");
-  int rc = cg_merkle_log_create(out, 0);
+  cg_merkle_log* made = nullptr; int rc = cg_merkle_log_create(&made, 0);
   if (rc) return rc;
   std::lock_guard<std::mutex> lk(g_mu);
-  cg_merkle_log* L = *out; uint32_t k = 0;
-  for (int h = 63; h >= 0; h--) if ((n >> h) & 1ull) { CU(cudaMemcpy(L->d_slots + 8 * h, frontier32 + 32 * (size_t)k, 32, cudaMemcpyHostToDevice)); k++; }
+  std::unique_ptr<cg_merkle_log> L(made); uint32_t k = 0;  // (destroyed unless complete: *out is set on success only)
+  for (int h = 63; h >= 0; h--) if ((n >> h) & 1ull) { CU(cudaMemcpy(L->d_slots.get() + 8 * h, frontier32 + 32 * (size_t)k, 32, cudaMemcpyHostToDevice)); k++; }
   L->n = n;
+  *out = L.release();
   return CG_OK;
 }
 
@@ -1831,7 +1798,7 @@ int cg_merkle_log_frontier(cg_merkle_log* L, uint8_t* out_frontier32, uint32_t* 
   InOrder turn(&L->order, G.stream);
   if ((rc = turn.rc)) return rc;
   uint32_t k = 0;
-  for (int h = 63; h >= 0; h--) if ((L->n >> h) & 1ull) { if (out_frontier32) CU(cudaMemcpyAsync(out_frontier32 + 32 * (size_t)k, L->d_slots + 8 * h, 32, cudaMemcpyDeviceToHost, G.stream)); k++; }
+  for (int h = 63; h >= 0; h--) if ((L->n >> h) & 1ull) { if (out_frontier32) CU(cudaMemcpyAsync(out_frontier32 + 32 * (size_t)k, L->d_slots.get() + 8 * h, 32, cudaMemcpyDeviceToHost, G.stream)); k++; }
   CU(cudaStreamSynchronize(G.stream));
   *out_count = k;
   return CG_OK;
@@ -1840,28 +1807,23 @@ int cg_merkle_log_frontier(cg_merkle_log* L, uint8_t* out_frontier32, uint32_t* 
 namespace {
 // room for m more leaf digests; returns where they go
 int log_digest_room(cg_merkle_log* L, uint64_t m, cudaStream_t st, uint32_t** out) {
-  int rc;
-  if (L->keep) {
-    if (L->n + m > L->cap_leaves) {                         // grow the digest store (amortised doubling), keeping what is there
-      uint64_t cap = std::max<uint64_t>(L->n + m, L->cap_leaves * 2); uint32_t* nd = nullptr;
-      CU(cudaMalloc((void**)&nd, (size_t)cap * 32));
-      if (L->n) CU(cudaMemcpyAsync(nd, L->d_leaves, (size_t)L->n * 32, cudaMemcpyDeviceToDevice, st));
-      // a tree log's node levels follow: level h holds up to cap >> h nodes
-      uint32_t* nl[64] = {};
-      for (uint32_t h = 1; L->tree && h < 64 && (cap >> h); h++) {
-        if ((cap >> h) <= L->cap_lvl[h]) continue;
-        cudaError_t e = cudaMalloc((void**)&nl[h], (size_t)(cap >> h) * 32);
-        if (e != cudaSuccess) { cudaStreamSynchronize(st); cudaFree(nd); for (uint32_t* p : nl) cudaFree(p); return cuda_fail(e, "cudaMalloc"); }
-        if (L->n >> h) CU(cudaMemcpyAsync(nl[h], L->d_lvl[h], (size_t)(L->n >> h) * 32, cudaMemcpyDeviceToDevice, st));
-      }
-      CU(cudaStreamSynchronize(st)); cudaFree(L->d_leaves); L->d_leaves = nd; L->cap_leaves = cap;
-      for (uint32_t h = 1; h < 64; h++) if (nl[h]) { cudaFree(L->d_lvl[h]); L->d_lvl[h] = nl[h]; L->cap_lvl[h] = cap >> h; }
+  if (!L->keep) { if (int rc = L->d_new.grow((size_t)m * 8)) return rc; *out = L->d_new.get(); return CG_OK; }
+  const uint64_t room = L->d_lvl[0].cap() / 8;
+  if (L->n + m > room) {               // grow the digest store (amortised doubling), keeping what is there; a tree log's node
+    const uint64_t cap = std::max<uint64_t>(L->n + m, room * 2);          // levels follow (level h holds up to cap >> h nodes)
+    DevBuf<uint32_t> nl[64];
+    int rc = CG_OK; cudaError_t e = cudaSuccess;
+    for (uint32_t h = 0; !rc && e == cudaSuccess && h < (L->tree ? 64u : 1u) && (cap >> h); h++) {
+      if ((cap >> h) <= L->d_lvl[h].cap() / 8) continue;
+      if (!(rc = nl[h].alloc((size_t)(cap >> h) * 8)) && (L->n >> h)) e = cudaMemcpyAsync(nl[h].get(), L->d_lvl[h].get(), (size_t)(L->n >> h) * 32, cudaMemcpyDeviceToDevice, st);
     }
-    *out = L->d_leaves + (size_t)L->n * 8;
-  } else {
-    if ((rc = grow(&L->d_new, &L->cap_new, (size_t)m * 8))) return rc;
-    *out = L->d_new;
+    // the copies read the old buffers and write the new ones: they are done before any buffer is freed, on failure too
+    const cudaError_t s = cudaStreamSynchronize(st);
+    if (rc) return rc;
+    if (e != cudaSuccess || s != cudaSuccess) return cuda_fail(e != cudaSuccess ? e : s, e != cudaSuccess ? "cudaMemcpyAsync" : "cudaStreamSynchronize(st)");
+    for (uint32_t h = 0; h < 64; h++) if (nl[h].get()) L->d_lvl[h] = std::move(nl[h]);
   }
+  *out = L->d_lvl[0].get() + (size_t)L->n * 8;
   return CG_OK;
 }
 // m new leaf digests at d_dig: cut [n, n+m) into aligned perfect blocks (block size <= lowest set bit of its position),
@@ -1880,11 +1842,11 @@ int log_absorb(cg_merkle_log* L, const uint32_t* d_dig, uint64_t m, cudaStream_t
     if (L->tree) for (int l = 1; l <= h; l++) lv[l] = log_node(L, l, pos >> l);
     else if (s > 1 && (rc = log_fold_room(L, s))) return rc;
     const uint32_t* acc;                                    // the block's root (a block of one leaf: the leaf digest, no launch)
-    count_launches(launch_merkle_fold(d_dig + (size_t)(pos - L->n) * 8, s, 64, L->d_a, L->d_b, st, &acc, L->tree ? lv : nullptr));
+    count_launches(launch_merkle_fold(d_dig + (size_t)(pos - L->n) * 8, s, 64, L->d_a.get(), L->d_b.get(), st, &acc, L->tree ? lv : nullptr));
     ChainOperands ops{}; uint32_t nl = 0; int top = h;     // slots h, h+1, ... that are occupied merge into the new subtree
-    while ((pos >> top) & 1ull) { ops.left[nl] = L->d_slots + 8 * top; top++; ops.keep[nl] = L->tree ? log_node(L, top, pos >> top) : nullptr; nl++; }
-    if (nl) count_launches(launch_merkle_chain_keep(ops, nl, acc, L->d_slots + 8 * top, st));
-    else CU(cudaMemcpyAsync(L->d_slots + 8 * top, acc, 32, cudaMemcpyDeviceToDevice, st));
+    while ((pos >> top) & 1ull) { ops.left[nl] = L->d_slots.get() + 8 * top; top++; ops.keep[nl] = L->tree ? log_node(L, top, pos >> top) : nullptr; nl++; }
+    if (nl) count_launches(launch_merkle_chain_keep(ops, nl, acc, L->d_slots.get() + 8 * top, st));
+    else CU(cudaMemcpyAsync(L->d_slots.get() + 8 * top, acc, 32, cudaMemcpyDeviceToDevice, st));
     pos += s; rem -= s;
   }
   CU(cudaGetLastError());
@@ -1905,8 +1867,8 @@ int cg_merkle_log_reserve(cg_merkle_log* L, uint64_t n_leaves, uint64_t n_bytes)
   uint32_t* unused;
   if (n_leaves && (rc = log_digest_room(L, n_leaves, G.stream, &unused))) return rc;
   if (n_leaves > 1 && !L->tree && (rc = log_fold_room(L, n_leaves))) return rc;     // (a tree log folds into its store)
-  if (n_bytes && (rc = grow_bytes((size_t)n_bytes + 64))) return rc;
-  if (n_leaves && (rc = grow(&G.d_off64, &G.cap_off64, (size_t)n_leaves + 1))) return rc;
+  if (n_bytes && (rc = G.d_bytes.grow((size_t)n_bytes + 64))) return rc;
+  if (n_leaves && (rc = G.d_off64.grow((size_t)n_leaves + 1))) return rc;
   return CG_OK;
 }
 
@@ -1921,13 +1883,13 @@ int cg_merkle_log_append(cg_merkle_log* L, const uint8_t* bytes, const uint64_t*
   InOrder turn(&L->order, st);
   if ((rc = turn.rc)) return rc;
   const size_t first = offsets[0], total = offsets[m];
-  if ((rc = grow_bytes(total + 64))) return rc;
-  if ((rc = grow(&G.d_off64, &G.cap_off64, (size_t)m + 1))) return rc;
+  if ((rc = G.d_bytes.grow(total + 64))) return rc;
+  if ((rc = G.d_off64.grow((size_t)m + 1))) return rc;
   if ((rc = ensure_copy_streams())) return rc;
   uint32_t* d_dig;                                          // where this batch's leaf digests go
   if ((rc = log_digest_room(L, m, st, &d_dig))) return rc;
   CU(cudaStreamSynchronize(st));                            // (whatever still read the staging buffer is done)
-  CU(cudaMemcpyAsync(G.d_off64, offsets, ((size_t)m + 1) * 8, cudaMemcpyHostToDevice, G.s_h2d));
+  CU(cudaMemcpyAsync(G.d_off64.get(), offsets, ((size_t)m + 1) * 8, cudaMemcpyHostToDevice, G.s_h2d));
   // the leaf bytes go over in pieces on the copy stream; the leaf kernel of piece c runs while piece c + 1 is still in flight
   const int C = (total - first) > ((size_t)4 << 20) ? Ctx::kChunks : 1;
   const uint64_t per = (m + C - 1) / C;
@@ -1935,10 +1897,10 @@ int cg_merkle_log_append(cg_merkle_log* L, const uint8_t* bytes, const uint64_t*
     const uint64_t m0 = std::min<uint64_t>((uint64_t)c * per, m), m1 = std::min<uint64_t>((uint64_t)(c + 1) * per, m);
     if (m1 <= m0) break;
     const size_t b0 = offsets[m0], b1 = offsets[m1];
-    if (b1 > b0) CU(cudaMemcpyAsync(G.d_bytes + b0, bytes + b0, b1 - b0, cudaMemcpyHostToDevice, G.s_h2d));
+    if (b1 > b0) CU(cudaMemcpyAsync(G.d_bytes.get() + b0, bytes + b0, b1 - b0, cudaMemcpyHostToDevice, G.s_h2d));
     CU(cudaEventRecord(G.e_h2d[c], G.s_h2d));
     CU(cudaStreamWaitEvent(st, G.e_h2d[c], 0));
-    int k = launch_merkle_leaves_var(G.d_bytes, G.d_off64 + m0, m1 - m0, d_dig + (size_t)m0 * 8, st);
+    int k = launch_merkle_leaves_var(G.d_bytes.get(), G.d_off64.get() + m0, m1 - m0, d_dig + (size_t)m0 * 8, st);
     count_launches(k);
   }
   G.stats.merkle_leaves += m;
@@ -1957,22 +1919,22 @@ int cg_merkle_log_append_jsonl(cg_merkle_log* L, const uint8_t* bytes, uint64_t 
   InOrder turn(&L->order, st);
   if ((rc = turn.rc)) return rc;
   const uint32_t n_pieces = (uint32_t)((len + 4095) / 4096);
-  if ((rc = grow_bytes((size_t)len + 64))) return rc;
-  if ((rc = grow(&G.d_off32, &G.cap_off32, (size_t)n_pieces + 4))) return rc;          // newline counts per 4 KB piece
-  if ((rc = grow(&G.d_off64, &G.cap_off64, 2))) return rc;
-  CU(cudaMemcpyAsync(G.d_bytes, bytes, len, cudaMemcpyHostToDevice, st));
-  uint64_t* d_total = G.d_off64;                           // (re-grown below once the line count is known)
-  int k = launch_newline_split(G.d_bytes, len, G.d_off32, d_total, st);
+  if ((rc = G.d_bytes.grow((size_t)len + 64))) return rc;
+  if ((rc = G.d_off32.grow((size_t)n_pieces + 4))) return rc;          // newline counts per 4 KB piece
+  if ((rc = G.d_off64.grow(2))) return rc;
+  CU(cudaMemcpyAsync(G.d_bytes.get(), bytes, len, cudaMemcpyHostToDevice, st));
+  uint64_t* d_total = G.d_off64.get();                           // (re-grown below once the line count is known)
+  int k = launch_newline_split(G.d_bytes.get(), len, G.d_off32.get(), d_total, st);
   uint64_t n_lines = 0;
   CU(cudaMemcpyAsync(&n_lines, d_total, 8, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   if (!n_lines) return CG_OK;
   if (L->n + n_lines < L->n) return fail(CG_ERR_TOO_LARGE, "log size overflows 64 bits");
-  if ((rc = grow(&G.d_off64, &G.cap_off64, (size_t)n_lines + 1))) return rc;
-  k += launch_newline_starts(G.d_bytes, len, G.d_off32, G.d_off64, n_lines, st);
+  if ((rc = G.d_off64.grow((size_t)n_lines + 1))) return rc;
+  k += launch_newline_starts(G.d_bytes.get(), len, G.d_off32.get(), G.d_off64.get(), n_lines, st);
   uint32_t* d_dig;
   if ((rc = log_digest_room(L, n_lines, st, &d_dig))) return rc;
-  k += launch_merkle_leaves_var(G.d_bytes, G.d_off64, n_lines, d_dig, st, /*trim_newline=*/true);
+  k += launch_merkle_leaves_var(G.d_bytes.get(), G.d_off64.get(), n_lines, d_dig, st, /*trim_newline=*/true);
   count_launches(k); G.stats.merkle_leaves += n_lines;
   if (out_lines) *out_lines = n_lines;
   return log_absorb(L, d_dig, n_lines, st);
@@ -1987,7 +1949,7 @@ int cg_merkle_log_root(cg_merkle_log* L, uint8_t out_root[32]) {
     if ((rc = turn.rc)) return rc;
     if (L->n) {
       if ((rc = log_root_device(L, G.stream))) return rc;
-      CU(cudaMemcpyAsync(out_root, L->d_tmp + 8 * 64, 32, cudaMemcpyDeviceToHost, G.stream));
+      CU(cudaMemcpyAsync(out_root, L->d_tmp.get() + 8 * 64, 32, cudaMemcpyDeviceToHost, G.stream));
       CU(cudaStreamSynchronize(G.stream));
       return CG_OK;
     }
@@ -2002,13 +1964,13 @@ namespace {
 int log_spine(cg_merkle_log* L, uint64_t s, cudaStream_t st) {
   const int lowest = __builtin_ctzll(s);
   ChainOperands ops{}; uint32_t nl = 0;
-  for (int h = lowest + 1; h < 64; h++) if ((s >> h) & 1ull) { ops.left[nl] = log_node(L, h, (s >> h) - 1); ops.keep[nl] = L->d_spine + 8 * h; nl++; }
+  for (int h = lowest + 1; h < 64; h++) if ((s >> h) & 1ull) { ops.left[nl] = log_node(L, h, (s >> h) - 1); ops.keep[nl] = L->d_spine.get() + 8 * h; nl++; }
   count_launches(launch_merkle_chain_keep(ops, nl, log_node(L, lowest, (s >> lowest) - 1), nullptr, st));
   return CG_OK;
 }
 NodeStore log_store(cg_merkle_log* L) {
   NodeStore ns{};
-  for (uint32_t h = 0; h < 64; h++) ns.lvl[h] = h ? L->d_lvl[h] : L->d_leaves;
+  for (uint32_t h = 0; h < 64; h++) ns.lvl[h] = L->d_lvl[h].get();
   return ns;
 }
 // The leaf ranges [a, b) of PATH(i, D[0:size]) (RFC 6962 2.1.1; first == 0), or of PROOF(first, D[0:size]) (2.1.2; i unused),
@@ -2037,12 +1999,12 @@ int log_gather(cg_merkle_log* L, const uint64_t* h_idx, uint32_t m, uint64_t siz
   InOrder turn(&G.dig_order, st);
   if ((rc = turn.rc)) return rc;
   const size_t path_words = (size_t)m * stride * 8, lens_words = ((size_t)m + 7) / 8 * 8;
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], path_words + lens_words))) return rc;
-  if (h_idx && (rc = grow(&G.d_off64, &G.cap_off64, (size_t)m))) return rc;
-  uint32_t* d_paths = G.d_dig[0]; uint32_t* d_lens = d_paths + path_words;
-  if (h_idx) CU(cudaMemcpyAsync(G.d_off64, h_idx, (size_t)m * 8, cudaMemcpyHostToDevice, st));
+  if ((rc = G.d_dig[0].grow(path_words + lens_words))) return rc;
+  if (h_idx && (rc = G.d_off64.grow((size_t)m))) return rc;
+  uint32_t* d_paths = G.d_dig[0].get(); uint32_t* d_lens = d_paths + path_words;
+  if (h_idx) CU(cudaMemcpyAsync(G.d_off64.get(), h_idx, (size_t)m * 8, cudaMemcpyHostToDevice, st));
   if ((rc = log_spine(L, size, st))) return rc;
-  count_launches(launch_merkle_gather(log_store(L), L->d_spine, size, h_idx ? G.d_off64 : nullptr, first, m, stride, d_paths, d_lens, G.sm_count, st));
+  count_launches(launch_merkle_gather(log_store(L), L->d_spine.get(), size, h_idx ? G.d_off64.get() : nullptr, first, m, stride, d_paths, d_lens, G.sm_count, st));
   CU(cudaGetLastError());
   if (path_words) CU(cudaMemcpyAsync(out_paths32, d_paths, path_words * 4, cudaMemcpyDeviceToHost, st));
   if (out_lens) CU(cudaMemcpyAsync(out_lens, d_lens, (size_t)m * 4, cudaMemcpyDeviceToHost, st));
@@ -2055,8 +2017,8 @@ int log_proof(cg_merkle_log* L, const std::vector<std::pair<uint64_t, uint64_t>>
   if (L->tree) return ranges.empty() ? CG_OK : log_gather(L, h_idx, 1, L->n, first, out_path32, (uint32_t)ranges.size(), nullptr);
   cudaStream_t st = G.stream; int rc;
   for (size_t i = 0; i < ranges.size(); i++)
-    if ((rc = log_range_root(L, L->d_leaves + (size_t)ranges[i].first * 8, ranges[i].second - ranges[i].first, L->d_tmp + 8 * i, st))) return rc;
-  if (!ranges.empty()) CU(cudaMemcpyAsync(out_path32, L->d_tmp, ranges.size() * 32, cudaMemcpyDeviceToHost, st));
+    if ((rc = log_range_root(L, L->d_lvl[0].get() + (size_t)ranges[i].first * 8, ranges[i].second - ranges[i].first, L->d_tmp.get() + 8 * i, st))) return rc;
+  if (!ranges.empty()) CU(cudaMemcpyAsync(out_path32, L->d_tmp.get(), ranges.size() * 32, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
 }
@@ -2132,8 +2094,8 @@ int cg_merkle_verify_consistency(uint64_t first_size, uint64_t second_size, cons
   int rc; cudaStream_t st = G.stream;
   InOrder turn(&G.dig_order, st);
   if ((rc = turn.rc)) return rc;
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)(path_len + 4) * 8))) return rc;
-  uint32_t* d_r1 = G.d_dig[0]; uint32_t* d_r2 = d_r1 + 8; uint32_t* d_ok = d_r2 + 8; uint32_t* d_path = d_ok + 8;
+  if ((rc = G.d_dig[0].grow((size_t)(path_len + 4) * 8))) return rc;
+  uint32_t* d_r1 = G.d_dig[0].get(); uint32_t* d_r2 = d_r1 + 8; uint32_t* d_ok = d_r2 + 8; uint32_t* d_path = d_ok + 8;
   CU(cudaMemcpyAsync(d_r1, root_first, 32, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(d_r2, root_second, 32, cudaMemcpyHostToDevice, st));
   if (path_len) CU(cudaMemcpyAsync(d_path, path32, (size_t)path_len * 32, cudaMemcpyHostToDevice, st));
@@ -2166,20 +2128,20 @@ int verify_proofs(const uint8_t* leaf_bytes, const uint64_t* leaf_offsets, const
   // d_dig[0]: leaf digests | root ; d_dig[1]: paths | indices | lengths | verdicts (every region a multiple of 32 bytes)
   const size_t leaf_words = (size_t)m * 8, path_words = (size_t)m * path_stride * 8, idx_words = ((size_t)m * 2 + 7) / 8 * 8,
                len_words = ((size_t)m + 7) / 8 * 8, ok_words = ((size_t)m + 31) / 32 * 8;
-  if ((rc = grow_bytes(total + 64))) return rc;
-  if ((rc = grow(&G.d_off64, &G.cap_off64, (size_t)m + 1))) return rc;
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], leaf_words + 8))) return rc;
-  if ((rc = grow(&G.d_dig[1], &G.cap_dig[1], path_words + idx_words + len_words + ok_words))) return rc;
-  uint32_t* d_leaf = G.d_dig[0]; uint32_t* d_root = d_leaf + leaf_words;
-  uint32_t* d_paths = G.d_dig[1]; uint64_t* d_idx = reinterpret_cast<uint64_t*>(d_paths + path_words);
+  if ((rc = G.d_bytes.grow(total + 64))) return rc;
+  if ((rc = G.d_off64.grow((size_t)m + 1))) return rc;
+  if ((rc = G.d_dig[0].grow(leaf_words + 8))) return rc;
+  if ((rc = G.d_dig[1].grow(path_words + idx_words + len_words + ok_words))) return rc;
+  uint32_t* d_leaf = G.d_dig[0].get(); uint32_t* d_root = d_leaf + leaf_words;
+  uint32_t* d_paths = G.d_dig[1].get(); uint64_t* d_idx = reinterpret_cast<uint64_t*>(d_paths + path_words);
   uint32_t* d_lens = d_paths + path_words + idx_words; uint8_t* d_ok = reinterpret_cast<uint8_t*>(d_lens + len_words);
-  if (total) CU(cudaMemcpyAsync(G.d_bytes, leaf_bytes, total, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(G.d_off64, leaf_offsets, ((size_t)m + 1) * 8, cudaMemcpyHostToDevice, st));
+  if (total) CU(cudaMemcpyAsync(G.d_bytes.get(), leaf_bytes, total, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(G.d_off64.get(), leaf_offsets, ((size_t)m + 1) * 8, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(d_root, root, 32, cudaMemcpyHostToDevice, st));
   if (path_words) CU(cudaMemcpyAsync(d_paths, paths32, path_words * 4, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(d_idx, indices, (size_t)m * 8, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(d_lens, path_lens, (size_t)m * 4, cudaMemcpyHostToDevice, st));
-  int k = launch_merkle_leaves_var(G.d_bytes, G.d_off64, m, d_leaf, st);
+  int k = launch_merkle_leaves_var(G.d_bytes.get(), G.d_off64.get(), m, d_leaf, st);
   k += launch_merkle_verify_batch(d_leaf, d_idx, m, tree_size, d_paths, path_stride, d_lens, d_root, d_ok, G.sm_count, st);
   count_launches(k);
   CU(cudaGetLastError());
@@ -2227,7 +2189,7 @@ int log_append_device(cg_merkle_log* L, const uint8_t* d_bytes, const uint64_t* 
   if ((rc = turn.rc)) return rc;
   uint32_t* d_dig;
   if ((rc = log_digest_room(L, m, st, &d_dig))) return rc;
-  count_launches(d_off ? launch_merkle_leaves_guarded(d_bytes, d_off, m, d_dig, L->d_err, st) : launch_merkle_leaves_fixed(d_bytes, leaf_len, m, d_dig, st));
+  count_launches(d_off ? launch_merkle_leaves_guarded(d_bytes, d_off, m, d_dig, L->d_err.get(), st) : launch_merkle_leaves_fixed(d_bytes, leaf_len, m, d_dig, st));
   G.stats.merkle_leaves += m;
   return log_absorb(L, d_dig, m, st, /*wait=*/false);
 }
@@ -2265,10 +2227,10 @@ int cg_merkle_log_root_device(cg_merkle_log* L, void* d_out_root32, void* stream
   } else {
     // SHA-256("") by the same kernel as the host twin's, but from the log's own scratch, never the library's staging (whose
     // other users take no turn before they write it): 16 zero bytes of d_tmp are both the offsets pair and the word it loads
-    CU(cudaMemsetAsync(L->d_tmp, 0, 32, st));
-    count_launches(launch_sha256_batch((const uint8_t*)L->d_tmp, (const uint64_t*)L->d_tmp, 1, (uint8_t*)(L->d_tmp + 8 * 64), st));
+    CU(cudaMemsetAsync(L->d_tmp.get(), 0, 32, st));
+    count_launches(launch_sha256_batch((const uint8_t*)L->d_tmp.get(), (const uint64_t*)L->d_tmp.get(), 1, (uint8_t*)(L->d_tmp.get() + 8 * 64), st));
   }
-  CU(cudaMemcpyAsync(d_out_root32, L->d_tmp + 8 * 64, 32, cudaMemcpyDeviceToDevice, st));
+  CU(cudaMemcpyAsync(d_out_root32, L->d_tmp.get() + 8 * 64, 32, cudaMemcpyDeviceToDevice, st));
   CU(cudaGetLastError());
   return CG_OK;
 }
@@ -2289,7 +2251,7 @@ int cg_merkle_log_proofs_device(cg_merkle_log* L, const void* d_indices, uint32_
   InOrder turn(&L->order, st), dig(&G.dig_order, st);
   if ((rc = turn.rc) || (rc = dig.rc)) return rc;
   if ((rc = log_spine(L, tree_size, st))) return rc;
-  count_launches(launch_merkle_gather(log_store(L), L->d_spine, tree_size, (const uint64_t*)d_indices, 0, m, path_stride, (uint32_t*)d_out_paths32,
+  count_launches(launch_merkle_gather(log_store(L), L->d_spine.get(), tree_size, (const uint64_t*)d_indices, 0, m, path_stride, (uint32_t*)d_out_paths32,
                                       (uint32_t*)d_out_lens, G.sm_count, st, /*checked=*/true));
   CU(cudaGetLastError());
   return CG_OK;
@@ -2311,7 +2273,7 @@ int cg_merkle_log_consistency_between_device(cg_merkle_log* L, uint64_t first_si
   if ((rc = turn.rc) || (rc = dig.rc)) return rc;
   if (!len) { CU(cudaMemsetAsync(d_out_len, 0, 4, st)); return CG_OK; }
   if ((rc = log_spine(L, second_size, st))) return rc;
-  count_launches(launch_merkle_gather(log_store(L), L->d_spine, second_size, nullptr, first_size, 1, len, (uint32_t*)d_out_path32, (uint32_t*)d_out_len,
+  count_launches(launch_merkle_gather(log_store(L), L->d_spine.get(), second_size, nullptr, first_size, 1, len, (uint32_t*)d_out_path32, (uint32_t*)d_out_len,
                                       G.sm_count, st));
   CU(cudaGetLastError());
   return CG_OK;
@@ -2332,8 +2294,8 @@ int cg_merkle_verify_proofs_device(const void* d_leaf_bytes, const void* d_leaf_
   InOrder turn(&G.dig_order, st);
   if ((rc = turn.rc)) return rc;
   // d_dig[0]: leaf digests | root (the caller's root copied, so that it may have any alignment)
-  if ((rc = grow(&G.d_dig[0], &G.cap_dig[0], (size_t)m * 8 + 8))) return rc;
-  uint32_t* d_leaf = G.d_dig[0]; uint32_t* d_root = d_leaf + (size_t)m * 8;
+  if ((rc = G.d_dig[0].grow((size_t)m * 8 + 8))) return rc;
+  uint32_t* d_leaf = G.d_dig[0].get(); uint32_t* d_root = d_leaf + (size_t)m * 8;
   CU(cudaMemcpyAsync(d_root, d_root32, 32, cudaMemcpyDeviceToDevice, st));
   const uint64_t* d_off = (const uint64_t*)d_leaf_offsets;
   int k = launch_merkle_leaves_guarded((const uint8_t*)d_leaf_bytes, d_off, m, d_leaf, nullptr, st);
@@ -2350,7 +2312,7 @@ int cg_merkle_log_join(cg_merkle_log* L, void* stream) {
   CU(cudaStreamSynchronize(caller_stream(stream)));
   CU(cudaEventSynchronize(L->order.ev));                    // (every call issued on the log has run: each one ran behind the one before)
   uint32_t err = 0;
-  CU(cudaMemcpyAsync(&err, L->d_err, 4, cudaMemcpyDeviceToHost, G.stream));
+  CU(cudaMemcpyAsync(&err, L->d_err.get(), 4, cudaMemcpyDeviceToHost, G.stream));
   CU(cudaStreamSynchronize(G.stream));
   if (err) {
     L->failed = true;
@@ -2411,7 +2373,7 @@ int cg_comm_init(int rank, int world, const cg_nccl_id* id) {
 void cg_comm_destroy(void) {
   std::lock_guard<std::mutex> lk(g_mu);
   if (g_nccl.comm && g_nccl.CommDestroy) { if (G.ready) cudaStreamSynchronize(G.stream); g_nccl.CommDestroy(g_nccl.comm); }
-  free_shard_roots();
+  G.d_roots.reset();
   g_nccl.comm = nullptr; g_nccl.world = 1; g_nccl.rank = 0;
 }
 
@@ -2433,23 +2395,23 @@ int cg_merkle_root_sharded_device(const void* d_bytes, uint64_t leaf_len, uint64
   for (int r = 0; r < world; r++) { uint64_t a, b; cg_shard_range(n_total, r, world, 1ull << block_log2, &a, &b); nblk[(size_t)r] = (b - a + (1ull << block_log2) - 1) >> block_log2; max_blocks = std::max(max_blocks, nblk[(size_t)r]); total_blocks += nblk[(size_t)r]; }
   if (max_blocks == 0) return empty_root(out_root);
   int rc;
-  if ((rc = grow(&g_nccl.d_roots, &g_nccl.cap_roots, (size_t)world * max_blocks * 8))) return rc;
-  uint32_t* const all = g_nccl.d_roots; uint32_t* const mine = all + (size_t)rank * max_blocks * 8;   // (an in-place all-gather)
+  if ((rc = G.d_roots.grow((size_t)world * max_blocks * 8))) return rc;
+  uint32_t* const all = G.d_roots.get(); uint32_t* const mine = all + (size_t)rank * max_blocks * 8;   // (an in-place all-gather)
   CU(cudaMemsetAsync(mine, 0, max_blocks * 32, st));
   if (n_local && (rc = block_roots(d_bytes, leaf_len, n_local, block_log2, mine, st))) return rc;
   if (world > 1) {
     lk.unlock(); const int r = g_nccl.AllGather(mine, all, max_blocks * 32, /*ncclChar*/ 0, comm, st); lk.lock();
     if (r) return nccl_fail(r, "ncclAllGather");
     // (a cg_shutdown, cg_comm_destroy or other sharded call during the gather is misuse, but must not make the fold read freed memory)
-    if (!G.ready || g_nccl.d_roots != all) return fail(CG_ERR_NOT_INITIALIZED, "the library or the communicator's buffer changed during the all-gather");
+    if (!G.ready || G.d_roots.get() != all) return fail(CG_ERR_NOT_INITIALIZED, "the library or the communicator's buffer changed during the all-gather");
   }
   const uint32_t* d_root;                                   // the fold's input: the gathered roots without the empty slots
   InOrder turn(&G.dig_order, st);                           // (block_roots took its own turn: the lock was let go since)
   if ((rc = turn.rc)) return rc;
   if ((rc = size_dig(total_blocks))) return rc;
-  uint32_t* d = G.d_dig[0];
+  uint32_t* d = G.d_dig[0].get();
   for (int r = 0; r < world; r++) if (nblk[(size_t)r]) { CU(cudaMemcpyAsync(d, all + (size_t)r * max_blocks * 8, nblk[(size_t)r] * 32, cudaMemcpyDeviceToDevice, st)); d += nblk[(size_t)r] * 8; }
-  if ((rc = fold_dig(G.d_dig[0], total_blocks, 64, st, &d_root))) return rc;
+  if ((rc = fold_dig(G.d_dig[0].get(), total_blocks, 64, st, &d_root))) return rc;
   CU(cudaMemcpyAsync(out_root, d_root, 32, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return CG_OK;
